@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Headline benchmark (BASELINE.json): tokens/sec, Llama-1B DiLoCo H=100 on 1/2/4/8 B200; outer all-reduce GB/s.
+"""Headline benchmark (BASELINE.json): tokens/sec, Llama-1B DiLoCo H=100 on 1/2/4/8 H100; outer all-reduce GB/s.
 
     python bench.py --gpus 1 --steps 10 --warmup 3
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 8 --master-addr 127.0.0.1 \
@@ -7,8 +7,10 @@
 
 Mesh: N=1 → 1 worker × 1 GPU;  N>=2 → (N/2) DiLoCo workers × 2-GPU FSDP (config 2 of BASELINE.json).
 Weak scaling: every GPU processes the same number of tokens per step for every N.
-Other BASELINE configs through the same harness:  ``--model 7B --fsdp 8`` (config 4, FSDP only, no outer step),
-``--model 7B --workers 2 --fsdp 4 --H 500`` (config 3), ``--reshard 0|1`` picks replicated parameters vs ZeRO-3.
+Other BASELINE configs through the same harness:  ``--model 7B --fsdp 8 --H 0`` (config 4, FSDP only, no outer step; 7B runs
+micro-batch 1 × seq 4096 so that it fits 80 GB), ``--reshard 0|1`` picks replicated parameters vs ZeRO-3. Config 3 (7B DiLoCo,
+2 workers × 4-GPU FSDP) does not fit an 80 GB H100: with 4-way sharding the replicated fp32 main_grad, the 1/4 optimizer shards and
+the DiLoCo θ₀ + momentum alone take 76 GB per GPU before any activation (``python -m prime_b200.utils.memory_plan``).
 
 A "step" is one full inner optimizer step (ACCUM micro-batches fwd+bwd, gradient reduce-scatter, clip, AdamW, parameter
 all-gather).  The outer DiLoCo step (int8 pseudo-gradient all-reduce ⊕ Nesterov) runs every H inner steps *and* is forced at
@@ -21,6 +23,11 @@ host→device input copies:
 Then, in the same invocation on the same box, the stock-PyTorch arm B0 (``baseline/torch_b0.py``: FSDP2 + NCCL + cuBLAS +
 SDPA + fused AdamW, same config, same protocol) → ``b0`` and the ratio ``vs_b0``.  ``--impl torch_b0`` runs only that arm;
 ``--impl reference`` reports why the mounted reference cannot run the metric.
+
+``--dump-outputs DIR`` writes, after the timed regions, what the last timed step computed for its caller: the step's loss and
+gradient norm, and a fixed seeded sample of every parameter after the update, as ``DIR/<name>.npy`` (float32 / float64, < 64 MB).
+The synthetic inputs and the initial weights are seeded, so two builds run with the same arguments can be compared output by output.
+It needs replicated parameters (refused under ZeRO-3, where the model's parameters are views of one shared gather scratch).
 """
 
 from __future__ import annotations
@@ -56,6 +63,26 @@ def reference_arm() -> None:
 
 from prime_b200.utils.clocks import ClockSampler, NvlinkCounters  # noqa: E402
 
+DUMP_SAMPLE = 32768  # elements per parameter tensor written by --dump-outputs (seeded positions; whole tensor if smaller)
+
+
+def dump_outputs(out_dir: Path, result, model) -> None:
+    import numpy as np
+    import torch
+
+    out_dir.mkdir(parents=True, exist_ok=True)
+    np.save(out_dir / "loss.npy", np.array([float(result.loss.item())], dtype=np.float64))
+    if result.grad_norm is not None:
+        np.save(out_dir / "grad_norm.npy", np.array([float(torch.as_tensor(result.grad_norm).item())], dtype=np.float64))
+    for i, (name, p) in enumerate(model.named_parameters()):
+        flat = p.detach().reshape(-1)
+        if flat.numel() > DUMP_SAMPLE:
+            gen = torch.Generator().manual_seed(i)
+            idx = torch.randint(0, flat.numel(), (DUMP_SAMPLE,), generator=gen).to(flat.device)
+            flat = flat[idx]
+        np.save(out_dir / f"param.{name}.npy", flat.float().cpu().numpy())
+
+
 MODEL_DESC = {"1B": "Llama-1B (dim 2048, 18 layers, 16 heads, vocab 32000)", "7B": "Llama-7B (dim 4096, 32 layers, 32 heads, vocab 32000)",
               "150M": "Llama-150M (dim 1024, 12 layers, 16 heads, vocab 32000)"}  # fmt: skip
 
@@ -82,6 +109,7 @@ def main() -> None:
     ap.add_argument("--no-b0", action="store_true", help="skip the stock-PyTorch comparison arm")
     ap.add_argument("--b0-compile", action="store_true", help="B0 with torch.compile on every block")
     ap.add_argument("--trace", action="store_true", help="per-rank device timeline of the step phases (stderr + JSON key step_trace)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="write the last timed step's outputs as DIR/<name>.npy (rank 0)")
     args = ap.parse_args()
 
     if args.impl == "reference":
@@ -97,7 +125,7 @@ def main() -> None:
     warmup = max(3, args.warmup)
     K = max(1, args.steps)
     seq = args.seq or (4096 if args.model == "7B" else SEQ)
-    micro_bs = args.micro_bs or (4 if args.model == "7B" else MICRO_BS)
+    micro_bs = args.micro_bs or (1 if args.model == "7B" else MICRO_BS)  # 7B: micro-batch 4 × 4096 needs ≈ 119 GB per GPU at F = 8
     accum = args.accum or ACCUM
 
     fsdp = args.fsdp or (1 if world == 1 else 2)
@@ -150,6 +178,10 @@ def main() -> None:
         tree["diloco"] = {"inner_steps": args.H, "compression": args.compression, "outer_lr": 0.7}
     cfg = Config.model_validate(tree)
     trainer = Trainer(cfg)
+    if args.dump_outputs and trainer.engine.shard_params:
+        # under ZeRO-3 every model parameter is a view into one shared gather scratch (the embedding a zero placeholder): the
+        # parameters a dump would read are not the trained weights
+        raise SystemExit("--dump-outputs needs replicated parameters: add --reshard 0 (ZeRO-3 keeps only shards of the weights)")
     dev = trainer.device
     rank = trainer.mesh.world.rank
     if args.trace and trainer.engine.backend == "fused":
@@ -163,6 +195,7 @@ def main() -> None:
         torch.cuda.synchronize()
 
     losses: list[float] = []
+    last_step: dict = {}
 
     def run_region(n_steps: int, read_loss: bool) -> tuple[float, float, int]:
         """Returns (device ms, host s, launches) for n_steps inner steps incl. >= 1 outer step."""
@@ -175,6 +208,7 @@ def main() -> None:
         last = None
         for i in range(n_steps):
             r = trainer.inner_step()
+            last_step["result"] = r
             did_outer |= r.did_outer
             if i == n_steps - 1 and not did_outer and trainer.outer is not None:
                 trainer.outer.step()
@@ -221,6 +255,8 @@ def main() -> None:
     trace = trainer.engine.trace.summary() if trainer.engine.trace is not None else None
     trainer.engine.trace = None
     e2e_ms, e2e_host_s, _ = run_region(K, read_loss=True)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(Path(args.dump_outputs), last_step["result"], trainer.model)
     clocks = sampler.finish() if rank == 0 else {}
     trainer.check_health()
     memory = None
@@ -316,7 +352,7 @@ def main() -> None:
                 "comm": "fused P2P kernels" if not args.no_fused_comm else "NCCL collectives",
                 "params": shard_mode,
                 "cuda_graphs": bool(args.graphs),
-                "l2": "working set (params+activations, >20 GB/step) far larger than the 126 MB L2; no flush needed",
+                "l2": "working set (params+activations, >20 GB/step) far larger than the 50 MB L2; no flush needed",
             },
             "clocks": clocks,
             "e2e": {

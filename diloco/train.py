@@ -1,4 +1,4 @@
-"""``python -m diloco.train @configs/1B/b200.toml [--section.key value ...]`` → :func:`prime_b200.train.main`."""
+"""``python -m diloco.train @configs/1B/h100.toml [--section.key value ...]`` → :func:`prime_b200.train.main`."""
 
 import sys
 

@@ -1,7 +1,7 @@
 #!/bin/bash
 # Continue training a Hugging Face Llama checkpoint on your own corpus, then hand the result back to transformers.
 #   HF=/models/llama-1b TOK=/models/llama-1b CORPUS="corpus/*.jsonl" examples/finetune_from_hf.sh
-# Runs on the CPU with the debug model when HF is unset (a random donor is exported first), on a B200 with the real one.
+# Runs on the CPU with the debug model when HF is unset (a random donor is exported first), on an H100 with the real one.
 set -euo pipefail
 cd "$(dirname "$0")/.."
 OUT="${OUT:-/tmp/prime_b200/finetune}"

@@ -1,4 +1,4 @@
-"""Block-scaled fp8 (MXFP8) linear layer: quantise → tcgen05 block-scaled GEMM, against the bf16 GEMM. Runs on one B200; on CPU it
+"""Block-scaled fp8 (MXFP8) linear layer: quantise → block-scaled fp8 GEMM, against the bf16 GEMM. Runs on one H100; on CPU it
 falls back to the torch reference of the same format (prime_b200/ops/reference.py), which is also its specification.
 
     python examples/mxfp8_linear.py

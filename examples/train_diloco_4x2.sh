@@ -1,5 +1,5 @@
 #!/bin/bash
-# BASELINE config 2: 4 DiLoCo workers × 2-GPU FSDP on one 8×B200 NVSwitch box, fused P2P reduce/AdamW/all-gather kernels.
+# BASELINE config 2: 4 DiLoCo workers × 2-GPU FSDP on one 8×H100 NVSwitch box, fused P2P reduce/AdamW/all-gather kernels.
 set -euo pipefail
 cd "$(dirname "$0")/.."
 python -c "import __graft_entry__ as g; g.build()"

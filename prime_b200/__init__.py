@@ -1,9 +1,9 @@
-"""prime_b200 — a Blackwell (B200, sm_100a)-native DiLoCo / local-SGD training engine plus the
+"""prime_b200 — an H100 (Hopper, sm_90a)-native DiLoCo / local-SGD training engine plus the
 platform CLI & SDK surface of PrimeIntellect-ai/prime, rebuilt from scratch.
 
 Layout
 ------
-``prime_b200.ops``       hand-written sm_100a kernels (tcgen05/TMEM/TMA GEMM, fused norm/rope/
+``prime_b200.ops``       hand-written sm_90a kernels (wgmma/TMA GEMM, flash attention, fused norm/rope/
                          swiglu/loss, fused collective+optimizer kernels) and their torch oracles
 ``prime_b200.models``    Llama family built on those ops
 ``prime_b200.parallel``  two-level mesh (DiLoCo workers × FSDP shards), symmetric NVLink heap,

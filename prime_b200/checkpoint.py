@@ -8,7 +8,7 @@ Layout::
     <ckpt.path>/latest                  ← text file naming the newest complete step (written after the rename)
 
 Write path (``save``): the shard (master + m + v + θ₀ + momentum = 20 B/param/F) is first cloned on the device at HBM
-speed (≈7 ms for a whole 1B model; 180 GB parts have the room), so training resumes immediately; the clone drains to
+speed (≈7 ms for a whole 1B model; the device has the room), so training resumes immediately; the clone drains to
 reusable pinned host buffers on a side stream (PCIe 5, ≈0.4 s for 22 GB, overlapped with the next steps), a writer thread
 streams the pinned buffers to disk and fsyncs, then ranks meet on a barrier and rank 0 publishes by rename.
 

@@ -114,11 +114,13 @@ def reference_public_names(packages_dir: str | Path) -> dict[str, list[str]]:
     return json.loads(r.stdout.strip().splitlines()[-1])
 
 
-def check(packages_dir: str | Path) -> dict[str, dict]:
-    """Per reference package: how many public names, and which of them do NOT resolve through the alias."""
+def check(packages_dir: str | Path | dict) -> dict[str, dict]:
+    """Per reference package: how many public names, and which of them do NOT resolve through the alias. ``packages_dir`` is the
+    reference tree, or the output of :func:`reference_public_names` recorded from it."""
+    ref = packages_dir if isinstance(packages_dir, dict) else reference_public_names(packages_dir)
     install()
     out = {}
-    for pkg, names in reference_public_names(packages_dir).items():
+    for pkg, names in ref.items():
         if names and names[0].startswith("!"):
             out[pkg] = {"error": names[0][1:]}
             continue
@@ -160,17 +162,25 @@ SIGNATURE_MODULES = ("prime_sandboxes", "prime_evals", "prime_tunnel", "prime_mc
                      "prime_cli.core.config")  # fmt: skip
 
 
-def check_signatures(packages_dir: str | Path) -> dict:
-    """Every public class of the reference's SDK packages and API clients: do its public methods exist here, and does each
-    accept the reference's parameter names? (pydantic validator methods — ``validate_*`` — are implementation detail and ignored)"""
-    import inspect
+def reference_signatures(packages_dir: str | Path) -> dict:
+    """Public classes / functions of the reference's SDK packages and API clients with their parameter names, read in a child
+    interpreter."""
     import os
 
     env = {**os.environ, "PYTHONPATH": os.pathsep.join(str(Path(packages_dir) / d / "src") for d in _REF_DIRS.values())}
     r = subprocess.run([sys.executable, "-c", _SIG_CODE, *SIGNATURE_MODULES], env=env, capture_output=True, text=True, cwd="/", timeout=300)
     if r.returncode != 0:
         raise RuntimeError(r.stderr[-2000:])
-    ref = json.loads(r.stdout.strip().splitlines()[-1])
+    return json.loads(r.stdout.strip().splitlines()[-1])
+
+
+def check_signatures(packages_dir: str | Path | dict) -> dict:
+    """Every public class of the reference's SDK packages and API clients: do its public methods exist here, and does each
+    accept the reference's parameter names? (pydantic validator methods — ``validate_*`` — are implementation detail and ignored)
+    ``packages_dir`` is the reference tree, or the output of :func:`reference_signatures` recorded from it."""
+    import inspect
+
+    ref = packages_dir if isinstance(packages_dir, dict) else reference_signatures(packages_dir)
     install()
     compared, missing, param_diffs, errors = 0, [], [], []
     for modname, classes in ref.items():

@@ -1,7 +1,7 @@
 """Training configuration: pydantic schema, TOML loading and CLI overrides.
 
 Surface follows the DiLoCo engine's public contract named in BASELINE.json
-(``diloco.train @configs/1B/b200.toml --optim.lr 3e-4``): nested sections
+(``diloco.train @configs/1B/h100.toml --optim.lr 3e-4``): nested sections
 ``data / optim / train / ckpt / diloco / mesh``; unknown keys are rejected.
 
 The merge order (CLI > TOML > defaults) and the ``extra="forbid"`` +
@@ -62,7 +62,7 @@ class TrainConfig(_Section):
     micro_bs: int = 16
     ac_ckpt: bool | int = False
     # ZeRO-3: bf16 parameters sharded 1/F, gathered from the peers INSIDE the consuming GEMMs (parallel/fsdp.py). None = automatic:
-    # on for models of 5 B parameters and more when fsdp_size > 1, off below that (180 GB HBM: small models stay resident)
+    # on for models of 5 B parameters and more when fsdp_size > 1, off below that (small models stay resident)
     reshard_after_forward: bool | None = None
     cuda_graphs: bool = False
     log_model_hash: bool = False

@@ -172,7 +172,7 @@ __global__ void __launch_bounds__(512) grad_reduce_kernel(PeerPtrs grads, int64_
   if (threadIdx.x == 0) sumsq_partial[blockIdx.x] += ss;
 }
 
-PB_EXPORT int pb_grad_reduce_grid() { return 148 * 2; }
+PB_EXPORT int pb_grad_reduce_grid() { return 132 * 2; }
 
 PB_EXPORT int pb_grad_reduce(const PeerPtrs* grads, int64_t off, int64_t n, float scale, float* out, float* sumsq_partial,
                              const uint32_t* wait_flags, int slot_base, uint32_t expect, uint32_t* err, int max_ctas,
@@ -364,7 +364,7 @@ PB_EXPORT int pb_adamw_push(float* p32, const float* g32, float* m, float* v, in
                             uint32_t epoch, const PeerPtrs* dst, int64_t dst_off, float* gnorm_out, uint32_t* err,
                             void* mc_dst, cudaStream_t stream) {
   if (n % 8 != 0 || dst_off % 8 != 0) return -1;
-  adamw_push_kernel<<<148 * 2, 512, 0, stream>>>(p32, g32, m, v, n, *a, norm_slots, n_norm, wait_flags, flag_slot, epoch,
+  adamw_push_kernel<<<132 * 2, 512, 0, stream>>>(p32, g32, m, v, n, *a, norm_slots, n_norm, wait_flags, flag_slot, epoch,
                                                  *dst, dst_off, gnorm_out, err, reinterpret_cast<__nv_bfloat16*>(mc_dst));
   PB_CHECK_LAUNCH();
   return 0;
@@ -459,7 +459,7 @@ PB_EXPORT int pb_pseudograd_quant(const float* theta0, const float* theta, int8_
                                   cudaStream_t stream) {
   if (n % 1024 != 0) return -1;
   int64_t ctas = (n / 1024 + 3) / 4;
-  if (ctas > 148 * 8) ctas = 148 * 8;
+  if (ctas > 132 * 8) ctas = 132 * 8;
   if (ctas < 1) ctas = 1;
   pseudograd_quant_kernel<<<(unsigned)ctas, 256, 0, stream>>>(theta0, theta, q, scales, n);
   PB_CHECK_LAUNCH();
@@ -549,7 +549,7 @@ PB_EXPORT int pb_outer_nesterov(const PeerPtrs* qs, const PeerPtrs* ss, float* t
                                 int nb, const uint32_t* err, cudaStream_t stream) {
   if (n % 1024 != 0 || nb < 1) return -1;
   int64_t ctas = (n / 1024 + 3) / 4;
-  if (ctas > 148 * 8) ctas = 148 * 8;
+  if (ctas > 132 * 8) ctas = 132 * 8;
   if (ctas < 1) ctas = 1;
   BucketTable tab{shard_start, dst_start, nb};
   outer_nesterov_kernel<<<(unsigned)ctas, 256, 0, stream>>>(*qs, *ss, theta0, mom, theta, n, *a, *dst, tab, err);
@@ -613,7 +613,7 @@ PB_EXPORT int pb_outer_nesterov_f32(const PeerPtrs* thetas, float* theta0, float
                                     const uint32_t* err, cudaStream_t stream) {
   if (n % 8 != 0 || nb < 1) return -1;
   BucketTable tab{shard_start, dst_start, nb};
-  outer_nesterov_f32_kernel<<<148 * 4, 256, 0, stream>>>(*thetas, theta0, mom, theta_new, n, *a, *dst, tab, err);
+  outer_nesterov_f32_kernel<<<132 * 4, 256, 0, stream>>>(*thetas, theta0, mom, theta_new, n, *a, *dst, tab, err);
   PB_CHECK_LAUNCH();
   return 0;
 }
@@ -633,7 +633,7 @@ __global__ void __launch_bounds__(512) cast_push_kernel(const float* __restrict_
 }
 PB_EXPORT int pb_cast_push(const float* src, int64_t n, const PeerPtrs* dst, int64_t dst_off, cudaStream_t stream) {
   if (n % 8 != 0 || dst_off % 8 != 0) return -1;
-  cast_push_kernel<<<148 * 2, 512, 0, stream>>>(src, n, *dst, dst_off);
+  cast_push_kernel<<<132 * 2, 512, 0, stream>>>(src, n, *dst, dst_off);
   PB_CHECK_LAUNCH();
   return 0;
 }

@@ -1,4 +1,4 @@
-// Shared device helpers for the prime_b200 sm_100a kernel library.
+// Shared device helpers for the prime_b200 sm_90a kernel library.
 // Everything here is plain CUDA C++ / inline PTX: no torch headers, no CUTLASS,
 // so a full rebuild is seconds and the .so has a C ABI loaded through ctypes.
 #pragma once

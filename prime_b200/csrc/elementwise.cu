@@ -1,4 +1,4 @@
-// Memory-bound Llama block ops for sm_100a: RMSNorm (+fused residual add), RoPE,
+// Memory-bound Llama block ops for sm_90a: RMSNorm (+fused residual add), RoPE,
 // SwiGLU, fused softmax-cross-entropy (forward + in-place gradient).
 // All kernels: 16-byte vector accesses, fp32 math, bf16 storage, one pass over HBM
 // wherever the op allows it.  Roofline target: measured copy bandwidth (MEASURED_PEAKS.json).
@@ -185,7 +185,7 @@ __global__ void __launch_bounds__(256) colsum_partials_kernel(const float* __res
 PB_EXPORT int pb_rmsnorm_bwd_grid(int64_t R) {
   // 4 resident CTAs per SM (register-capped by __launch_bounds__): each row iteration is load → block reduction → store, i.e. latency-bound per CTA, so HBM is only
   // saturated by many CTAs in flight (2 per SM measured 28 % of copy bandwidth). Cost: a [grid, D] fp32 partial buffer.
-  int64_t g = 148 * 4;
+  int64_t g = 132 * 4;
   return (int)(R < g ? R : g);
 }
 
@@ -250,7 +250,7 @@ PB_EXPORT int pb_rope_inplace(void* qkv, const float* cosb, const float* sinb, i
   if (D % 8 != 0) return -1;
   const int64_t total = tokens * rot_heads * (D / 8);
   int64_t blocks = (total + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   rope_inplace_kernel<<<(unsigned)blocks, 256, 0, stream>>>((bf16x8*)qkv, (const float4*)cosb, (const float4*)sinb,
                                                            tokens, S, rot_heads, total_heads, D / 8, sign);
   PB_CHECK_LAUNCH();
@@ -300,7 +300,7 @@ __global__ void __launch_bounds__(256) swiglu_bwd_kernel(const bf16x8* __restric
 PB_EXPORT int pb_swiglu_fwd(const void* gu, void* out, int64_t R, int F, cudaStream_t stream) {
   if (F % 8 != 0) return -1;
   int64_t blocks = (R * (F / 8) + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   swiglu_fwd_kernel<<<(unsigned)blocks, 256, 0, stream>>>((const bf16x8*)gu, (bf16x8*)out, R, F / 8);
   PB_CHECK_LAUNCH();
   return 0;
@@ -308,7 +308,7 @@ PB_EXPORT int pb_swiglu_fwd(const void* gu, void* out, int64_t R, int F, cudaStr
 PB_EXPORT int pb_swiglu_bwd(const void* gu, const void* dout, void* dgu, int64_t R, int F, cudaStream_t stream) {
   if (F % 8 != 0) return -1;
   int64_t blocks = (R * (F / 8) + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   swiglu_bwd_kernel<<<(unsigned)blocks, 256, 0, stream>>>((const bf16x8*)gu, (const bf16x8*)dout, (bf16x8*)dgu, R,
                                                          F / 8);
   PB_CHECK_LAUNCH();

@@ -123,7 +123,7 @@ PB_EXPORT int pb_embedding_fwd(const int64_t* tokens, int64_t T, const PeerPtrs*
   if (T == 0) return 0;
   const int64_t total = T * (dim >> 3);
   int64_t grid = (total + 255) / 256;
-  if (grid > 148 * 16) grid = 148 * 16;
+  if (grid > 132 * 16) grid = 132 * 16;
   embedding_fwd_kernel<<<(unsigned)grid, 256, 0, stream>>>(tokens, T, *w, rows_per_rank, dim, reinterpret_cast<__nv_bfloat16*>(out));
   PB_CHECK_LAUNCH();
   return 0;
@@ -173,7 +173,7 @@ PB_EXPORT int pb_embedding_bwd(const int64_t* tokens, int64_t T, const void* dou
 PB_EXPORT int pb_allgather_copy(const PeerPtrs* src, int64_t bytes_per_rank, void* dst, cudaStream_t stream) {
   if (bytes_per_rank % 16 != 0 || src->n < 1 || src->n > kMaxPeers) return -1;
   if (bytes_per_rank == 0) return 0;
-  allgather_copy_kernel<<<148 * 4, 512, 0, stream>>>(*src, bytes_per_rank / 16, reinterpret_cast<uint4*>(dst));
+  allgather_copy_kernel<<<132 * 4, 512, 0, stream>>>(*src, bytes_per_rank / 16, reinterpret_cast<uint4*>(dst));
   PB_CHECK_LAUNCH();
   return 0;
 }

@@ -345,7 +345,7 @@ __global__ void __launch_bounds__(512) mc_grad_reduce_kernel(const float* __rest
 
 // Number of flag words an all-reduce needs (one per block) — the grid is fixed so that every rank launches the same one
 // and all blocks are co-resident (a spinning block must never wait for a partner that is queued behind it).
-PB_EXPORT int pb_mc_all_reduce_grid() { return 148; }
+PB_EXPORT int pb_mc_all_reduce_grid() { return 132; }
 
 // dtype: 0 = f32, 1 = bf16. `mc_data` and `mc_flags` are addresses in the MULTICAST mapping, `local_flags` the same words
 // in this rank's unicast mapping. nbytes must be a multiple of 16. `epoch` starts at 1 and grows by 1 per call on every rank.
@@ -369,7 +369,7 @@ PB_EXPORT int pb_mc_grad_reduce(const float* mc_grads, int64_t off, int64_t n, f
                                 const uint32_t* wait_flags, int slot_base, uint32_t expect, int npeers, uint32_t* err,
                                 int max_ctas, cudaStream_t stream) {
   if ((off & 3) || (n & 3)) return -1;
-  int grid = 148 * 2;  // = pb_grad_reduce_grid(): sumsq_partial has one slot per block of the widest launch
+  int grid = 132 * 2;  // = pb_grad_reduce_grid(): sumsq_partial has one slot per block of the widest launch
   if (max_ctas > 0 && max_ctas < grid) grid = max_ctas;  // leave SMs to the backward pass this runs under
   mc_grad_reduce_kernel<<<grid, 512, 0, stream>>>(mc_grads, off, n, scale, out, sumsq_partial, wait_flags, slot_base, expect, npeers,
                                                   err);

@@ -126,7 +126,7 @@ int cached_tmap3(CUtensorMap* out, const void* ptr, uint64_t rows, uint64_t cols
 }
 
 // [blocks][rows][cols] bf16 (dense: block stride = rows*cols) with boxes of {box_cols, box_rows, 1}: a box never crosses a block, rows
-// past the end of a block are clipped on stores / zero-filled on loads (the weight-gather copier of gemm_sm100.cu relies on that).
+// past the end of a block are clipped on stores / zero-filled on loads (the weight-gather copier of gemm_sm90.cu relies on that).
 int cached_tmap_blocks(CUtensorMap* out, const void* ptr, uint64_t rows, uint64_t cols, uint64_t blocks, uint32_t box_cols, uint32_t box_rows) {
   static std::unordered_map<MapKey, CUtensorMap, MapKeyHash> cache;
   static std::mutex mu;

@@ -5,7 +5,7 @@
     python -m prime_b200.eval generate --ckpt … --model 1B --prompt-ids 1,306,626 --max-new 32
 
 The model is rebuilt on one device from the per-rank optimizer shards (``checkpoint.assemble_full_model``) or from a Hugging
-Face directory (``models.hf.load_hf_dir``); the forward runs through the same ops as training (native kernels on a B200, the
+Face directory (``models.hf.load_hf_dir``); the forward runs through the same ops as training (native kernels on an H100, the
 reference ops on the CPU).  Generation recomputes the whole prefix for every token — there is no KV cache in a training engine —
 and pads the sequence to a multiple of 128 on CUDA (causal attention makes right padding invisible to the position that is read),
 which is fine for inspecting a checkpoint and not a serving path.

@@ -1,6 +1,6 @@
 """Local run manager: start, watch, stop and resume training jobs on THIS box.
 
-    python -m prime_b200.launch run @configs/1B/b200.toml --gpus 8 --detach           # one world of 8 ranks
+    python -m prime_b200.launch run @configs/1B/h100.toml --gpus 8 --detach           # one world of 8 ranks
     python -m prime_b200.launch run @configs/1B/elastic.toml --workers 4 --gpus 2 \\
            --elastic --respawn 3                                                      # 4 elastic DiLoCo workers × 2 GPUs
     python -m prime_b200.launch list | get <id> | logs <id> -f | metrics <id> | checkpoints <id>

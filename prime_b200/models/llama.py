@@ -1,7 +1,7 @@
 """Llama-2/3 family on prime_b200 ops.
 
-B200-first choices:
-  * fused ``wqkv`` ([H+2Hkv]·D × dim) and ``w13`` (2·hidden × dim) parameters → one tcgen05 GEMM each;
+Hopper-first choices:
+  * fused ``wqkv`` ([H+2Hkv]·D × dim) and ``w13`` (2·hidden × dim) parameters → one wgmma GEMM each;
   * RoPE applied in place on the fused QKV activation; attention reads strided Q/K/V views of it;
   * the residual add is fused into the following RMSNorm (``add_rmsnorm``): a block returns
     ``(residual_stream, pending_delta)`` so no stand-alone elementwise add ever touches HBM;
@@ -180,7 +180,7 @@ class Transformer(nn.Module):
 
     # ------------------------------------------------------------------ init
     def set_fp8(self, on: bool) -> None:
-        """MXFP8 (block-scaled e4m3, tcgen05 kind::mxf8f6f4) for the forward and input-gradient GEMMs of every block's four
+        """MXFP8 (block-scaled e4m3) for the forward and input-gradient GEMMs of every block's four
         projections; weight gradients, the LM head, norms and attention stay bf16 / fp32."""
         for blk in self.layers:
             blk.attention.fp8 = blk.feed_forward.fp8 = bool(on)

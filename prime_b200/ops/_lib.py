@@ -1,9 +1,8 @@
-"""Build and load the native sm_100a kernel library (C ABI, ctypes).
+"""Build and load the native sm_90a kernel library (C ABI, ctypes).
 
 The library is compiled in-tree (``prime_b200/_C/libprime_b200.so``) straight from
-``prime_b200/csrc/*.cu`` with ``nvcc -gencode arch=compute_100a,code=sm_100a`` — no torch
-headers, so a full rebuild takes seconds and the artefact travels with the repo snapshot to
-the GPU box.  On a CUDA device every op in :mod:`prime_b200.ops.functional` requires this
+``prime_b200/csrc/*.cu`` with ``nvcc -gencode arch=compute_90a,code=sm_90a`` — no torch
+headers, so a full rebuild takes seconds.  On a CUDA device every op in :mod:`prime_b200.ops.functional` requires this
 library and raises if it is missing: there is no silent eager fallback on the GPU.
 """
 
@@ -24,7 +23,7 @@ HASH_PATH = OUT_DIR / "build.hash"
 
 NVCC_FLAGS = [
     "-gencode",
-    "arch=compute_100a,code=sm_100a",
+    "arch=compute_90a,code=sm_90a",
     "-lineinfo",
     "-O3",
     "-std=c++17",
@@ -51,7 +50,7 @@ def sources() -> list[Path]:
 
 
 def source_hash() -> str:
-    """Content hash of every kernel source + the flags (mtimes do not survive the gpurun snapshot)."""
+    """Content hash of every kernel source + the flags (mtimes do not survive a copy of the tree)."""
     import hashlib
 
     h = hashlib.sha256(" ".join(NVCC_FLAGS).encode())
@@ -68,7 +67,7 @@ def needs_build() -> bool:
 
 
 def build(force: bool = False, verbose: bool = False) -> Path:
-    """Compile every ``.cu`` under ``csrc/`` into one shared library for sm_100a."""
+    """Compile every ``.cu`` under ``csrc/`` into one shared library for sm_90a."""
     with _lock:
         if not force and not needs_build():
             return LIB_PATH

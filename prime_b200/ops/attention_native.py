@@ -1,7 +1,7 @@
-"""Flash attention on sm_100a over the fused QKV activation (tcgen05 QKᵀ / P·V, TMEM accumulators, TMA).
+"""Flash attention on sm_90a over the fused QKV activation (mma.sync QKᵀ / P·V tiles, registers as accumulators).
 
-Forward : ``csrc/attention_sm100.cu``      qkv [B,S,(H+2Hkv)·D] → out [B,S,H·D], lse2 [B,H,S]
-Backward: ``csrc/attention_bwd_sm100.cu``  → dqkv [B,S,(H+2Hkv)·D]  (dK/dV kernel + dQ kernel + delta preprocess)
+Forward : ``csrc/attention_sm90.cu``      qkv [B,S,(H+2Hkv)·D] → out [B,S,H·D], lse2 [B,H,S]
+Backward: ``csrc/attention_sm90.cu``    → dqkv [B,S,(H+2Hkv)·D]  (dK/dV kernel + dQ kernel + delta preprocess)
 
 No transposes, slices or concatenations ever touch HBM: the kernels address Q/K/V heads inside the fused buffer
 through one TMA tensor map and write gradients straight back in the same layout.

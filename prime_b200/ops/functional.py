@@ -1,4 +1,4 @@
-"""Public op surface.  CUDA tensors → hand-written sm_100a kernels (required, loud failure);
+"""Public op surface.  CUDA tensors → hand-written sm_90a kernels (required, loud failure);
 CPU tensors → the torch reference in :mod:`prime_b200.ops.reference`.
 
 Every CUDA op is a ``torch.autograd.Function`` whose forward/backward launch kernels from the
@@ -52,7 +52,7 @@ def gemm(
     accumulate: bool = False,
     max_ctas: int = 0,
 ) -> torch.Tensor:
-    """C[M,N] (+)= A·Bᵀ on the tcgen05 kernel.
+    """C[M,N] (+)= A·Bᵀ on the wgmma kernel.
 
     ``a``: [M,K] (K-major) or, if ``a_mn_major``, stored [K,M].
     ``b``: [N,K] (K-major) or, if ``b_mn_major``, stored [K,N].
@@ -85,8 +85,8 @@ def gemm(
 
 
 def set_gemm_pair_mode(on: bool | None) -> int:
-    """Tile scheduler of the tcgen05 GEMM: ``False`` = one CTA per 128×256 tile, ``True`` = a CTA pair (``cta_group::2``,
-    the two SMs of a TPC) per 256×256 tile, ``None`` = re-read ``PB_GEMM_PAIR``. Returns the previous mode."""
+    """Tile-scheduler selector of the GEMM, kept for API compatibility: on sm_90a every mode runs the one scheduler (one CTA per
+    128×128 tile). ``None`` = re-read ``PB_GEMM_PAIR``. Returns the previous mode."""
     return int(_lib.load().pb_gemm_set_pair_mode(-1 if on is None else int(bool(on))))
 
 
@@ -146,7 +146,7 @@ def gemm_wgather(a: torch.Tensor, z, *, b_mn_major: bool = False, out: torch.Ten
     C = gate_up, ``swiglu_h`` = h).  ``b_mn_major=True``: C[M, cols] = a[M, rows]·W (input gradient; with ``swiglu_bwd_gu`` = the
     saved gate_up the epilogue turns dh into d_gate_up [M, 2·cols] on the fly).
 
-    The peers' row blocks are pulled over NVLink by copier warps INSIDE the GEMM kernel (csrc/gemm_sm100.cu, IO = 3). The same
+    The peers' row blocks are pulled over NVLink by copier warps INSIDE the GEMM kernel (csrc/gemm_sm90.cu, IO = 3). The same
     kernel also gathers AHEAD the weight the next GEMM of the pass will consume (``z.next_fwd`` / ``z.next_bwd``), so in steady
     state a kernel finds its own operand already resident (no gating, full speed) and only carries the next one's transfer."""
     import ctypes
@@ -316,7 +316,7 @@ def quantize_mxfp8(x: torch.Tensor, transpose: bool = False) -> tuple[torch.Tens
 
 def gemm_mxfp8(aq: torch.Tensor, asf: torch.Tensor, bq: torch.Tensor, bsf: torch.Tensor, out: torch.Tensor | None = None,
                max_ctas: int = 0) -> torch.Tensor:  # fmt: skip
-    """C[M,N] bf16 = dequant(A)·dequant(B)ᵀ on ``tcgen05.mma.kind::mxf8f6f4.block_scale`` (scales applied by the tensor core)."""
+    """C[M,N] bf16 = dequant(A)·dequant(B)ᵀ with e4m3 tensor-core MMAs, scaled per 32-element block in registers."""
     M, K = aq.shape
     N, Kb = bq.shape
     assert K == Kb and aq.dtype == torch.uint8 and bq.dtype == torch.uint8 and aq.is_contiguous() and bq.is_contiguous()
@@ -886,7 +886,7 @@ def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, causal: bool = 
 def attention_qkv(qkv: torch.Tensor, n_heads: int, n_kv_heads: int, causal: bool = True, impl: str = "auto") -> torch.Tensor:
     """Attention over the fused, RoPE-rotated QKV activation [B,S,(H+2Hkv)·D] → [B,S,H·D].
 
-    ``impl``: "native" = tcgen05 flash-attention kernels (error if the shape is unsupported); "sdpa" = library
+    ``impl``: "native" = the project's flash-attention kernels (error if the shape is unsupported); "sdpa" = library
     fallback; "auto" = native whenever supported.
     """
     B, S, W = qkv.shape

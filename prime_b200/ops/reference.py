@@ -1,7 +1,7 @@
 """Plain-PyTorch reference implementations of every hot op.
 
 These are (a) the CPU/gloo execution path (BASELINE.json config 1) and (b) the
-fp32 numerical oracle every sm_100a kernel is tested against
+fp32 numerical oracle every sm_90a kernel is tested against
 (``tests/test_kernels_gpu.py``).  Nothing here is ever selected on a CUDA
 tensor by :mod:`prime_b200.ops.functional` — on the GPU the native kernels run
 or the call fails loudly.
@@ -147,7 +147,7 @@ def nesterov_outer_step(
 
 # ----------------------------------------------------------------------------------------------------------- MXFP8
 def _mxfp8_sf_index(rows: int, k: int, device=None) -> torch.Tensor:
-    """Byte offset of the scale of (row r, 32-block kb) in the tensor-core layout used by csrc/gemm_mxfp8_sm100.cu:
+    """Byte offset of the scale of (row r, 32-block kb) in the tensor-core layout used by csrc/gemm_mxfp8_sm90.cu:
     [k/128][ceil(rows/128)+1] atoms of 512 bytes; inside an atom (r % 32) * 16 + ((r % 128) // 32) * 4 + kb % 4."""
     atoms = (rows + 127) // 128 + 1
     r = torch.arange(rows, device=device).view(-1, 1)

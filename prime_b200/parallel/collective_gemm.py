@@ -8,7 +8,7 @@
 ``gemm_reduce_scatter``  every rank multiplies its K-shard; the GEMM epilogue TMA-reduce-adds each fp32 tile into the buffer of the
                          rank that owns those rows (row-parallel linear → sequence-sharded output).
 
-Both are ONE kernel each (``csrc/gemm_sm100.cu``, IO = 1 / 2); the only extra launches are two flag barriers that fence the
+Both are ONE kernel each (``csrc/gemm_sm90.cu``, IO = 1 / 2); the only extra launches are two flag barriers that fence the
 symmetric buffers. The NCCL formulation of the same ops (``all_gather_into_tensor`` + GEMM, GEMM + ``reduce_scatter_tensor``) is
 the baseline they are benchmarked against in ``tools/collective_gemm_bench.py``.
 """

@@ -2,7 +2,7 @@
 across workers and take a Nesterov-SGD step on the replicated outer parameters θ₀.
 
 State lives on the GPU (θ₀ and the momentum buffer are sharded exactly like the inner optimizer:
-1/F per rank, so 180 GB parts never need the host offload the H100-era engine used).
+1/F per rank, so no host offload is needed).
 
 Exchange design (SURVEY §7.3 #1): int8 payloads cannot be summed in the switch, so the all-reduce is
 an *all-gather of (int8, per-1024 scales)* followed by a local dequantise-and-sum in fixed worker

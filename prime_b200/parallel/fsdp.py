@@ -1,6 +1,6 @@
 """Sharded inner-loop engine (the FSDP level of the two-level mesh).
 
-Memory plan for 180 GB HBM3e parts: the bf16 parameters stay *resident and replicated* inside a
+Memory plan for 80 GB HBM3 parts: the bf16 parameters stay *resident and replicated* inside a
 worker (one flat buffer), while everything optimizer-side — fp32 master weights, AdamW moments, the
 reduced gradient — is partitioned 1/F per rank.  Per optimizer step the traffic is exactly FSDP's
 (one gradient reduce-scatter + one parameter all-gather per bucket); what differs is *how*:
@@ -21,7 +21,7 @@ Both share bucket layout and optimizer state, so checkpoints move freely between
 ``shard_params=True`` (``train.reshard_after_forward``; ZeRO-3, the default for 7B and larger)
     the bf16 parameters are NOT replicated: every 2-D weight is sharded by rows (dim 0, like FSDP2) and rank r keeps only
     rows [r·N/F, (r+1)·N/F) in its symmetric heap.  There is no all-gather collective at all — the GEMM that consumes a
-    weight gathers it from the peers' shards while it multiplies (``pb_gemm_wgather``, IO = 3 of ``csrc/gemm_sm100.cu``:
+    weight gathers it from the peers' shards while it multiplies (``pb_gemm_wgather``, IO = 3 of ``csrc/gemm_sm90.cu``:
     copier warps TMA the peer rows over NVLink into ONE layer-sized scratch that every layer reuses, the MMA tiles are
     released quarter block by quarter block), in the forward (y = x·Wᵀ, with the RoPE / SwiGLU epilogues) and again in the
     backward (dx = dy·W).  The embedding row gather reads the owners' shards directly.  The optimizer then updates only

@@ -8,10 +8,10 @@ backward, the only cross-GPU traffic is inside four GEMM kernels:
                y_local = reduce_scatter(h · W2ᵀ)     GEMM ⊕ reduce-scatter
     backward   dh      = all_gather(dy) · W2         all-gather ⊕ GEMM   (keeps the gathered dy for dW2)
                dx_local= reduce_scatter(dgu · W13)   GEMM ⊕ reduce-scatter
-               dW2 += dy_fullᵀ · h,  dW13 += dguᵀ · x_full                local tcgen05 GEMMs (fp32 accumulate into main_grad)
+               dW2 += dy_fullᵀ · h,  dW13 += dguᵀ · x_full                local wgmma GEMMs (fp32 accumulate into main_grad)
 
 The reference has no parallel-training code at all (SURVEY.md §2.4: every strategy ABSENT); this module exists because the
-B200 task statement asks for compute ⊕ collective kernels wherever a GEMM neighbours a collective.
+engine wants compute ⊕ collective kernels wherever a GEMM neighbours a collective.
 """
 
 from __future__ import annotations

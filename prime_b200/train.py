@@ -1,4 +1,4 @@
-"""Training entrypoint: ``python -m prime_b200.train @configs/1B/b200.toml --optim.lr 3e-4`` (alias: ``python -m diloco.train``).
+"""Training entrypoint: ``python -m prime_b200.train @configs/1B/h100.toml --optim.lr 3e-4`` (alias: ``python -m diloco.train``).
 
     torchrun --nproc-per-node 8 -m prime_b200.train @configs/1B/diloco_4x2.toml          # static mesh, one world
     GLOBAL_PORT=29400 GLOBAL_UNIQUE_ID=w0 torchrun --nproc-per-node 2 --master-port 29510 \

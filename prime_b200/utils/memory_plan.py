@@ -3,7 +3,7 @@
     python -m prime_b200.utils.memory_plan @configs/7B/fsdp_8.toml --world 8
     python -m prime_b200.utils.memory_plan --model 70B --fsdp 8 --micro-bs 1 --seq 4096
 
-Why it exists: a B200 has 180 GB and the engine takes its big buffers once, at start-up, from two places — the symmetric NVLink
+Why it exists: an H100 has 80 GB and the engine takes its big buffers once, at start-up, from two places — the symmetric NVLink
 heap (``parallel/symm.py``: one ``cudaMalloc`` + IPC mapping per rank, invisible to torch's allocator statistics) and torch's caching
 allocator. A configuration that cannot fit used to die inside ``cudaMalloc`` on one rank while its peers waited in the handle
 exchange; on a shared box that is a hung job. ``Trainer`` now calls :func:`plan_from_config` first and refuses with the table below.
@@ -15,9 +15,9 @@ Two kinds of rows:
   gradient shard, DiLoCo θ₀ / momentum / int8 payload, ZeRO-3 gather scratch. Bucket padding (< 0.1 %) is covered by a margin.
 * **activations** (estimate, conservative): tensors the autograd functions in ``ops/functional.py`` keep for the backward, per
   token and layer ``2·(5·dim + qkv_width + 3·ffn_hidden)`` bytes (residual, normed input, rotated QKV, attention output, second
-  residual / normed input, gate‖up, SwiGLU output) + row statistics, plus the logits / loss workspace. Checked against the one
-  committed measurement of a large model (``profiles/train_7b_fsdp4_r1.log``: 90.8 GiB peak in torch's allocator; the torch rows of this
-  plan sum to 92.8 GiB for the same configuration).
+  residual / normed input, gate‖up, SwiGLU output) + row statistics, plus the logits / loss workspace. Checked against a
+  measured run (``bench.py --gpus 1`` on an H100 80GB HBM3, Llama-1B, micro-batch 16 × 1024, DiLoCo: 42.0 GB peak in torch's allocator;
+  the torch rows of this plan sum to 42.8 GB for the same configuration).
 
 Only the exact rows can make a configuration an error; the estimate produces a warning. (The reference has no counterpart: its
 ``prime rl`` / ``prime pods`` commands pick a GPU count from a table in the control plane — reference:
@@ -35,7 +35,7 @@ from dataclasses import dataclass, field
 from ..models.llama import ModelArgs, get_model_args
 
 GB = 1e9
-B200_HBM_BYTES = int(180 * GB)
+H100_HBM_BYTES = int(80 * GB)
 SHARD_ALIGN = 1024
 CUDA_CONTEXT_BYTES = int(1.5 * GB)  # context + loaded modules + cuBLAS / NCCL workspaces of the comparison paths (measured ≈ 1.1 GB)
 
@@ -69,7 +69,7 @@ class Row:
 @dataclass
 class MemoryPlan:
     rows: list[Row] = field(default_factory=list)
-    capacity: int = B200_HBM_BYTES
+    capacity: int = H100_HBM_BYTES
     describe: str = ""
 
     def add(self, name: str, nbytes: float, where: str, exact: bool = True, note: str = "") -> None:
@@ -118,7 +118,7 @@ class MemoryPlanError(ValueError):
 
 def plan_memory(a: ModelArgs, *, fsdp_size: int = 1, micro_bs: int = 1, seq_len: int = 1024, shard_params: bool | None = None,
                 ac_ckpt: bool | int = False, diloco: bool = False, compression: str = "int8", fused: bool = True, fp8: bool = False,
-                capacity: int = B200_HBM_BYTES, name: str = "") -> MemoryPlan:  # fmt: skip
+                capacity: int = H100_HBM_BYTES, name: str = "") -> MemoryPlan:  # fmt: skip
     """The budget of ONE rank. ``shard_params=None`` applies the Trainer's rule (ZeRO-3 from 5 B parameters when F > 1 and the fused
     backend is on)."""
     c = count_params(a)
@@ -178,7 +178,7 @@ def plan_memory(a: ModelArgs, *, fsdp_size: int = 1, micro_bs: int = 1, seq_len:
     return p
 
 
-def plan_from_config(cfg, world_size: int, *, capacity: int = B200_HBM_BYTES, fused: bool | None = None, fsdp_size: int | None = None,
+def plan_from_config(cfg, world_size: int, *, capacity: int = H100_HBM_BYTES, fused: bool | None = None, fsdp_size: int | None = None,
                      model_overrides: dict | None = None) -> MemoryPlan:  # fmt: skip
     """The plan of a ``prime_b200.config.Config`` on ``world_size`` ranks (mesh derivation as in ``parallel/mesh.py``; ``fsdp_size``
     overrides it when the caller already built the mesh)."""
@@ -235,7 +235,7 @@ def main(argv: list[str] | None = None) -> int:
     ap.add_argument("--ac-ckpt", action="store_true")
     ap.add_argument("--diloco", action="store_true")
     ap.add_argument("--reshard", type=int, choices=(0, 1), default=None)
-    ap.add_argument("--capacity-gb", type=float, default=B200_HBM_BYTES / GB)
+    ap.add_argument("--capacity-gb", type=float, default=H100_HBM_BYTES / GB)
     ap.add_argument("--json", action="store_true")
     ns = ap.parse_args(argv)
     cap = int(ns.capacity_gb * GB)

@@ -15,7 +15,7 @@ os.environ["COLUMNS"], os.environ["LINES"] = "200", "50"
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the H100 box)")
     config.addinivalue_line("markers", "multigpu: needs >= 2 CUDA devices")
     config.addinivalue_line("markers", "slow: multi-process tests that take tens of seconds")
 

@@ -50,10 +50,13 @@ def test_tailnet_example_with_stub_tailscale(tmp_path):
     waited for through its socket, the auth key reaches `tailscale up` as a sandbox secret (environment) and is in no record or output."""
     bin_dir = tmp_path / "bin"
     bin_dir.mkdir()
+    # the service maps the sandbox's /tmp under its scratch root, so the socket's host path can exceed the 108-byte AF_UNIX limit
+    # when the temporary directory is deep: bind by basename from inside the socket's directory (the limit applies to that string)
     (bin_dir / "tailscaled").write_text(
-        "#!/usr/bin/env python3\nimport socket, sys, time\n"
+        f"#!{sys.executable}\nimport os, socket, sys, time\n"
         "path = [a.split('=', 1)[1] for a in sys.argv if a.startswith('--socket=')][0]\n"
-        "s = socket.socket(socket.AF_UNIX); s.bind(path); s.listen(1); time.sleep(120)\n")  # fmt: skip
+        "os.chdir(os.path.dirname(path) or '.')\n"
+        "s = socket.socket(socket.AF_UNIX); s.bind(os.path.basename(path)); s.listen(1); time.sleep(120)\n")  # fmt: skip
     (bin_dir / "tailscale").write_text(
         "#!/bin/bash\nshift  # --socket=…\ncase \"$1\" in\n"
         "  up) [[ \"$*\" == *\"--authkey=tskey-test-123\"* ]] || { echo 'bad key' >&2; exit 1; } ;;\n"

@@ -1,7 +1,7 @@
-"""CPU-side guards on the BUILT library: the Blackwell instruction paths must stay in the binary (cuobjdump needs no GPU).
+"""CPU-side guards on the BUILT library: the Hopper instruction paths must stay in the binary (cuobjdump needs no GPU).
 
-If a refactor silently turns a tcgen05 kernel into a legacy `mma.sync` one, or drops the block-scaled / TMEM-operand / peer paths,
-these fail here, before any GPU time is spent."""
+If a refactor silently turns the wgmma GEMM into an `mma.sync` one, drops its TMA loads, or loses the peer / NVLS paths, these fail
+here, before any GPU time is spent."""
 
 import csv
 import io
@@ -38,15 +38,16 @@ def _kernels(sass: str) -> dict[str, str]:
 
 
 @needs_toolchain
-def test_no_legacy_tensor_core_instructions(sass):
-    import re
-
-    assert not re.search(r"\sHMMA\.", sass), "legacy mma.sync (HMMA) found: a kernel fell off the tcgen05 path"
-    assert "arch = sm_100a" in sass
+def test_gemm_kernels_use_wgmma(sass):
+    assert "arch = sm_90a" in sass
+    gemms = {n: b for n, b in _kernels(sass).items() if "gemm_bf16_kernel" in n}
+    assert gemms
+    for n, b in gemms.items():
+        assert "HGMMA" in b and "HMMA" not in b.replace("HGMMA", ""), f"{n} is not on the wgmma path"
 
 
 @needs_toolchain
-def test_blackwell_paths_are_present(sass):
+def test_hopper_paths_are_present(sass):
     k = _kernels(sass)
 
     def body(*needles):
@@ -55,12 +56,11 @@ def test_blackwell_paths_are_present(sass):
         return "\n".join(hits)
 
     gemm = body("gemm_bf16_kernel")
-    assert "UTCHMMA.2CTA" in gemm and "UTMALDG" in gemm and "UTMAREDG" in gemm and "LDTM" in gemm  # cta_group::2 MMAs, TMA load / reduce-add
-    mx = body("gemm_mxfp8_kernel")
-    assert "UTCQMMA" in mx and "UTCCP" in mx  # block-scaled MMA with the scales copied into TMEM
-    fwd2 = body("flash_fwd2_kernel")
-    assert "UTCHMMA" in fwd2 and "STTM" in fwd2 and "MUFU.EX2" in fwd2  # P written to TMEM, consumed as an MMA operand
-    assert "UTCHMMA" in body("bwd_dkdv_kernel") and "UTCHMMA" in body("bwd_dq_kernel")
+    assert "HGMMA" in gemm and "UTMALDG" in gemm and "UTMASTG" in gemm  # wgmma fed by TMA loads; TMA stores of the gather copiers
+    assert "HMMA" in body("gemm_mxfp8_kernel")
+    for name in ("flash_fwd_kernel", "bwd_dkdv_kernel", "bwd_dq_kernel"):
+        a = body(name)
+        assert "HMMA" in a and "LDSM" in a and "MUFU.EX2" in a, name  # tensor-core tiles fed by ldmatrix, exp2 softmax
     comm = body("adamw_push_kernel")
     assert "STG.E.128" in comm  # 128-bit peer stores
     assert "LD.E.STRONG.SYS" in body("outer_nesterov") or "STRONG.SYS" in body("outer_nesterov")
@@ -88,21 +88,3 @@ def test_ncu_source_hotspots_condenses_runs(tmp_path, capsys):
     out = capsys.readouterr().out
     assert "4 instructions, 100 stall samples" in out
     assert "exec       100" in out and "FFMA 90" in out and "(90.0 %)" in out
-
-
-def test_step_composition_is_reproducible_from_the_committed_launch_list(capsys):
-    """profiles/step_composition_r2_final.md is what tools/launch_breakdown.py prints for the committed ncu launch list."""
-    import sys
-
-    sys.path.insert(0, str(ROOT))
-    from tools.launch_breakdown import family, main
-
-    csv = ROOT / "profiles" / "launches_1gpu_step_r2_final.csv"
-    if not csv.exists():
-        pytest.skip("launch list not committed")
-    main(str(csv))
-    out = capsys.readouterr().out
-    rows = {ln.split("|")[1].strip(): float(ln.split("|")[4].strip().rstrip(" %")) for ln in out.splitlines() if ln.startswith("| ") and ln.rstrip().endswith("% |") and "`" not in ln}
-    assert rows["GEMM (tcgen05)"] > 70 and rows["attention"] < 16 and rows["torch / runtime kernels"] < 0.5, rows
-    assert family("void <unnamed>::gemm_bf16_kernel<1, 1, 1, 0, 0>(CUtensorMap_st)") == "GEMM (tcgen05)"
-    assert family("void at::native::vectorized_elementwise_kernel<4, at::native::FillFunctor<float>>") == "torch / runtime kernels"

@@ -60,11 +60,11 @@ def test_worker_command_injects_paths_once(runs):
 
 
 def test_run_refuses_a_configuration_that_cannot_fit_before_starting_anything(runs, monkeypatch):
-    """`run --gpus 8` with llama2/70B: model + optimizer state alone exceed a 180 GB part → the command ends with the memory table and
+    """`run --gpus 8` with llama2/70B: model + optimizer state alone exceed an 80 GB part → the command ends with the memory table and
     no run directory, no supervisor, no ranks. A configuration the planner cannot read is not this check's business."""
     with pytest.raises(SystemExit) as e:
         launch.main(["run", "--gpus", "8", "--detach", "--", "--name_model", "70B", "--data.seq_length", "4096", "--train.micro_bs", "1"])
-    assert "cannot fit a 180 GB GPU" in str(e.value) and "fp32 main_grad" in str(e.value)
+    assert "cannot fit a 80 GB GPU" in str(e.value) and "fp32 main_grad" in str(e.value)
     assert list(launch.iter_runs()) == []
     launch.preflight_memory(["--name_model", "7B", "--data.seq_length", "4096", "--train.micro_bs", "1"], 8)  # fits: no exception
     launch.preflight_memory(["--no_such_key", "1"], 8)  # unreadable: left to the workers

@@ -1,4 +1,4 @@
-"""Full-model parity at the Llama-1B shape: logits and every parameter gradient of the native bf16 model (tcgen05 GEMMs, flash
+"""Full-model parity at the Llama-1B shape: logits and every parameter gradient of the native bf16 model (wgmma GEMMs, flash
 attention, fused epilogues, native embedding / loss) against an independent fp32 PyTorch model with the same weights
 (``baseline/torch_b0.Llama`` — nn.Linear, SDPA, complex-multiply RoPE). VERDICT r1 #7."""
 

@@ -82,9 +82,8 @@ def test_fsdp2_fused_matches_collective(tmp_path):
     assert r["la"][-1] < r["la"][0]
 
 
-# NVLS (multimem.ld_reduce / multimem.st over a VMM heap bound to an NVSwitch multicast object) was brought up on hardware in
-# round 2 (2 x B200: both tests green, gpurun_out/r2b_pytest_nvls.txt); the tests skip themselves only where the driver reports
-# no multicast support.
+# NVLS (multimem.ld_reduce / multimem.st over a VMM heap bound to an NVSwitch multicast object); the tests skip themselves only where
+# the driver reports no multicast support.
 def test_fsdp2_nvls_reduce_scatter_matches_collective(tmp_path):
     """PB_NVLS=1: the heap is VMM-backed with a multicast mapping and the gradient reduce-scatter is summed by the switch."""
     from prime_b200.parallel.multicast import nvls_available

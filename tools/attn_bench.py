@@ -1,4 +1,4 @@
-"""Time the native tcgen05 flash-attention (fwd, bwd) against SDPA/cuDNN on the Llama shapes. CUDA events, median."""
+"""Time the native flash-attention (fwd, bwd) against SDPA/cuDNN on the Llama shapes. CUDA events, median."""
 
 import json
 import sys

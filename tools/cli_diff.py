@@ -4,7 +4,9 @@ against the recording fake server of ``tools/wire_diff.py``. Compared per comman
 path, query, JSON body) and — where the command prints JSON (``--output json``) — the parsed JSON: every key and value of the
 reference's JSON must be present in this CLI's (which may add keys).
 
-    python tools/cli_diff.py > profiles/cli_diff.json          # exit code 1 on any difference
+    python tools/cli_diff.py > cli_diff.json                   # exit code 1 on any difference
+    python tools/cli_diff.py [6] --record tests/golden/reference_cli_diff.json.gz  # store the reference CLI's side for that stride (needs the reference)
+    python tools/cli_diff.py --reference tests/golden/reference_cli_diff.json.gz  # compare against the stored side
 """
 
 from __future__ import annotations
@@ -22,7 +24,7 @@ from pathlib import Path
 
 ROOT = Path(__file__).resolve().parent.parent
 sys.path.insert(0, str(ROOT))
-from tools.wire_diff import REF_PATHS, Recorder, covers  # noqa: E402
+from tools.wire_diff import REF_PATHS, Recorder, covers, read_json, write_json  # noqa: E402
 
 COMMANDS: list[list[str]] = [
     ["pods", "list", "--output", "json"], ["pods", "list", "--limit", "10", "--offset", "5", "-o", "json"], ["pods", "status", "p1", "-o", "json"],
@@ -246,8 +248,13 @@ def same_or_fewer_reads(ours: list, ref: list) -> tuple[bool, int]:
     return ok, len(dropped) if ok else 0
 
 
-def main(stride: int = 1) -> int:
-    """``stride`` > 1 runs every stride-th command line (the test suite's quick pass; the committed profile is the full run)."""
+def main(stride: int = 1, reference: str | Path | None = None, record: str | Path | None = None) -> int:
+    """``stride`` > 1 runs every stride-th command line (the test suite's quick pass). ``reference``: a JSON file with the reference
+    CLI's exit codes, requests, JSON output and ~/.prime files per command line, written earlier by ``record`` (a full run); the
+    reference packages are then not needed. Recordings are kept per stride: a command's requests depend on what the commands before
+    it left in ~/.prime (a cached sandbox gateway token, say)."""
+    recorded = read_json(reference)[str(stride)] if reference is not None else None
+    to_record: dict = {"commands": {}}
     srv = ThreadingHTTPServer(("127.0.0.1", 0), Recorder)
     srv.daemon_threads = True
     threading.Thread(target=srv.serve_forever, daemon=True).start()
@@ -258,18 +265,25 @@ def main(stride: int = 1) -> int:
             prepare_files(Path(h))
         for args in COMMANDS[::stride]:
             got = {}
+            key = " ".join(args)
             for arm, home in (("reference", h1), ("ours", h2)):
+                if arm == "reference" and recorded is not None:
+                    got[arm] = {**recorded["commands"][key], "stdout_tail": "", "stderr_tail": ""}
+                    continue
                 rc, out, err = run_cli(arm, base, home, args)
                 log = json.loads(urllib.request.urlopen(base + "/__log").read())
                 got[arm] = {"exit_code": rc, "requests": [{k: e[k] for k in ("method", "path", "query", "body")} for e in log], "json": parsed_json(out),
                             "stdout_tail": out.strip()[-300:], "stderr_tail": err.strip()[-300:]}  # fmt: skip
+            arms = (("ours", h2),) if recorded is not None else (("reference", h1), ("ours", h2))
             if args[:2] == ["env", "init"]:  # the scaffold each CLI wrote: same files, same contents
-                for arm, home in (("reference", h1), ("ours", h2)):
+                for arm, home in arms:
                     root = Path(home) / "environments"
                     got[arm]["json"] = {str(p.relative_to(home)): (p.read_text() if p.is_file() else None) for p in sorted(root.rglob("*"))} if root.exists() else None
             if args[:2] == ["rl", "init"]:  # the template each CLI wrote: compare what it configures, not its comments
-                got["reference"]["json"], got["ours"]["json"] = toml_of(Path(h1) / args[2]), toml_of(Path(h2) / args[2])
+                for arm, home in arms:
+                    got[arm]["json"] = toml_of(Path(home) / args[2])
             a, b = got["reference"], got["ours"]
+            to_record["commands"][key] = {k: a[k] for k in ("exit_code", "requests", "json")}
             row = {"command": "prime " + " ".join(args), "exit_code": b["exit_code"], "requests": len(b["requests"]),
                    "same_exit_code": a["exit_code"] == b["exit_code"], "same_requests": same_or_fewer_reads(b["requests"], a["requests"])[0],
                    "reads_saved": same_or_fewer_reads(b["requests"], a["requests"])[1],
@@ -282,6 +296,9 @@ def main(stride: int = 1) -> int:
         # what the commands left on disk: users who switch keep their ~/.prime
         state = {}
         for arm, home in (("reference", h1), ("ours", h2)):
+            if arm == "reference" and recorded is not None:
+                state[arm] = recorded["dot_prime"]
+                continue
             d = Path(home) / ".prime"
             files = {}
             for f in sorted(d.rglob("*.json")) if d.exists() else []:
@@ -291,14 +308,21 @@ def main(stride: int = 1) -> int:
                     files[str(f.relative_to(d))] = "<unreadable>"
             state[arm] = files
 
-        def stable(v, home):  # expiry stamps of cached gateway tokens differ run to run; paths under the arm's private $HOME → "~"
+        def stable(v, home):  # expiry stamps of cached gateway tokens differ run to run; paths under the arm's private $HOME → "~";
+            # the recording server's address (a free port per run) → "<server>"
             if isinstance(v, dict):
                 return {k: stable(x, home) for k, x in v.items() if k not in ("cached_at", "expires_at", "last_check", "timestamp")}
             if isinstance(v, list):
                 return [stable(x, home) for x in v]
-            return v.replace(home, "~") if isinstance(v, str) else v
+            return v.replace(home, "~").replace(base, "<server>") if isinstance(v, str) else v
 
-        on_disk_same = stride > 1 or covers(stable(state["ours"], h2), stable(state["reference"], h1))
+        ref_state = state["reference"] if recorded is not None else stable(state["reference"], h1)
+        on_disk_same = stride > 1 or covers(stable(state["ours"], h2), ref_state)
+        if record is not None and recorded is None:
+            to_record["dot_prime"] = stable(state["reference"], h1)
+            everything = read_json(record) if Path(record).exists() else {}
+            everything[str(stride)] = to_record
+            write_json(record, everything)
         if not on_disk_same:
             diffs.append({"command": "<files under ~/.prime after the run>", "reference": {"exit_code": 0, "requests": [], "json": state["reference"], "stdout_tail": "", "stderr_tail": ""},
                           "ours": {"exit_code": 0, "requests": [], "json": state["ours"], "stdout_tail": "", "stderr_tail": ""}})  # fmt: skip
@@ -309,4 +333,11 @@ def main(stride: int = 1) -> int:
 
 
 if __name__ == "__main__":
-    sys.exit(main(int(sys.argv[1]) if len(sys.argv) > 1 else 1))
+    import argparse
+
+    ap = argparse.ArgumentParser()
+    ap.add_argument("stride", nargs="?", type=int, default=1)
+    ap.add_argument("--reference", default=None, help="recorded reference CLI (JSON) instead of running the reference packages")
+    ap.add_argument("--record", default=None, help="add the reference CLI's results for this stride to this JSON file")
+    a = ap.parse_args()
+    sys.exit(main(a.stride, a.reference, a.record))

@@ -6,7 +6,6 @@ python -m pytest tests -m gpu -x -q 2>&1 | tail -3 | tee gpurun_out/pytest_gpu.t
 python __graft_entry__.py smoke 2>&1 | tail -1 | tee gpurun_out/smoke.txt
 python bench.py --steps 10 --warmup 3 2>gpurun_out/bench_final.err | tee gpurun_out/bench_final.json | cut -c1-160
 python bench.py --steps 6 --warmup 3 --no-fused-comm --attn sdpa 2>/dev/null | tee gpurun_out/bench_b0_sdpa_nccl.json | cut -c1-160
-python tools/gemm_pair_check.py > gpurun_out/gemm_pair.json 2>gpurun_out/gemm_pair.err; tail -1 gpurun_out/gemm_pair.err
 python tools/attn_bench.py > gpurun_out/attn_bench_final.json 2>/dev/null
 python tools/op_bench.py > gpurun_out/op_bench_final.json 2>/dev/null
 python tools/attn_trace.py > gpurun_out/attn_trace_final.json 2>/dev/null

@@ -1,4 +1,4 @@
-"""Time the tcgen05 GEMM against cuBLAS (torch.matmul) on the Llama shapes; report TFLOP/s and fraction
+"""Time the wgmma GEMM against cuBLAS (torch.matmul) on the Llama shapes; report TFLOP/s and fraction
 of the measured peak (MEASURED_PEAKS.json).  CUDA events, warm-up, L2 flushed between iterations."""
 
 import json

@@ -10,7 +10,24 @@ import torch
 ROOT = Path(__file__).resolve().parent.parent
 sys.path.insert(0, str(ROOT))
 from prime_b200 import ops  # noqa: E402
-from tools.gemm_pair_check import timeit  # noqa: E402
+
+
+def timeit(fn, flush, iters=10, warm=3):
+    """Median device time (ms) of fn over iters launches, L2 flushed before each."""
+    for _ in range(warm):
+        fn()
+    torch.cuda.synchronize()
+    ts = []
+    for _ in range(iters):
+        flush.zero_()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        fn()
+        e1.record()
+        torch.cuda.synchronize()
+        ts.append(e0.elapsed_time(e1))
+    ts.sort()
+    return ts[len(ts) // 2]
 
 
 def main():

@@ -13,7 +13,7 @@ import sys
 from collections import defaultdict
 
 FAMILIES = [
-    (r"gemm_bf16_kernel", "GEMM (tcgen05)"),
+    (r"gemm_bf16_kernel", "GEMM (wgmma)"),
     (r"gemm_mxfp8|quantize_mxfp8", "MXFP8 GEMM / quantisers"),
     (r"flash_fwd|bwd_dkdv|bwd_dq|bwd_delta", "attention"),
     (r"rmsnorm|colsum", "RMSNorm (fwd, bwd, weight-grad column sums)"),

@@ -1,6 +1,6 @@
 // TMA delivery rate per SM as a function of box geometry, ring depth and row pitch: one CTA per SM, one thread issues 2-D tiled
 // loads (SWIZZLE_128B, 64 bf16 = 128 B wide boxes) into a ring of 32 KB "tiles" and waits for each tile in order.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/micro/tma_bench tools/micro/tma_bench.cu -lcuda
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/micro/tma_bench tools/micro/tma_bench.cu -lcuda
 // Run  : tools/micro/tma_bench            → one JSON line per configuration (bytes per clock per SM, clocks per 32 KB tile)
 #include <cstdio>
 #include <cstdint>
@@ -86,7 +86,7 @@ int main() {
     for (int promo = 0; promo < 2; ++promo)
       for (int box_rows : {64, 128})
         for (int stages : {2, 4, 6})
-          for (int rows_per_cta : {1024, 110}) {  // 110 rows x 148 CTAs: everything L2-resident and reused
+          for (int rows_per_cta : {1024, 110}) {  // 110 rows x 132 CTAs: everything L2-resident and reused
             CUtensorMap map;
             cuuint64_t dims[2] = {cols, rows};
             cuuint64_t strides[1] = {cols * 2};

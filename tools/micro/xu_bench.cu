@@ -1,5 +1,5 @@
 // Per-SM throughput of the instructions the attention softmax leans on: MUFU.EX2, F2FP (fp32x2 → bf16x2 pack), FFMA.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/micro/xu_bench tools/micro/xu_bench.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/micro/xu_bench tools/micro/xu_bench.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 

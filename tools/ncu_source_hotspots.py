@@ -4,8 +4,8 @@
     python tools/ncu_source_hotspots.py /tmp/dkdv.csv
 
 Instructions are grouped into runs with the same execution count (= same loop nest / branch); for every run the share of all
-stall samples and the opcodes that collected them are printed, then the top single instructions. This is how the attention
-backward's lse/delta loads and its masked-tile cost were found (profiles/README.md, "Attention backward, v6").
+stall samples and the opcodes that collected them are printed, then the top single instructions. Useful to find which loads or
+branches of a kernel collect the stalls.
 """
 
 import collections

@@ -87,7 +87,7 @@ def main(paths):
         peaks = json.loads((ROOT / "MEASURED_PEAKS.json").read_text())
     except Exception:
         pass
-    hbm = peaks.get("hbm_gbs", 6571.0)
+    hbm = peaks.get("hbm_gbs", 3350.0)  # default: H100 SXM data-sheet HBM3 bandwidth (not a measured rate)
     print("# ncu summary (one row per captured launch; `--set full --clock-control none`, durations are under the profiler's cache control — "
           "compare shares and utilisations, not absolute times; event-timed numbers live in the *_bench JSON files)\n")  # fmt: skip
     cols = ["kernel", "tmpl", "dur_us", "dram_rd_MB", "dram_wr_MB", "dram_GBps", "dram_pct", "tensor_pct", "sm_pct", "warps_active_pct", "regs", "grid", "block",

@@ -45,7 +45,7 @@ def main():
     dev = torch.device("cuda", 0)
     torch.cuda.set_device(dev)
     peaks = json.loads((ROOT / "MEASURED_PEAKS.json").read_text()) if (ROOT / "MEASURED_PEAKS.json").exists() else {}
-    hbm = float(peaks.get("hbm_gbs", 6571.0))
+    hbm = float(peaks.get("hbm_gbs", 3350.0))  # default: H100 SXM data-sheet HBM3 bandwidth (not a measured rate)
     flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
     from prime_b200.utils.clocks import ClockSampler
 

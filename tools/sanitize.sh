@@ -1,6 +1,6 @@
 #!/bin/bash
 # Run ON the GPU box: compute-sanitizer over the kernel tests. memcheck = out-of-bounds / misaligned global+shared accesses,
-# racecheck = shared-memory hazards, synccheck = invalid barrier usage. tcgen05/TMA kernels run ~50-100x slower under the tool,
+# racecheck = shared-memory hazards, synccheck = invalid barrier usage. TMA / tensor-core kernels run ~50-100x slower under the tool,
 # so each tool gets a focused subset; summaries land in gpurun_out/sanitizer_*.txt (copy to profiles/).
 set -u
 SAN=compute-sanitizer

@@ -1,12 +1,12 @@
 #!/usr/bin/env python
-"""Per-kernel SASS listings of the built library → ``profiles/sass/`` (VERDICT r1 #9: listings, not a mnemonic-count summary).
+"""Per-kernel SASS listings of the built library → ``profiles/sass/`` (local output, not committed).
 
     python tools/sass_listings.py            # every kernel family, one representative instantiation each, + INDEX.md
     python tools/sass_listings.py --all      # every instantiation (≈30 MB of text: not committed)
 
 A listing is the ``cuobjdump -sass -fun <mangled>`` output with the encoding words stripped: address + instruction per line.
 INDEX.md tabulates, per listed kernel, the instruction count and the mnemonics that prove the hardware path
-(UTC*MMA = tcgen05.mma, LDTM/STTM = TMEM, UTMA* = TMA, SYNCS = mbarrier, *.SYS = peer traffic, LDGMC/multimem = NVLS).
+(HGMMA = wgmma, HMMA = mma.sync, LDSM = ldmatrix, UTMA* = TMA, SYNCS = mbarrier, *.SYS = peer traffic, LDGMC/multimem = NVLS).
 """
 
 from __future__ import annotations
@@ -20,25 +20,25 @@ from pathlib import Path
 ROOT = Path(__file__).resolve().parent.parent
 LIB = ROOT / "prime_b200" / "_C" / "libprime_b200.so"
 OUT = ROOT / "profiles" / "sass"
-PROOF = ["UTCHMMA", "UTCQMMA", "UTCCP", "LDTM", "STTM", "UTMALDG", "UTMASTG", "UTMAREDG", "UBLKCP", "SYNCS", "LDGMC", "HMMA", "MUFU.EX2"]
-# representative instantiation per family (demangled-name regex → short file name); first match wins
+PROOF = ["HGMMA", "UTMALDG", "UTMASTG", "SYNCS", "LDSM", "HMMA", "MUFU.EX2", "LDGMC"]
+# representative instantiation per family (demangled-name regex → short file name); first match wins.
+# gemm_bf16_kernel<A_MN, B_MN, EPI, IO>: EPI 0 plain | 1 RoPE | 2 SwiGLU | 3 SwiGLU backward; IO 0 local | 1 all-gather | 2 reduce-scatter | 3 weight gather
 PICK = [
-    (r"gemm_bf16_kernel<0, 0, 1, 0, 0>", "gemm_bf16_pair_kmajor"),
-    (r"gemm_bf16_kernel<1, 1, 1, 0, 0>", "gemm_bf16_pair_wgrad_mnmajor"),
-    (r"gemm_bf16_kernel<0, 0, 1, 1, 0>", "gemm_bf16_pair_rope_epilogue"),
-    (r"gemm_bf16_kernel<0, 0, 1, 2, 0>", "gemm_bf16_pair_swiglu_epilogue"),
-    (r"gemm_bf16_kernel<0, 0, 1, 0, 1>", "gemm_allgather_activation_IO1"),
-    (r"gemm_bf16_kernel<0, 0, 1, 0, 2>", "gemm_reduce_scatter_IO2"),
-    (r"gemm_bf16_kernel<0, 0, 1, 0, 3>", "gemm_param_gather_fwd_IO3"),
-    (r"gemm_bf16_kernel<0, 1, 1, 0, 3>", "gemm_param_gather_dgrad_IO3"),
-    (r"gemm_bf16_kernel<0, 0, 1, 2, 3>", "gemm_param_gather_swiglu_IO3"),
-    (r"gemm_bf16_kernel<0, 0, 0, 0, 0>", "gemm_bf16_single_cta"),
-    (r"gemm_mxfp8_kernel<1>", "gemm_mxfp8_pair"),
+    (r"gemm_bf16_kernel<0, 0, 0, 0>", "gemm_bf16_kmajor"),
+    (r"gemm_bf16_kernel<1, 1, 0, 0>", "gemm_bf16_wgrad_mnmajor"),
+    (r"gemm_bf16_kernel<0, 0, 1, 0>", "gemm_bf16_rope_epilogue"),
+    (r"gemm_bf16_kernel<0, 0, 2, 0>", "gemm_bf16_swiglu_epilogue"),
+    (r"gemm_bf16_kernel<0, 1, 3, 0>", "gemm_bf16_swiglu_bwd_epilogue"),
+    (r"gemm_bf16_kernel<0, 0, 0, 1>", "gemm_allgather_activation_IO1"),
+    (r"gemm_bf16_kernel<0, 0, 0, 2>", "gemm_reduce_scatter_IO2"),
+    (r"gemm_bf16_kernel<0, 0, 0, 3>", "gemm_param_gather_fwd_IO3"),
+    (r"gemm_bf16_kernel<0, 1, 0, 3>", "gemm_param_gather_dgrad_IO3"),
+    (r"gemm_bf16_kernel<0, 0, 2, 3>", "gemm_param_gather_swiglu_IO3"),
+    (r"gemm_mxfp8_kernel", "gemm_mxfp8"),
     (r"quantize_mxfp8_kernel", "quantize_mxfp8"),
-    (r"flash_fwd2_kernel<128>", "flash_fwd2_d128"),
-    (r"flash_fwd_kernel<128>", "flash_fwd1_d128"),
-    (r"bwd_dkdv_kernel<128, 1>", "flash_bwd_dkdv_d128"),
-    (r"bwd_dq_kernel<128, 1>", "flash_bwd_dq_d128"),
+    (r"flash_fwd_kernel<128>", "flash_fwd_d128"),
+    (r"bwd_dkdv_kernel<128>", "flash_bwd_dkdv_d128"),
+    (r"bwd_dq_kernel<128>", "flash_bwd_dq_d128"),
     (r"bwd_delta_kernel", "flash_bwd_delta"),
     (r"rmsnorm_fwd_kernel<4, true>", "rmsnorm_fwd_residual"),
     (r"rmsnorm_bwd_kernel<4, true>", "rmsnorm_bwd_residual"),

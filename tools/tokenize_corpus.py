@@ -3,7 +3,7 @@
 
     python tools/tokenize_corpus.py --tokenizer /models/llama-2-7b --out data/c4 corpus/*.jsonl corpus/notes.txt
     python tools/tokenize_corpus.py --tokenizer bytes --out data/tiny README.md        # no tokenizer files needed
-    python -m diloco.train @configs/1B/b200.toml --data.fake false --data.dataset_name_or_paths data/c4
+    python -m diloco.train @configs/1B/h100.toml --data.fake false --data.dataset_name_or_paths data/c4
 
 Inputs: ``.txt`` (one document per file), ``.jsonl`` / ``.json`` lines with a ``--field`` (default ``text``) per document.
 Tokenizers: a local Hugging Face tokenizer directory (``transformers.AutoTokenizer``), a SentencePiece ``.model`` file, or

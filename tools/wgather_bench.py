@@ -1,4 +1,4 @@
-"""Parameter all-gather ⊕ GEMM (ZeRO-3 hot path, IO = 3 of csrc/gemm_sm100.cu) against its roofline and against NCCL + GEMM.
+"""Parameter all-gather ⊕ GEMM (ZeRO-3 hot path, IO = 3 of csrc/gemm_sm90.cu) against its roofline and against NCCL + GEMM.
 
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 8 --master-addr 127.0.0.1 tools/wgather_bench.py --model 7B
 
@@ -63,8 +63,8 @@ def main():
     heap = SymmetricHeap(3 << 30, r, n, dist_exchange(), dev)
     flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
     peaks = json.loads((ROOT / "MEASURED_PEAKS.json").read_text()) if (ROOT / "MEASURED_PEAKS.json").exists() else {}
-    peak = float(peaks.get("bf16_tflops_sustained", 1386.0)) * 1e12
-    link = 770e9
+    peak = float(peaks.get("bf16_tflops_sustained", 989.0)) * 1e12  # default: H100 SXM data-sheet dense bf16 (not a measured rate)
+    link = 450e9  # H100 NVLink 4: 900 GB/s bidirectional per GPU = 450 GB/s per direction (data sheet)
     sampler = ClockSampler(torch.cuda.current_device())
     if r == 0:
         sampler.start()

@@ -3,7 +3,9 @@
 packages and against this repo (through ``prime_b200.compat``); a recording fake server logs every HTTP request each arm
 sends. The request sequences (method, path, query, JSON body) and the outcome of every call must be identical.
 
-    python tools/wire_diff.py > profiles/wire_diff.json        # exit code 1 on any difference
+    python tools/wire_diff.py > wire_diff.json                 # exit code 1 on any difference
+    python tools/wire_diff.py --record tests/golden/reference_wire_diff.json.gz   # store the reference arm (needs the reference)
+    python tools/wire_diff.py --reference tests/golden/reference_wire_diff.json.gz   # compare against the stored arm
 
 What it covers: 108 SDK / API-client / MCP-tool calls — sync and async sandbox and evaluation clients, RL, deployments and tunnel clients, the
 nine MCP tools; sandbox lifecycle, command execution, file transfer, ports, SSH sessions, bulk delete,
@@ -433,6 +435,21 @@ print(json.dumps(results))
 '''
 
 
+def read_json(path) -> object:
+    """JSON from ``path``; gzip-compressed when the name ends in ``.gz`` (the recorded reference arms under tests/golden/)."""
+    import gzip
+
+    raw = Path(path).read_bytes()
+    return json.loads(gzip.decompress(raw) if str(path).endswith(".gz") else raw)
+
+
+def write_json(path, obj) -> None:
+    import gzip
+
+    raw = (json.dumps(obj, sort_keys=True, separators=(",", ":")) + "\n").encode()
+    Path(path).write_bytes(gzip.compress(raw, mtime=0) if str(path).endswith(".gz") else raw)
+
+
 def run_arm(arm: str, base: str) -> tuple[list, list]:
     import urllib.request
 
@@ -470,14 +487,23 @@ def normalise(log: list) -> list:
     return out
 
 
-def main() -> int:
+def main(reference: str | Path | None = None, record: str | Path | None = None) -> int:
+    """``reference``: a JSON file with the reference arm's outcomes and normalised request log, written earlier by ``record``; the
+    reference packages are then not needed. Without it the reference arm runs from REF (and ``record`` stores what it produced)."""
     srv = ThreadingHTTPServer(("127.0.0.1", 0), Recorder)
     srv.daemon_threads = True
     threading.Thread(target=srv.serve_forever, daemon=True).start()
     base = f"http://127.0.0.1:{srv.server_address[1]}"
-    ref_res, ref_log = run_arm("reference", base)
+    if reference is not None:
+        rec = read_json(reference)
+        ref_res, ref_log = [tuple(r) for r in rec["results"]], rec["requests"]
+    else:
+        ref_res, ref_log = run_arm("reference", base)
+        ref_log = normalise(ref_log)
+        if record is not None:
+            write_json(record, {"results": ref_res, "requests": ref_log})
     our_res, our_log = run_arm("ours", base)
-    ref_log, our_log = normalise(ref_log), normalise(our_log)
+    our_log = normalise(our_log)
     diffs, wording = [], []
     for (la, sa, va), (lb, sb, vb) in zip(ref_res, our_res):
         if (la, sa) != (lb, sb):
@@ -506,4 +532,10 @@ def main() -> int:
 
 
 if __name__ == "__main__":
-    sys.exit(main())
+    import argparse
+
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--reference", default=None, help="recorded reference arm (JSON) instead of running the reference packages")
+    ap.add_argument("--record", default=None, help="write the reference arm's outcomes and request log to this JSON file")
+    a = ap.parse_args()
+    sys.exit(main(a.reference, a.record))
