@@ -33,6 +33,10 @@ class DataConfig(_Section):
     shuffle: bool = True  # per-epoch permutation of the sequence windows (seeded by data.seed)
     # held-out corpus for the periodic validation loss (same formats as dataset_name_or_paths); with data.fake a second synthetic stream
     eval_dataset_name_or_paths: str = ""
+    # document masking of packed windows: a token attends only to earlier tokens of its own document (documents end with EOS).
+    # The EOS id is data.eos_id, or else the "eos_id" of the first shard's .meta.json (tools/tokenize_corpus.py writes it)
+    document_mask: bool = False
+    eos_id: int | None = None
     num_workers: int = 2
     seed: int = 1337
     pin_memory: bool = True

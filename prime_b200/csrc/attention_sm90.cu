@@ -13,6 +13,8 @@
 //   dQ:     one CTA per (64-query block, b, h); loops over 64-key tiles: S = Q Kᵀ, dP = dO Vᵀ,  dQ += dS K
 // With dS = P ∘ (dP·scale − delta·scale) the results need no further scaling; P is recomputed from lse2.
 // Optional RoPE backward (pb_flash_attn_bwd_rope): the inverse rotation is applied to dQ / dK in registers before the store.
+// Optional document masking of packed rows (kDoc, pb_flash_attn_{fwd,bwd}_doc with the bounds of pb_doc_bounds): key tiles that
+// lie before a query block's first document are skipped, not masked.
 #include "common.cuh"
 
 namespace {
@@ -106,10 +108,15 @@ struct AttnParams {
   int causal;
   const float* rope_cos;  // backward only: fp32 [S, D/2] tables of the forward rotation, nullptr = no RoPE
   const float* rope_sin;
+  const int* doc_start;  // kDoc kernels only: int32 [B, S] first position of the document holding s (pb_doc_bounds)
+  const int* doc_end;    //                     int32 [B, S] one past its last position
 };
 
 // ------------------------------------------------------------------------------------------------------------------ forward
-template <int D>
+// kDoc: document masking (always causal). Query q sees key k iff doc_start[b, q] <= k <= q. doc_start never decreases along a
+// row, so the key loop starts at the tile of doc_start[b, q0]; only tiles below doc_start[b, q0 + BQ - 1] and the diagonal tile
+// need a mask, the others take the plain path.
+template <int D, bool kDoc>
 __global__ void __launch_bounds__(kThreads) flash_fwd_kernel(const AttnParams p) {
   extern __shared__ __align__(128) uint8_t smem[];
   const int qb = (int)blockIdx.x, bh = (int)blockIdx.y;
@@ -123,9 +130,14 @@ __global__ void __launch_bounds__(kThreads) flash_fwd_kernel(const AttnParams p)
 
   const int q0 = qb * BQ;
   const int n_kv = p.causal ? qb + 1 : p.S / BKV;
+  // kDoc: first key tile, document start of the block's last row, document starts of this thread's two rows
+  const int* ds = kDoc ? p.doc_start + (int64_t)b * p.S : nullptr;
+  const int j0 = kDoc ? ds[q0] / BKV : 0;
+  const int ds_max = kDoc ? ds[q0 + BQ - 1] : 0;
+  const int rds[2] = {kDoc ? ds[q0 + warp * 16 + g] : 0, kDoc ? ds[q0 + warp * 16 + g + 8] : 0};
   load_tile<D>(sq, base + (int64_t)q0 * W + h * D, W, BQ);
-  load_tile<D>(skv, base + p.H * D + hk * D, W, BKV);
-  load_tile<D>(skv + kKV, base + (p.H + p.Hkv) * D + hk * D, W, BKV);
+  load_tile<D>(skv, base + (int64_t)j0 * BKV * W + p.H * D + hk * D, W, BKV);
+  load_tile<D>(skv + kKV, base + (int64_t)j0 * BKV * W + (p.H + p.Hkv) * D + hk * D, W, BKV);
   cp_async_commit();
 
   uint32_t qf[D / 16][4];
@@ -134,8 +146,8 @@ __global__ void __launch_bounds__(kThreads) flash_fwd_kernel(const AttnParams p)
   for (int i = 0; i < D / 8; ++i) o[i][0] = o[i][1] = o[i][2] = o[i][3] = 0.f;
   float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
 
-  for (int j = 0; j < n_kv; ++j) {
-    const int st = j & 1;
+  for (int j = j0; j < n_kv; ++j) {
+    const int st = (j - j0) & 1;
     if (j + 1 < n_kv) {  // prefetch the next key/value tile into the other stage
       const int k1 = (j + 1) * BKV;
       const uint32_t nxt = skv + (st ^ 1) * 2 * kKV;
@@ -145,7 +157,7 @@ __global__ void __launch_bounds__(kThreads) flash_fwd_kernel(const AttnParams p)
     cp_async_commit();
     cp_async_wait<1>();
     __syncthreads();
-    if (j == 0) {
+    if (j == j0) {
 #pragma unroll
       for (int kk = 0; kk < D / 16; ++kk) ld_a<D>(sq, warp * 16, kk * 16, qf[kk]);
     }
@@ -165,13 +177,19 @@ __global__ void __launch_bounds__(kThreads) flash_fwd_kernel(const AttnParams p)
     }
     // online softmax (log2 domain); rows g and g + 8 of this warp's 16
     const bool diag = p.causal && j == qb;
+    const bool edge = kDoc && (diag || j * BKV < ds_max);
     float mx[2] = {m[0], m[1]};
 #pragma unroll
     for (int n = 0; n < BKV / 8; ++n)
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
         float v = s[n][e] * p.scale_log2;
-        if (diag) {
+        if constexpr (kDoc) {
+          if (edge) {
+            const int qi = q0 + warp * 16 + g + (e >> 1) * 8, ki = j * BKV + n * 8 + 2 * t + (e & 1);
+            if (ki > qi || ki < rds[e >> 1]) v = -INFINITY;
+          }
+        } else if (diag) {
           const int qi = warp * 16 + g + (e >> 1) * 8, ki = n * 8 + 2 * t + (e & 1);
           if (ki > qi) v = -INFINITY;
         }
@@ -186,8 +204,16 @@ __global__ void __launch_bounds__(kThreads) flash_fwd_kernel(const AttnParams p)
     float corr[2], rs[2] = {0.f, 0.f};
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
-      corr[r] = fast_exp2(m[r] - mx[r]);  // m = -inf on the first tile → 0
-      m[r] = mx[r];
+      if constexpr (kDoc) {
+        // a row whose document starts later in the block can meet tiles in which every key is masked; while its maximum is
+        // still -inf, subtract 0 so that exp2 gives 0 instead of exp2(-inf - -inf) = NaN (m is reset to -inf below)
+        const float mref = mx[r] == -INFINITY ? 0.f : mx[r];
+        corr[r] = fast_exp2(m[r] - mref);
+        m[r] = mref;
+      } else {
+        corr[r] = fast_exp2(m[r] - mx[r]);  // m = -inf on the first tile → 0
+        m[r] = mx[r];
+      }
     }
     uint32_t pf[BKV / 16][4];
 #pragma unroll
@@ -201,6 +227,10 @@ __global__ void __launch_bounds__(kThreads) flash_fwd_kernel(const AttnParams p)
     }
 #pragma unroll
     for (int r = 0; r < 2; ++r) l[r] = l[r] * corr[r] + rs[r];
+    if constexpr (kDoc) {
+#pragma unroll
+      for (int r = 0; r < 2; ++r) m[r] = mx[r];
+    }
 #pragma unroll
     for (int i = 0; i < D / 8; ++i) {
       o[i][0] *= corr[0];
@@ -293,7 +323,9 @@ __device__ __forceinline__ void store_rows(__nv_bfloat16* dst, int64_t ld, int r
   }
 }
 
-template <int D>
+// kDoc: the query-tile loop stops at the tile holding doc_end[b, k0 + BKV - 1] (no later query sees a key of this block) and
+// Pᵀ is zero unless doc_start[q] <= key <= q; the tile's doc_start values are staged in shared memory after lse2 and delta.
+template <int D, bool kDoc>
 __global__ void __launch_bounds__(kThreads) bwd_dkdv_kernel(const AttnParams p) {
   extern __shared__ __align__(128) uint8_t smem[];
   const int kb = (int)blockIdx.x, bhk = (int)blockIdx.y;
@@ -305,6 +337,7 @@ __global__ void __launch_bounds__(kThreads) bwd_dkdv_kernel(const AttnParams p) 
   const uint32_t sk = smem_u32(smem), sv = sk + Tile<D>::bytes(BKV);
   const uint32_t sq = sv + Tile<D>::bytes(BKV), sdo = sq + Tile<D>::bytes(BQB);
   float* s_ld = reinterpret_cast<float*>(smem + 2 * Tile<D>::bytes(BKV) + 2 * Tile<D>::bytes(BQB));  // [lse2 BQB | delta BQB]
+  int* s_ds = reinterpret_cast<int*>(s_ld + 2 * BQB);  // kDoc: [doc_start BQB]
   const int k0 = kb * BKV;
   load_tile<D>(sk, base + (int64_t)k0 * W + (p.H + hk) * D, W, BKV);
   load_tile<D>(sv, base + (int64_t)k0 * W + (p.H + p.Hkv + hk) * D, W, BKV);
@@ -317,9 +350,10 @@ __global__ void __launch_bounds__(kThreads) bwd_dkdv_kernel(const AttnParams p) 
     for (int e = 0; e < 4; ++e) dk[i][e] = dv[i][e] = 0.f;
 
   const int qt0 = p.causal ? k0 / BQB : 0;
+  const int qt_doc = kDoc ? (p.doc_end[(int64_t)b * p.S + k0 + BKV - 1] + BQB - 1) / BQB : 0;
   for (int hh = 0; hh < grp; ++hh) {
     const int h = hk * grp + hh;
-    for (int qt = qt0; qt < p.S / BQB; ++qt) {
+    for (int qt = qt0; qt < (kDoc ? qt_doc : p.S / BQB); ++qt) {
       const int q0 = qt * BQB;
       __syncthreads();  // the previous tile has been consumed
       load_tile<D>(sq, base + (int64_t)q0 * W + h * D, W, BQB);
@@ -327,6 +361,9 @@ __global__ void __launch_bounds__(kThreads) bwd_dkdv_kernel(const AttnParams p) 
       cp_async_commit();
       if (threadIdx.x < BQB) s_ld[threadIdx.x] = p.lse2[((int64_t)b * p.H + h) * p.S + q0 + threadIdx.x];
       else if (threadIdx.x < 2 * BQB) s_ld[threadIdx.x] = p.delta[((int64_t)b * p.H + h) * p.S + q0 + threadIdx.x - BQB];
+      if constexpr (kDoc) {
+        if (threadIdx.x >= 2 * BQB && threadIdx.x < 3 * BQB) s_ds[threadIdx.x - 2 * BQB] = p.doc_start[(int64_t)b * p.S + q0 + threadIdx.x - 2 * BQB];
+      }
       cp_async_wait<0>();
       __syncthreads();
       // Sᵀ = K Qᵀ and dPᵀ = V dOᵀ: 16 keys (this warp) x BQB queries
@@ -360,7 +397,11 @@ __global__ void __launch_bounds__(kThreads) bwd_dkdv_kernel(const AttnParams p) 
         for (int e = 0; e < 4; ++e) {
           const int qi = n * 8 + 2 * t + (e & 1), ki = k0 + warp * 16 + g + (e >> 1) * 8;
           float pe = fast_exp2(st[n][e] * p.scale_log2 - s_ld[qi]);
-          if (p.causal && q0 + qi < ki) pe = 0.f;
+          if constexpr (kDoc) {
+            if (q0 + qi < ki || s_ds[qi] > ki) pe = 0.f;
+          } else if (p.causal && q0 + qi < ki) {
+            pe = 0.f;
+          }
           pv[e] = pe;
           dsv[e] = pe * (dpt[n][e] * p.scale - s_ld[BQB + qi]);
         }
@@ -390,7 +431,8 @@ __global__ void __launch_bounds__(kThreads) bwd_dkdv_kernel(const AttnParams p) 
   store_rows<D>(dst + (p.H + p.Hkv + hk) * D, W, k0 + warp * 16, k0 + warp * 16, dv, p, false);
 }
 
-template <int D>
+// kDoc: key tiles from doc_start[b, q0] / BKV to the diagonal, masks as in the forward
+template <int D, bool kDoc>
 __global__ void __launch_bounds__(kThreads) bwd_dq_kernel(const AttnParams p) {
   extern __shared__ __align__(128) uint8_t smem[];
   const int qb = (int)blockIdx.x, bh = (int)blockIdx.y;
@@ -415,8 +457,13 @@ __global__ void __launch_bounds__(kThreads) bwd_dq_kernel(const AttnParams p) {
 #pragma unroll
   for (int i = 0; i < D / 8; ++i) dq[i][0] = dq[i][1] = dq[i][2] = dq[i][3] = 0.f;
   const int n_kv = p.causal ? qb + 1 : p.S / BKV;
-  for (int j = 0; j < n_kv; ++j) {
+  const int* ds = kDoc ? p.doc_start + (int64_t)b * p.S : nullptr;
+  const int j0 = kDoc ? ds[q0] / BKV : 0;
+  const int ds_max = kDoc ? ds[q0 + BQ - 1] : 0;
+  const int rds[2] = {kDoc ? ds[q0 + warp * 16 + g] : 0, kDoc ? ds[q0 + warp * 16 + g + 8] : 0};
+  for (int j = j0; j < n_kv; ++j) {
     const int k0 = j * BKV;
+    const bool edge = kDoc && (j == qb || k0 < ds_max);
     __syncthreads();
     load_tile<D>(sk, base + (int64_t)k0 * W + (p.H + hk) * D, W, BKV);
     load_tile<D>(sv, base + (int64_t)k0 * W + (p.H + p.Hkv + hk) * D, W, BKV);
@@ -452,7 +499,11 @@ __global__ void __launch_bounds__(kThreads) bwd_dq_kernel(const AttnParams p) {
       for (int e = 0; e < 4; ++e) {
         const int r = e >> 1, qi = q0 + warp * 16 + g + r * 8, ki = k0 + n * 8 + 2 * t + (e & 1);
         float pe = fast_exp2(s[n][e] * p.scale_log2 - lse[r]);
-        if (p.causal && ki > qi) pe = 0.f;
+        if constexpr (kDoc) {
+          if (edge && (ki > qi || ki < rds[r])) pe = 0.f;
+        } else if (p.causal && ki > qi) {
+          pe = 0.f;
+        }
         dsv[e] = pe * (dp[n][e] * p.scale - del[r]);
       }
       da[n >> 1][(n & 1) * 2] = pack_bf16(dsv[0], dsv[1]);
@@ -479,41 +530,88 @@ int set_smem(K kernel, uint32_t bytes) {
   return e == cudaSuccess ? 0 : (int)e;
 }
 
-template <int D>
+template <int D, bool kDoc>
 int launch_fwd(const AttnParams& p, cudaStream_t stream) {
   constexpr uint32_t kSmem = Tile<D>::bytes(BQ) + 4 * Tile<D>::bytes(BKV);
-  static int rc = set_smem(flash_fwd_kernel<D>, kSmem);
+  static int rc = set_smem(flash_fwd_kernel<D, kDoc>, kSmem);
   if (rc) return rc;
-  flash_fwd_kernel<D><<<dim3(p.S / BQ, p.B * p.H), kThreads, kSmem, stream>>>(p);
+  flash_fwd_kernel<D, kDoc><<<dim3(p.S / BQ, p.B * p.H), kThreads, kSmem, stream>>>(p);
   PB_CHECK_LAUNCH();
   return 0;
 }
 
-template <int D>
+template <int D, bool kDoc>
 int launch_bwd(const AttnParams& p, cudaStream_t stream) {
   const int64_t tokens = (int64_t)p.B * p.S;
   const int64_t blocks = (tokens * 32 + 255) / 256;
   bwd_delta_kernel<<<(unsigned)blocks, 256, 0, stream>>>((const pb::bf16x8*)p.dout, (const pb::bf16x8*)p.out, const_cast<float*>(p.delta),
                                                          tokens, p.S, p.H, D / 8, p.scale);
   PB_CHECK_LAUNCH();
-  constexpr uint32_t kDkv = 2 * Tile<D>::bytes(BKV) + 2 * Tile<D>::bytes(BQB) + 2 * BQB * 4;
+  constexpr uint32_t kDkv = 2 * Tile<D>::bytes(BKV) + 2 * Tile<D>::bytes(BQB) + (kDoc ? 3 : 2) * BQB * 4;
   constexpr uint32_t kDq = 2 * Tile<D>::bytes(BQ) + 2 * Tile<D>::bytes(BKV);
-  static int rc = set_smem(bwd_dkdv_kernel<D>, kDkv) | set_smem(bwd_dq_kernel<D>, kDq);
+  static int rc = set_smem(bwd_dkdv_kernel<D, kDoc>, kDkv) | set_smem(bwd_dq_kernel<D, kDoc>, kDq);
   if (rc) return rc;
-  bwd_dkdv_kernel<D><<<dim3(p.S / BKV, p.B * p.Hkv), kThreads, kDkv, stream>>>(p);
-  bwd_dq_kernel<D><<<dim3(p.S / BQ, p.B * p.H), kThreads, kDq, stream>>>(p);
+  bwd_dkdv_kernel<D, kDoc><<<dim3(p.S / BKV, p.B * p.Hkv), kThreads, kDkv, stream>>>(p);
+  bwd_dq_kernel<D, kDoc><<<dim3(p.S / BQ, p.B * p.H), kThreads, kDq, stream>>>(p);
   PB_CHECK_LAUNCH();
   return 0;
 }
 
 int bwd(const void* qkv, const void* out, const void* dout, const float* lse2, float* delta, void* dqkv, int B, int S, int H, int Hkv,
-        int D, float scale, int causal, const float* rope_cos, const float* rope_sin, cudaStream_t stream) {
+        int D, float scale, int causal, const float* rope_cos, const float* rope_sin, const int* doc_start, const int* doc_end,
+        cudaStream_t stream) {
   if (S % 128 != 0 || H % Hkv != 0) return -1;
   AttnParams p{(const __nv_bfloat16*)qkv, (__nv_bfloat16*)out, (const __nv_bfloat16*)dout, (__nv_bfloat16*)dqkv, lse2, delta, nullptr,
-               B, S, H, Hkv, scale, scale * 1.4426950408889634f, causal, rope_cos, rope_sin};
-  if (D == 128) return launch_bwd<128>(p, stream);
-  if (D == 64) return launch_bwd<64>(p, stream);
+               B, S, H, Hkv, scale, scale * 1.4426950408889634f, causal, rope_cos, rope_sin, doc_start, doc_end};
+  if (doc_start != nullptr) {
+    if (D == 128) return launch_bwd<128, true>(p, stream);
+    if (D == 64) return launch_bwd<64, true>(p, stream);
+    return -2;
+  }
+  if (D == 128) return launch_bwd<128, false>(p, stream);
+  if (D == 64) return launch_bwd<64, false>(p, stream);
   return -2;
+}
+
+// Document bounds of packed rows: one CTA per row. Every thread owns a contiguous run of positions; a block-wide exclusive
+// max-scan of the last document start per run (and min-scan, from the right, of the first EOS end) gives each run its carry-in.
+constexpr int kBoundsThreads = 256;
+__global__ void __launch_bounds__(kBoundsThreads) doc_bounds_kernel(const int64_t* __restrict__ tokens, int S, int64_t eos,
+                                                                    int* __restrict__ doc_start, int* __restrict__ doc_end) {
+  constexpr int kWarps = kBoundsThreads / 32;
+  __shared__ int s_lo[kWarps], s_hi[kWarps];
+  const int64_t row = (int64_t)blockIdx.x * S;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int per = (S + kBoundsThreads - 1) / kBoundsThreads;
+  const int s0 = min(S, (int)threadIdx.x * per), s1 = min(S, s0 + per);
+  int lo = 0, hi = S;  // last document start in [s0, s1), first end (EOS position + 1) in [s0, s1)
+  for (int s = s0; s < s1; ++s)
+    if (s > 0 && tokens[row + s - 1] == eos) lo = s;
+  for (int s = s1 - 1; s >= s0; --s)
+    if (tokens[row + s] == eos) hi = s + 1;
+  int in_lo = lo, in_hi = hi;  // inclusive warp scans: max from the left, min from the right
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int a = __shfl_up_sync(0xffffffffu, in_lo, o), c = __shfl_down_sync(0xffffffffu, in_hi, o);
+    if (lane >= o) in_lo = max(in_lo, a);
+    if (lane + o < 32) in_hi = min(in_hi, c);
+  }
+  if (lane == 31) s_lo[warp] = in_lo;
+  if (lane == 0) s_hi[warp] = in_hi;
+  __syncthreads();
+  int cur_lo = __shfl_up_sync(0xffffffffu, in_lo, 1), cur_hi = __shfl_down_sync(0xffffffffu, in_hi, 1);
+  if (lane == 0) cur_lo = 0;
+  if (lane == 31) cur_hi = S;
+  for (int w = 0; w < warp; ++w) cur_lo = max(cur_lo, s_lo[w]);
+  for (int w = warp + 1; w < kWarps; ++w) cur_hi = min(cur_hi, s_hi[w]);
+  for (int s = s0; s < s1; ++s) {
+    if (s > 0 && tokens[row + s - 1] == eos) cur_lo = s;
+    doc_start[row + s] = cur_lo;
+  }
+  for (int s = s1 - 1; s >= s0; --s) {
+    if (tokens[row + s] == eos) cur_hi = s + 1;
+    doc_end[row + s] = cur_hi;
+  }
 }
 
 int g_fwd_variant = -1;
@@ -539,21 +637,49 @@ PB_EXPORT int pb_flash_attn_fwd(const void* qkv, void* out, float* lse2, int B, 
                                 int causal, cudaStream_t stream) {
   if (S % 128 != 0 || H % Hkv != 0) return -1;
   AttnParams p{(const __nv_bfloat16*)qkv, (__nv_bfloat16*)out, nullptr, nullptr, nullptr, nullptr, lse2,
-               B, S, H, Hkv, scale, scale * 1.4426950408889634f, causal, nullptr, nullptr};
-  if (D == 128) return launch_fwd<128>(p, stream);
-  if (D == 64) return launch_fwd<64>(p, stream);
+               B, S, H, Hkv, scale, scale * 1.4426950408889634f, causal, nullptr, nullptr, nullptr, nullptr};
+  if (D == 128) return launch_fwd<128, false>(p, stream);
+  if (D == 64) return launch_fwd<64, false>(p, stream);
   return -2;
 }
 
 // delta: [B, H, S] fp32 scratch.  dqkv: [B, S, (H+2Hkv)·D] bf16, fully overwritten.
 PB_EXPORT int pb_flash_attn_bwd(const void* qkv, const void* out, const void* dout, const float* lse2, float* delta, void* dqkv,
                                 int B, int S, int H, int Hkv, int D, float scale, int causal, cudaStream_t stream) {
-  return bwd(qkv, out, dout, lse2, delta, dqkv, B, S, H, Hkv, D, scale, causal, nullptr, nullptr, stream);
+  return bwd(qkv, out, dout, lse2, delta, dqkv, B, S, H, Hkv, D, scale, causal, nullptr, nullptr, nullptr, nullptr, stream);
 }
 
 // Same, with the RoPE backward fused into the dQ / dK stores (cos/sin: fp32 [S, D/2] tables of the forward rotation).
 PB_EXPORT int pb_flash_attn_bwd_rope(const void* qkv, const void* out, const void* dout, const float* lse2, float* delta, void* dqkv,
                                      int B, int S, int H, int Hkv, int D, float scale, int causal, const float* rope_cos,
                                      const float* rope_sin, cudaStream_t stream) {
-  return bwd(qkv, out, dout, lse2, delta, dqkv, B, S, H, Hkv, D, scale, causal, rope_cos, rope_sin, stream);
+  return bwd(qkv, out, dout, lse2, delta, dqkv, B, S, H, Hkv, D, scale, causal, rope_cos, rope_sin, nullptr, nullptr, stream);
+}
+
+// tokens int64 [B, S] → doc_start, doc_end int32 [B, S]: position s starts a document when s == 0 or tokens[b, s-1] == eos;
+// doc_start = first position of the document holding s, doc_end = one past its last position (after its EOS, or S).
+PB_EXPORT int pb_doc_bounds(const int64_t* tokens, int B, int S, int64_t eos, int* doc_start, int* doc_end, cudaStream_t stream) {
+  if (B <= 0 || S <= 0) return -1;
+  doc_bounds_kernel<<<B, kBoundsThreads, 0, stream>>>(tokens, S, eos, doc_start, doc_end);
+  PB_CHECK_LAUNCH();
+  return 0;
+}
+
+// Document-masked (always causal) forward: query q attends key k iff doc_start[b, q] <= k <= q.  doc_start: int32 [B, S].
+PB_EXPORT int pb_flash_attn_fwd_doc(const void* qkv, void* out, float* lse2, const int* doc_start, int B, int S, int H, int Hkv, int D,
+                                    float scale, cudaStream_t stream) {
+  if (S % 128 != 0 || H % Hkv != 0 || doc_start == nullptr) return -1;
+  AttnParams p{(const __nv_bfloat16*)qkv, (__nv_bfloat16*)out, nullptr, nullptr, nullptr, nullptr, lse2,
+               B, S, H, Hkv, scale, scale * 1.4426950408889634f, 1, nullptr, nullptr, doc_start, nullptr};
+  if (D == 128) return launch_fwd<128, true>(p, stream);
+  if (D == 64) return launch_fwd<64, true>(p, stream);
+  return -2;
+}
+
+// Document-masked backward; rope_cos / rope_sin may be null (plain backward) or the forward's tables (fused RoPE backward).
+PB_EXPORT int pb_flash_attn_bwd_doc(const void* qkv, const void* out, const void* dout, const float* lse2, float* delta, void* dqkv,
+                                    const int* doc_start, const int* doc_end, int B, int S, int H, int Hkv, int D, float scale,
+                                    const float* rope_cos, const float* rope_sin, cudaStream_t stream) {
+  if (doc_start == nullptr || doc_end == nullptr) return -1;
+  return bwd(qkv, out, dout, lse2, delta, dqkv, B, S, H, Hkv, D, scale, 1, rope_cos, rope_sin, doc_start, doc_end, stream);
 }

@@ -262,6 +262,33 @@ class PinnedPrefetcher:
         return Batch(t[0], t[1])
 
 
+def eos_id_from_meta(paths: str) -> int | None:
+    """EOS id recorded in the ``.meta.json`` sidecar of the first token file of ``paths`` (None without a sidecar or an id)."""
+    import json
+
+    meta = _expand_paths(paths)[0].with_suffix(".meta.json")
+    if not meta.exists():
+        return None
+    eos = json.loads(meta.read_text()).get("eos_id")
+    return None if eos is None else int(eos)
+
+
+def document_eos_id(cfg_data) -> int | None:
+    """EOS id for document masking (``data.document_mask``): ``data.eos_id``, else the first shard's sidecar; None when masking is
+    off. Raises ``ValueError`` when masking is on and no EOS id can be found."""
+    if not cfg_data.document_mask:
+        return None
+    if cfg_data.eos_id is not None:
+        return int(cfg_data.eos_id)
+    if cfg_data.fake or not cfg_data.dataset_name_or_paths:
+        raise ValueError("data.document_mask=true with synthetic data needs an explicit data.eos_id")
+    eos = eos_id_from_meta(cfg_data.dataset_name_or_paths)
+    if eos is None:
+        raise ValueError(f"data.document_mask=true: no eos_id in the .meta.json of the first shard of {cfg_data.dataset_name_or_paths!r} "
+                         "(tools/tokenize_corpus.py writes it); set data.eos_id")  # fmt: skip
+    return eos
+
+
 def build_dataset(cfg_data, vocab_size: int, rank: int, world: int):
     if cfg_data.fake or not cfg_data.dataset_name_or_paths:
         return FakeTokenDataset(vocab_size, cfg_data.seq_length, cfg_data.seed, rank, world)

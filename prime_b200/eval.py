@@ -2,6 +2,7 @@
 
     python -m prime_b200.eval ppl --ckpt runs/x/ckpt/step_001000 --model 1B --data data/c4_val --seq 1024 --batches 50
     python -m prime_b200.eval ppl --hf path/to/llama --data data/c4_val
+    python -m prime_b200.eval ppl --ckpt … --model 1B --data data/c4_val --document-mask   # attention within documents only
     python -m prime_b200.eval generate --ckpt … --model 1B --prompt-ids 1,306,626 --max-new 32
 
 The model is rebuilt on one device from the per-rank optimizer shards (``checkpoint.assemble_full_model``) or from a Hugging
@@ -96,6 +97,10 @@ def main(argv: list[str] | None = None) -> dict:
     p.add_argument("--seq", type=int, default=1024)
     p.add_argument("--batches", type=int, default=20)
     p.add_argument("--batch-size", type=int, default=8)
+    p.add_argument("--document-mask", action="store_true",
+                   help="document-masked attention: a token attends only to earlier tokens of its own document (EOS id from the "
+                        "first shard's .meta.json unless --eos-id is given)")  # fmt: skip
+    p.add_argument("--eos-id", type=int, default=None, help="EOS id that ends a document; implies --document-mask")
     g = sub.choices["generate"]
     g.add_argument("--prompt-ids", required=True, help="comma-separated token ids")
     g.add_argument("--max-new", type=int, default=32)
@@ -105,6 +110,13 @@ def main(argv: list[str] | None = None) -> dict:
     a = ap.parse_args(argv)
     model = load_model(a, a.device)
     if a.cmd == "ppl":
+        if a.document_mask or a.eos_id is not None:
+            from .data import eos_id_from_meta
+
+            eos = a.eos_id if a.eos_id is not None else eos_id_from_meta(a.data)
+            if eos is None:
+                raise SystemExit(f"--document-mask: no eos_id in the .meta.json of the first shard of {a.data!r}; pass --eos-id")
+            model.doc_eos_id = eos
         ds = MemmapTokenDataset(a.data, a.seq, vocab_size=model.args.vocab_size, shuffle=False)
         out = perplexity(model, ds, batches=min(a.batches, max(1, ds.windows // a.batch_size)), batch_size=a.batch_size, device=a.device)
     else:

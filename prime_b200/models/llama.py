@@ -105,20 +105,21 @@ class Attention(nn.Module):
         self.wo = nn.Parameter(torch.empty(args.dim, self.n_heads * self.head_dim))
         self.fp8 = False  # train.fp8: MXFP8 forward / input-gradient GEMMs (Transformer.set_fp8)
 
-    def forward(self, x: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor, attn_impl: str = "auto") -> torch.Tensor:
+    def forward(self, x: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor, attn_impl: str = "auto", doc: tuple | None = None) -> torch.Tensor:
+        """``doc``: (doc_start, doc_end) of ``ops.document_bounds`` for document-masked attention, None = plain causal."""
         B, S, _ = x.shape
         H, Hkv, D = self.n_heads, self.n_kv_heads, self.head_dim
         if self.fp8:
             qkv = ops.linear_mxfp8(x, self.wqkv)
-            out = ops.rope_attention_qkv(qkv, cos, sin, H, Hkv, causal=True, impl=attn_impl)
+            out = ops.rope_attention_qkv(qkv, cos, sin, H, Hkv, causal=True, impl=attn_impl, doc=doc)
             return ops.linear_mxfp8(out, self.wo)
         if attn_impl in ("auto", "native") and ops.rope_fusable(x, H, Hkv, D):
             # RoPE rides in the QKV GEMM epilogue (forward) and in the dQ/dK epilogues of the attention backward: no rotation pass
             qkv = ops.linear_qkv_rope(x, self.wqkv, cos, sin, H, Hkv)  # [B, S, (H+2Hkv)·D], Q/K heads rotated
-            out = ops.rope_attention_qkv(qkv, cos, sin, H, Hkv, causal=True, impl=attn_impl, pre_rotated=True)
+            out = ops.rope_attention_qkv(qkv, cos, sin, H, Hkv, causal=True, impl=attn_impl, pre_rotated=True, doc=doc)
         else:
             qkv = ops.linear(x, self.wqkv)  # [B, S, (H+2Hkv)·D]
-            out = ops.rope_attention_qkv(qkv, cos, sin, H, Hkv, causal=True, impl=attn_impl)  # [B, S, H·D], no layout shuffles
+            out = ops.rope_attention_qkv(qkv, cos, sin, H, Hkv, causal=True, impl=attn_impl, doc=doc)  # [B, S, H·D], no layout shuffles
         return ops.linear(out, self.wo)
 
 
@@ -147,13 +148,13 @@ class TransformerBlock(nn.Module):
         self.eps = args.norm_eps
         self.init_std = 0.02 / math.sqrt(2 * (layer_id + 1)) if args.depth_init else 0.02 / math.sqrt(2 * args.n_layers)
 
-    def forward(self, h: torch.Tensor, delta: torch.Tensor | None, cos, sin, attn_impl: str = "auto"):
-        """``h`` = residual stream, ``delta`` = output of the previous sub-block not yet added."""
+    def forward(self, h: torch.Tensor, delta: torch.Tensor | None, cos, sin, attn_impl: str = "auto", doc: tuple | None = None):
+        """``h`` = residual stream, ``delta`` = output of the previous sub-block not yet added, ``doc`` = document bounds or None."""
         if delta is None:
             x = ops.rmsnorm(h, self.attention_norm.weight, self.eps)
         else:
             x, h = ops.add_rmsnorm(delta, h, self.attention_norm.weight, self.eps)
-        a = self.attention(x, cos, sin, attn_impl)
+        a = self.attention(x, cos, sin, attn_impl, doc)
         y, h = ops.add_rmsnorm(a, h, self.ffn_norm.weight, self.eps)
         return h, self.feed_forward(y)
 
@@ -176,6 +177,9 @@ class Transformer(nn.Module):
         self.output = nn.Parameter(torch.empty(args.vocab_size, args.dim))
         self.ac_ckpt: bool | int = False  # True = every block, n = every n-th block (train.ac_ckpt)
         self.attn_impl = "auto"
+        # document masking of packed rows (data.document_mask): a token attends only to earlier tokens of its own document, where a
+        # document ends with this EOS id. None = plain causal attention
+        self.doc_eos_id: int | None = None
         self._rope: tuple[torch.Tensor, torch.Tensor] | None = None
 
     # ------------------------------------------------------------------ init
@@ -210,6 +214,8 @@ class Transformer(nn.Module):
         B, S = tokens.shape
         cos, sin = self.rope_tables(S, tokens.device)
         h = ops.embedding(tokens, self.tok_embeddings.weight)
+        # computed once per micro-batch, read by every layer
+        doc = ops.document_bounds(tokens, self.doc_eos_id) if self.doc_eos_id is not None else None
         delta = None
         ac = self.ac_ckpt if torch.is_grad_enabled() else False
         for i, layer in enumerate(self.layers):
@@ -218,9 +224,9 @@ class Transformer(nn.Module):
                 # the block (RoPE on the QKV GEMM output) act on tensors the block itself creates, so replaying it is safe.
                 from torch.utils.checkpoint import checkpoint
 
-                h, delta = checkpoint(layer, h, delta, cos, sin, self.attn_impl, use_reentrant=False)
+                h, delta = checkpoint(layer, h, delta, cos, sin, self.attn_impl, doc, use_reentrant=False)
             else:
-                h, delta = layer(h, delta, cos, sin, self.attn_impl)
+                h, delta = layer(h, delta, cos, sin, self.attn_impl, doc)
         x, _ = ops.add_rmsnorm(delta, h, self.norm.weight, self.args.norm_eps)
         return x
 

@@ -157,6 +157,9 @@ def _declare(lib: ctypes.CDLL) -> None:
         "pb_flash_attn_bwd_set_variant": [i32],
         "pb_flash_attn_fwd_set_variant": [i32],
         "pb_flash_attn_bwd_rope": [vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, f32, i32, vp, vp, vp],
+        "pb_doc_bounds": [vp, i32, i32, i64, vp, vp, vp],
+        "pb_flash_attn_fwd_doc": [vp, vp, vp, vp, i32, i32, i32, i32, i32, f32, vp],
+        "pb_flash_attn_bwd_doc": [vp, vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, f32, vp, vp, vp],
         "pb_ipc_alloc": [ctypes.POINTER(vp), ctypes.c_size_t],
         "pb_ipc_free": [vp],
         "pb_ipc_handle_size": [],

@@ -869,25 +869,44 @@ def cross_entropy(
 # --------------------------------------------------------------------------- attention
 
 
-def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, causal: bool = True) -> torch.Tensor:
+def document_bounds(tokens: torch.Tensor, eos_id: int) -> tuple[torch.Tensor, torch.Tensor]:
+    """Documents of packed token rows [B, S] → (doc_start, doc_end), int32 [B, S] each: the ``doc`` argument of the attention ops.
+    Position s starts a document when s == 0 or tokens[b, s-1] == eos_id. One native kernel on CUDA; it reads only ``tokens``, so
+    it can be captured in a CUDA graph over a static token buffer."""
+    if tokens.is_cuda:
+        from . import attention_native as native
+
+        return native.document_bounds(tokens, eos_id)
+    return reference.document_bounds(tokens, eos_id)
+
+
+def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, causal: bool = True, doc: tuple | None = None) -> torch.Tensor:
     """Unfused-layout attention, q [B,S,H,D], k/v [B,S,Hkv,D] → [B,S,H,D].  SDPA on CUDA (not a hot path: the models
-    call :func:`attention_qkv`), torch reference on CPU."""
+    call :func:`attention_qkv`), torch reference on CPU. ``doc=(doc_start, doc_end)`` (:func:`document_bounds`): query q attends
+    key k iff doc_start[b, q] <= k <= q; on CUDA this builds a boolean [B, 1, S, S] mask (O(S²) memory)."""
+    if doc is not None and not causal:
+        raise ValueError("document masking implies causal attention: causal=False with doc=(doc_start, doc_end) is not supported")
     if not q.is_cuda:
-        return reference.attention(q, k, v, causal)
+        return reference.attention(q, k, v, causal, doc_start=None if doc is None else doc[0])
     import torch.nn.functional as F
 
     H, Hkv = q.shape[2], k.shape[2]
+    if doc is not None:
+        out = F.scaled_dot_product_attention(q.transpose(1, 2), k.transpose(1, 2), v.transpose(1, 2),
+                                             attn_mask=reference.document_mask(doc[0]).unsqueeze(1), enable_gqa=(H != Hkv))  # fmt: skip
+        return out.transpose(1, 2)
     out = F.scaled_dot_product_attention(
         q.transpose(1, 2), k.transpose(1, 2), v.transpose(1, 2), is_causal=causal, enable_gqa=(H != Hkv)
     )
     return out.transpose(1, 2)
 
 
-def attention_qkv(qkv: torch.Tensor, n_heads: int, n_kv_heads: int, causal: bool = True, impl: str = "auto") -> torch.Tensor:
+def attention_qkv(qkv: torch.Tensor, n_heads: int, n_kv_heads: int, causal: bool = True, impl: str = "auto",
+                  doc: tuple | None = None) -> torch.Tensor:  # fmt: skip
     """Attention over the fused, RoPE-rotated QKV activation [B,S,(H+2Hkv)·D] → [B,S,H·D].
 
     ``impl``: "native" = the project's flash-attention kernels (error if the shape is unsupported); "sdpa" = library
-    fallback; "auto" = native whenever supported.
+    fallback; "auto" = native whenever supported. ``doc=(doc_start, doc_end)`` (:func:`document_bounds`): document masking.
     """
     B, S, W = qkv.shape
     D = W // (n_heads + 2 * n_kv_heads)
@@ -895,24 +914,25 @@ def attention_qkv(qkv: torch.Tensor, n_heads: int, n_kv_heads: int, causal: bool
         from . import attention_native as native
 
         if native.supported(qkv, n_heads, n_kv_heads):
-            return native.flash_attention_qkv(qkv, n_heads, n_kv_heads, causal)
+            return native.flash_attention_qkv(qkv, n_heads, n_kv_heads, causal, doc)
         if impl == "native":
             raise RuntimeError(f"native flash attention does not support S={S}, D={D}, H={n_heads}, Hkv={n_kv_heads}")
     x = qkv.view(B, S, n_heads + 2 * n_kv_heads, D)
     q, k, v = x[:, :, :n_heads], x[:, :, n_heads : n_heads + n_kv_heads], x[:, :, n_heads + n_kv_heads :]
-    return attention(q, k, v, causal).reshape(B, S, n_heads * D)
+    return attention(q, k, v, causal, doc).reshape(B, S, n_heads * D)
 
 
 def rope_attention_qkv(qkv: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor, n_heads: int, n_kv_heads: int, causal: bool = True,
-                       impl: str = "auto", pre_rotated: bool = False) -> torch.Tensor:  # fmt: skip
+                       impl: str = "auto", pre_rotated: bool = False, doc: tuple | None = None) -> torch.Tensor:  # fmt: skip
     """RoPE on the Q/K heads of the fused QKV activation followed by attention → [B,S,H·D]. On the native path both run as one
     autograd node whose backward folds the inverse rotation into the dQ/dK epilogues. ``pre_rotated=True``: the producer
-    (:func:`linear_qkv_rope`) already rotated in its GEMM epilogue; only the backward un-rotation is needed (native path only)."""
+    (:func:`linear_qkv_rope`) already rotated in its GEMM epilogue; only the backward un-rotation is needed (native path only).
+    ``doc=(doc_start, doc_end)``: document masking (see :func:`attention`); RoPE positions stay absolute."""
     if qkv.is_cuda and impl in ("auto", "native"):
         from . import attention_native as native
 
         if native.supported(qkv, n_heads, n_kv_heads):
-            return native.rope_flash_attention_qkv(qkv, cos, sin, n_heads, n_kv_heads, causal, pre_rotated)
+            return native.rope_flash_attention_qkv(qkv, cos, sin, n_heads, n_kv_heads, causal, pre_rotated, doc)
     if pre_rotated:
         raise RuntimeError("pre_rotated=True needs the native attention path (its backward undoes the rotation)")
-    return attention_qkv(rope_qkv(qkv, cos, sin, n_heads, n_kv_heads), n_heads, n_kv_heads, causal, impl)
+    return attention_qkv(rope_qkv(qkv, cos, sin, n_heads, n_kv_heads), n_heads, n_kv_heads, causal, impl, doc)

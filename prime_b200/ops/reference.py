@@ -56,8 +56,31 @@ def swiglu(gate_up: torch.Tensor) -> torch.Tensor:
     return (F.silu(g) * u).to(gate_up.dtype)
 
 
-def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, causal: bool = True) -> torch.Tensor:
-    """q: [B, S, H, D]; k/v: [B, S, Hkv, D] → [B, S, H, D]."""
+def document_bounds(tokens: torch.Tensor, eos_id: int) -> tuple[torch.Tensor, torch.Tensor]:
+    """Documents of packed rows, tokens [B, S] → (doc_start, doc_end) int32 [B, S].
+
+    Position s starts a document when s == 0 or tokens[b, s-1] == eos_id (the EOS belongs to the document it ends).
+    ``doc_start[b, s]`` is the first position of the document holding s, ``doc_end[b, s]`` one past its last position."""
+    B, S = tokens.shape
+    is_eos = tokens == eos_id
+    starts = torch.zeros((B, S), dtype=torch.bool, device=tokens.device)
+    starts[:, 0] = True
+    starts[:, 1:] = is_eos[:, :-1]
+    pos = torch.arange(S, device=tokens.device).expand(B, S)
+    doc_start = torch.where(starts, pos, 0).cummax(1).values  # latest start at or before s
+    doc_end = torch.where(is_eos, pos + 1, S).flip(1).cummin(1).values.flip(1)  # first EOS at or after s, plus one
+    return doc_start.int(), doc_end.int()
+
+
+def document_mask(doc_start: torch.Tensor) -> torch.Tensor:
+    """Boolean [B, S, S] mask of document-masked causal attention: query q sees key k iff doc_start[b, q] <= k <= q."""
+    B, S = doc_start.shape
+    k = torch.arange(S, device=doc_start.device)
+    return (k.view(1, 1, S) <= k.view(1, S, 1)) & (k.view(1, 1, S) >= doc_start.long().view(B, S, 1))
+
+
+def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, causal: bool = True, doc_start: torch.Tensor | None = None) -> torch.Tensor:
+    """q: [B, S, H, D]; k/v: [B, S, Hkv, D] → [B, S, H, D].  ``doc_start`` [B, S]: document masking (implies causal)."""
     B, S, H, D = q.shape
     Hkv = k.shape[2]
     qf, kf, vf = (t.float().transpose(1, 2) for t in (q, k, v))
@@ -65,7 +88,11 @@ def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, causal: bool = 
         kf = kf.repeat_interleave(H // Hkv, dim=1)
         vf = vf.repeat_interleave(H // Hkv, dim=1)
     scores = qf @ kf.transpose(-1, -2) / math.sqrt(D)
-    if causal:
+    if doc_start is not None:
+        if not causal:
+            raise ValueError("document masking implies causal attention")
+        scores = scores.masked_fill(~document_mask(doc_start).unsqueeze(1), float("-inf"))
+    elif causal:
         mask = torch.ones(S, S, dtype=torch.bool, device=q.device).tril()
         scores = scores.masked_fill(~mask, float("-inf"))
     out = scores.softmax(-1) @ vf

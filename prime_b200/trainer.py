@@ -15,7 +15,7 @@ import torch
 import torch.distributed as dist
 
 from .config import Config
-from .data import Batch, PinnedPrefetcher, build_dataset
+from .data import Batch, PinnedPrefetcher, build_dataset, document_eos_id
 from .models.llama import Transformer, build_model
 from .optim.schedule import lr_at
 from .parallel.diloco import DilocoOuter, OuterHyper
@@ -48,6 +48,7 @@ class Trainer:
         cuda = self.device.type == "cuda"
         torch.manual_seed(cfg.seed)
         dtype = torch.bfloat16 if cuda else torch.float32
+        doc_eos_id = document_eos_id(cfg.data)  # before any allocation: a missing EOS id is a configuration error
         overrides = dict(model_overrides or {})
         overrides.setdefault("max_seq_len", max(cfg.data.seq_length, 128))
         self.memory_plan = self._plan_memory(cfg, mesh, overrides) if cuda else None  # refuse what cannot fit BEFORE allocating
@@ -56,6 +57,8 @@ class Trainer:
         if cfg.train.init_weights:
             load_initial_weights(self.model, cfg.train.init_weights)  # before the engine takes the parameters into its buffers
         self.model.attn_impl = cfg.train.attn_impl
+        # document masking: the bounds kernel reads the token buffer inside the forward, so a captured micro-step stays valid
+        self.model.doc_eos_id = doc_eos_id
         self.model.ac_ckpt = cfg.train.ac_ckpt
         self.model.set_fp8(cfg.train.fp8)  # MXFP8 forward / dgrad GEMMs (opt-in; the headline benchmark is bf16)
         self.heap = None

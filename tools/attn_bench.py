@@ -1,5 +1,12 @@
-"""Time the native flash-attention (fwd, bwd) against SDPA/cuDNN on the Llama shapes. CUDA events, median."""
+"""Time the native flash-attention (fwd, bwd) against SDPA/cuDNN on the Llama shapes. CUDA events, median.
 
+    python tools/attn_bench.py                                         # the default Llama shapes
+    python tools/attn_bench.py --shape 4,4096,16,16,128 --doc-len 256  # + document-masked kernels, 256-token documents
+
+``--doc-len N`` packs every row with documents of N tokens (EOS every N positions) and also times the document-masked kernels
+(``native_doc_*``) in the same process, so masked and plain causal attention are compared on one shape in one invocation."""
+
+import argparse
 import json
 import sys
 from pathlib import Path
@@ -30,6 +37,15 @@ def timeit(fn, iters=10, warm=3, flush=None):
 
 
 def main():
+    ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
+    ap.add_argument("--shape", action="append", default=None, metavar="B,S,H,Hkv,D", help="shape to time (repeatable); default: Llama shapes")
+    ap.add_argument("--doc-len", type=int, default=0, help="also time document-masked attention with documents of this many tokens")
+    a = ap.parse_args()
+    shapes = [("1B mb16", 16, 1024, 16, 16, 128), ("7B-like", 8, 2048, 32, 32, 128), ("150M", 16, 1024, 16, 16, 64)]
+    if a.shape:
+        shapes = [(s, *map(int, s.split(","))) for s in a.shape]
+    from prime_b200 import ops
+
     dev = torch.device("cuda", 0)
     flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
     from prime_b200.utils.clocks import ClockSampler
@@ -37,7 +53,7 @@ def main():
     sampler = ClockSampler(0, period_s=0.05)
     sampler.start()
     rows = []
-    for name, B, S, H, Hkv, D in [("1B mb16", 16, 1024, 16, 16, 128), ("7B-like", 8, 2048, 32, 32, 128), ("150M", 16, 1024, 16, 16, 64)]:
+    for name, B, S, H, Hkv, D in shapes:
         W = (H + 2 * Hkv) * D
         qkv = (torch.randn(B, S, W, device=dev) * 0.5).to(torch.bfloat16).requires_grad_(True)
         out = A.flash_attention_qkv(qkv, H, Hkv, True)
@@ -69,6 +85,19 @@ def main():
                      "native_bwd_ms": round(both - fwd, 4), "sdpa_bwd_ms": round(rboth - rfwd, 4),
                      "native_bwd_tflops_algorithmic": round(2.5 * fl_f / (both - fwd) / 1e9, 1),
                      "sdpa_bwd_tflops": round(2.5 * fl_f / (rboth - rfwd) / 1e9, 1)})  # fmt: skip
+        if a.doc_len:
+            tok = torch.full((B, S), 1, dtype=torch.int64, device=dev)
+            tok[:, a.doc_len - 1 :: a.doc_len] = 0  # EOS (id 0) ends every document
+            doc = ops.document_bounds(tok, 0)
+            dfwd = timeit(lambda: A.flash_attention_qkv(qkv, H, Hkv, True, doc), flush=flush)
+
+            def dfb():
+                qkv.grad = None
+                A.flash_attention_qkv(qkv, H, Hkv, True, doc).backward(dout)
+
+            dboth = timeit(dfb, flush=flush)
+            rows[-1].update({"doc_len": a.doc_len, "native_doc_fwd_ms": round(dfwd, 4), "native_doc_bwd_ms": round(dboth - dfwd, 4),
+                             "doc_fwd_speedup": round(fwd / dfwd, 2), "doc_bwd_speedup": round((both - fwd) / (dboth - dfwd), 2)})  # fmt: skip
         print(rows[-1], flush=True)
     (ROOT / "gpurun_out").mkdir(exist_ok=True)
     (ROOT / "gpurun_out" / "attn_bench.json").write_text(json.dumps({"rows": rows, "clocks": sampler.finish(),

@@ -36,9 +36,14 @@ PICK = [
     (r"gemm_bf16_kernel<0, 0, 2, 3>", "gemm_param_gather_swiglu_IO3"),
     (r"gemm_mxfp8_kernel", "gemm_mxfp8"),
     (r"quantize_mxfp8_kernel", "quantize_mxfp8"),
-    (r"flash_fwd_kernel<128>", "flash_fwd_d128"),
-    (r"bwd_dkdv_kernel<128>", "flash_bwd_dkdv_d128"),
-    (r"bwd_dq_kernel<128>", "flash_bwd_dq_d128"),
+    # attention kernels <D, kDoc>: kDoc = document masking
+    (r"flash_fwd_kernel<128, false>", "flash_fwd_d128"),
+    (r"bwd_dkdv_kernel<128, false>", "flash_bwd_dkdv_d128"),
+    (r"bwd_dq_kernel<128, false>", "flash_bwd_dq_d128"),
+    (r"flash_fwd_kernel<128, true>", "flash_fwd_doc_d128"),
+    (r"bwd_dkdv_kernel<128, true>", "flash_bwd_dkdv_doc_d128"),
+    (r"bwd_dq_kernel<128, true>", "flash_bwd_dq_doc_d128"),
+    (r"doc_bounds_kernel", "doc_bounds"),
     (r"bwd_delta_kernel", "flash_bwd_delta"),
     (r"rmsnorm_fwd_kernel<4, true>", "rmsnorm_fwd_residual"),
     (r"rmsnorm_bwd_kernel<4, true>", "rmsnorm_bwd_residual"),
