@@ -12,8 +12,9 @@
 //           TRANSPOSED scores Sᵀ = K Qᵀ and dPᵀ = V dOᵀ so that each warp owns 16 key rows:  dV += Pᵀ dO,  dK += dSᵀ Q
 //   dQ:     one CTA per (64-query block, b, h); loops over 64-key tiles: S = Q Kᵀ, dP = dO Vᵀ,  dQ += dS K
 // With dS = P ∘ (dP·scale − delta·scale) the results need no further scaling; P is recomputed from lse2.
-// Optional RoPE backward (pb_flash_attn_bwd_rope): the inverse rotation is applied to dQ / dK in registers before the store.
-// Optional document masking of packed rows (kDoc, pb_flash_attn_{fwd,bwd}_doc with the bounds of pb_doc_bounds): key tiles that
+// Optional RoPE backward (non-null rope_cos / rope_sin of pb_flash_attn_bwd): the inverse rotation is applied to dQ / dK in registers
+// before the store.
+// Optional document masking of packed rows (kDoc, selected by a non-null doc_start with the bounds of pb_doc_bounds): key tiles that
 // lie before a query block's first document are skipped, not masked.
 #include "common.cuh"
 
@@ -557,22 +558,6 @@ int launch_bwd(const AttnParams& p, cudaStream_t stream) {
   return 0;
 }
 
-int bwd(const void* qkv, const void* out, const void* dout, const float* lse2, float* delta, void* dqkv, int B, int S, int H, int Hkv,
-        int D, float scale, int causal, const float* rope_cos, const float* rope_sin, const int* doc_start, const int* doc_end,
-        cudaStream_t stream) {
-  if (S % 128 != 0 || H % Hkv != 0) return -1;
-  AttnParams p{(const __nv_bfloat16*)qkv, (__nv_bfloat16*)out, (const __nv_bfloat16*)dout, (__nv_bfloat16*)dqkv, lse2, delta, nullptr,
-               B, S, H, Hkv, scale, scale * 1.4426950408889634f, causal, rope_cos, rope_sin, doc_start, doc_end};
-  if (doc_start != nullptr) {
-    if (D == 128) return launch_bwd<128, true>(p, stream);
-    if (D == 64) return launch_bwd<64, true>(p, stream);
-    return -2;
-  }
-  if (D == 128) return launch_bwd<128, false>(p, stream);
-  if (D == 64) return launch_bwd<64, false>(p, stream);
-  return -2;
-}
-
 // Document bounds of packed rows: one CTA per row. Every thread owns a contiguous run of positions; a block-wide exclusive
 // max-scan of the last document start per run (and min-scan, from the right, of the first EOS end) gives each run its carry-in.
 constexpr int kBoundsThreads = 256;
@@ -614,46 +599,43 @@ __global__ void __launch_bounds__(kBoundsThreads) doc_bounds_kernel(const int64_
   }
 }
 
-int g_fwd_variant = -1;
-int g_bwd_variant = -1;
-
 }  // namespace
 
-// Kernel-variant selectors kept for API compatibility: sm_90a has one forward and one backward kernel, every value runs them.
-// Return the previous value.
-PB_EXPORT int pb_flash_attn_fwd_set_variant(int v) {
-  const int old = g_fwd_variant;
-  g_fwd_variant = v;
-  return old;
-}
-PB_EXPORT int pb_flash_attn_bwd_set_variant(int v) {
-  const int old = g_bwd_variant;
-  g_bwd_variant = v;
-  return old;
-}
-
 // qkv [B, S, (H+2Hkv)·D] → out [B, S, H·D], lse2 [B, H, S].  S % 128 == 0, D ∈ {64, 128}.
-PB_EXPORT int pb_flash_attn_fwd(const void* qkv, void* out, float* lse2, int B, int S, int H, int Hkv, int D, float scale,
-                                int causal, cudaStream_t stream) {
-  if (S % 128 != 0 || H % Hkv != 0) return -1;
+// doc_start: null, or the int32 [B, S] document starts of pb_doc_bounds for document-masked causal attention (causal != 0): query q
+// attends key k iff doc_start[b, q] <= k <= q.
+PB_EXPORT int pb_flash_attn_fwd(const void* qkv, void* out, float* lse2, const int* doc_start, int B, int S, int H, int Hkv, int D,
+                                float scale, int causal, cudaStream_t stream) {
+  if (S % 128 != 0 || H % Hkv != 0 || (doc_start != nullptr && !causal)) return -1;
   AttnParams p{(const __nv_bfloat16*)qkv, (__nv_bfloat16*)out, nullptr, nullptr, nullptr, nullptr, lse2,
-               B, S, H, Hkv, scale, scale * 1.4426950408889634f, causal, nullptr, nullptr, nullptr, nullptr};
+               B, S, H, Hkv, scale, scale * 1.4426950408889634f, causal, nullptr, nullptr, doc_start, nullptr};
+  if (doc_start != nullptr) {
+    if (D == 128) return launch_fwd<128, true>(p, stream);
+    if (D == 64) return launch_fwd<64, true>(p, stream);
+    return -2;
+  }
   if (D == 128) return launch_fwd<128, false>(p, stream);
   if (D == 64) return launch_fwd<64, false>(p, stream);
   return -2;
 }
 
 // delta: [B, H, S] fp32 scratch.  dqkv: [B, S, (H+2Hkv)·D] bf16, fully overwritten.
+// doc_start / doc_end: both null, or both the forward's document bounds (causal != 0).
+// rope_cos / rope_sin: null, or the fp32 [S, D/2] tables of a forward rotation, whose inverse is fused into the dQ / dK stores.
 PB_EXPORT int pb_flash_attn_bwd(const void* qkv, const void* out, const void* dout, const float* lse2, float* delta, void* dqkv,
-                                int B, int S, int H, int Hkv, int D, float scale, int causal, cudaStream_t stream) {
-  return bwd(qkv, out, dout, lse2, delta, dqkv, B, S, H, Hkv, D, scale, causal, nullptr, nullptr, nullptr, nullptr, stream);
-}
-
-// Same, with the RoPE backward fused into the dQ / dK stores (cos/sin: fp32 [S, D/2] tables of the forward rotation).
-PB_EXPORT int pb_flash_attn_bwd_rope(const void* qkv, const void* out, const void* dout, const float* lse2, float* delta, void* dqkv,
-                                     int B, int S, int H, int Hkv, int D, float scale, int causal, const float* rope_cos,
-                                     const float* rope_sin, cudaStream_t stream) {
-  return bwd(qkv, out, dout, lse2, delta, dqkv, B, S, H, Hkv, D, scale, causal, rope_cos, rope_sin, nullptr, nullptr, stream);
+                                const int* doc_start, const int* doc_end, int B, int S, int H, int Hkv, int D, float scale, int causal,
+                                const float* rope_cos, const float* rope_sin, cudaStream_t stream) {
+  if (S % 128 != 0 || H % Hkv != 0 || (doc_start == nullptr) != (doc_end == nullptr) || (doc_start != nullptr && !causal)) return -1;
+  AttnParams p{(const __nv_bfloat16*)qkv, (__nv_bfloat16*)out, (const __nv_bfloat16*)dout, (__nv_bfloat16*)dqkv, lse2, delta, nullptr,
+               B, S, H, Hkv, scale, scale * 1.4426950408889634f, causal, rope_cos, rope_sin, doc_start, doc_end};
+  if (doc_start != nullptr) {
+    if (D == 128) return launch_bwd<128, true>(p, stream);
+    if (D == 64) return launch_bwd<64, true>(p, stream);
+    return -2;
+  }
+  if (D == 128) return launch_bwd<128, false>(p, stream);
+  if (D == 64) return launch_bwd<64, false>(p, stream);
+  return -2;
 }
 
 // tokens int64 [B, S] → doc_start, doc_end int32 [B, S]: position s starts a document when s == 0 or tokens[b, s-1] == eos;
@@ -663,23 +645,4 @@ PB_EXPORT int pb_doc_bounds(const int64_t* tokens, int B, int S, int64_t eos, in
   doc_bounds_kernel<<<B, kBoundsThreads, 0, stream>>>(tokens, S, eos, doc_start, doc_end);
   PB_CHECK_LAUNCH();
   return 0;
-}
-
-// Document-masked (always causal) forward: query q attends key k iff doc_start[b, q] <= k <= q.  doc_start: int32 [B, S].
-PB_EXPORT int pb_flash_attn_fwd_doc(const void* qkv, void* out, float* lse2, const int* doc_start, int B, int S, int H, int Hkv, int D,
-                                    float scale, cudaStream_t stream) {
-  if (S % 128 != 0 || H % Hkv != 0 || doc_start == nullptr) return -1;
-  AttnParams p{(const __nv_bfloat16*)qkv, (__nv_bfloat16*)out, nullptr, nullptr, nullptr, nullptr, lse2,
-               B, S, H, Hkv, scale, scale * 1.4426950408889634f, 1, nullptr, nullptr, doc_start, nullptr};
-  if (D == 128) return launch_fwd<128, true>(p, stream);
-  if (D == 64) return launch_fwd<64, true>(p, stream);
-  return -2;
-}
-
-// Document-masked backward; rope_cos / rope_sin may be null (plain backward) or the forward's tables (fused RoPE backward).
-PB_EXPORT int pb_flash_attn_bwd_doc(const void* qkv, const void* out, const void* dout, const float* lse2, float* delta, void* dqkv,
-                                    const int* doc_start, const int* doc_end, int B, int S, int H, int Hkv, int D, float scale,
-                                    const float* rope_cos, const float* rope_sin, cudaStream_t stream) {
-  if (doc_start == nullptr || doc_end == nullptr) return -1;
-  return bwd(qkv, out, dout, lse2, delta, dqkv, B, S, H, Hkv, D, scale, 1, rope_cos, rope_sin, doc_start, doc_end, stream);
 }

@@ -464,11 +464,6 @@ static int launch_cross_entropy(void* logits, const int64_t* targets, float* los
   return 0;
 }
 
-PB_EXPORT int pb_cross_entropy_fwd_bwd(void* logits, const int64_t* targets, float* losses, const float* scale_ptr,
-                                       int64_t R, int V, int64_t ignore_index, cudaStream_t stream) {
-  return launch_cross_entropy(logits, targets, losses, scale_ptr, R, V, ignore_index, stream);
-}
-
 // Whole loss node without a single framework kernel: count the valid targets → gradient scale; the row kernel; a fixed-order sum
 // of the per-row losses → mean loss (deterministic). work: >= 2 floats of scratch ([0] = grad_scale / n_valid, [1] = 1 / n_valid).
 __global__ void __launch_bounds__(1024) ce_count_kernel(const int64_t* __restrict__ targets, int64_t R, int64_t ignore_index,

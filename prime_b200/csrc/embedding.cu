@@ -129,8 +129,6 @@ PB_EXPORT int pb_embedding_fwd(const int64_t* tokens, int64_t T, const PeerPtrs*
   return 0;
 }
 
-PB_EXPORT int pb_embedding_bwd_max_chunk() { return 16384; }
-
 // Step 1 (can run as soon as the token ids exist, e.g. on a side stream during the FORWARD pass — it is one CTA for ~0.2 ms):
 // sorted[pos0 .. pos0+n) = (token << 32 | position) keys of every 16384-token chunk, ascending.
 PB_EXPORT int pb_embedding_sort(const int64_t* tokens, int64_t T, unsigned long long* sorted, cudaStream_t stream) {
@@ -160,14 +158,6 @@ PB_EXPORT int pb_embedding_scatter(const unsigned long long* sorted, int64_t T, 
     PB_CHECK_LAUNCH();
   }
   return 0;
-}
-
-// both steps on one stream. scratch: >= T uint64.
-PB_EXPORT int pb_embedding_bwd(const int64_t* tokens, int64_t T, const void* dout, float* grad, int dim, unsigned long long* scratch,
-                               cudaStream_t stream) {
-  int rc = pb_embedding_sort(tokens, T, scratch, stream);
-  if (rc) return rc;
-  return pb_embedding_scatter(scratch, T, dout, grad, dim, stream);
 }
 
 PB_EXPORT int pb_allgather_copy(const PeerPtrs* src, int64_t bytes_per_rank, void* dst, cudaStream_t stream) {

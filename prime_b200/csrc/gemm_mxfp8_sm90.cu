@@ -221,19 +221,7 @@ __global__ void __launch_bounds__(128) quantize_mxfp8_t_kernel(const __nv_bfloat
   sf[sf_offset(c, rb >> 5, atoms_c)] = (uint8_t)e8;
 }
 
-int g_mx_pair_mode = -1;
-
 }  // namespace
-
-// Tile-scheduler selector kept for API compatibility: sm_90a has one MXFP8 kernel, every mode runs it. Returns the old mode.
-PB_EXPORT int pb_gemm_mxfp8_set_pair_mode(int mode) {
-  const int old = g_mx_pair_mode;
-  g_mx_pair_mode = mode;
-  return old;
-}
-
-// Bytes of the scale-factor buffer for an operand with `rows` rows and K contraction elements (K % 128 == 0).
-PB_EXPORT int64_t pb_mxfp8_sf_bytes(int rows, int K) { return (int64_t)(K / 128) * ((rows + 127) / 128 + 1) * 512; }
 
 // transpose = 0: q [R, C] with blocks along C (C % 128 == 0).   transpose = 1: q [C, R] with blocks along R (R % 128 == 0).
 PB_EXPORT int pb_quantize_mxfp8(const void* x, int64_t ld, void* q, void* sf, int R, int C, int transpose, cudaStream_t stream) {
@@ -255,8 +243,7 @@ PB_EXPORT int pb_quantize_mxfp8(const void* x, int64_t ld, void* q, void* sf, in
 
 // C[M,N] bf16 = A_q[M,K] · B_q[N,K]ᵀ with per-32 UE8M0 scales (buffers laid out as described at the top of this file).
 PB_EXPORT int pb_gemm_mxfp8(const void* Aq, const void* sfa, const void* Bq, const void* sfb, void* C, int M, int N, int K, int ldc,
-                            int max_ctas, cudaStream_t stream) {
-  (void)max_ctas;
+                            cudaStream_t stream) {
   if (M <= 0 || N <= 0 || K <= 0) return 0;
   if (K % 128 || ldc % 8 || N % 8) return -1;
   if ((reinterpret_cast<uintptr_t>(Aq) | reinterpret_cast<uintptr_t>(Bq) | reinterpret_cast<uintptr_t>(C)) & 15) return -2;

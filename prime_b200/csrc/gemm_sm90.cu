@@ -610,25 +610,7 @@ int launch(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, in
   return e == cudaSuccess ? 0 : (int)e;
 }
 
-// Kept for callers that select a tile scheduler: the sm_90a kernel has a single one (one CTA per 128 x 128 tile).
-int g_pair_mode = -1;
-int pair_mode() {
-  if (g_pair_mode < 0) {
-    const char* e = getenv("PB_GEMM_PAIR");
-    g_pair_mode = e ? (atoi(e) != 0) : 1;
-  }
-  return g_pair_mode;
-}
-
 }  // namespace
-
-// Tile-scheduler selector kept for API compatibility: sm_90a has one scheduler (one CTA per 128 x 128 tile), so every mode runs
-// the same kernel. -1 = re-read PB_GEMM_PAIR. Returns the previous mode.
-PB_EXPORT int pb_gemm_set_pair_mode(int mode) {
-  const int old = pair_mode();
-  g_pair_mode = mode;
-  return old;
-}
 
 // Split-K policy for fp32 reduce-add outputs: -1 = automatic (default), 0 = never, n > 1 = always n slices (testing).
 PB_EXPORT int pb_gemm_set_split_k(int mode) {

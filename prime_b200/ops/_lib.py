@@ -138,7 +138,6 @@ def _declare(lib: ctypes.CDLL) -> None:
         "pb_rope_inplace": [vp, vp, vp, i64, i32, i32, i32, i32, f32, vp],
         "pb_swiglu_fwd": [vp, vp, i64, i32, vp],
         "pb_swiglu_bwd": [vp, vp, vp, i64, i32, vp],
-        "pb_cross_entropy_fwd_bwd": [vp, vp, vp, vp, i64, i32, i64, vp],
         "pb_cross_entropy_loss": [vp, vp, vp, vp, vp, vp, i64, i32, i64, f32, vp],
         "pb_gemm_bf16": [vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, i32, i32, i32, i32, vp],
         "pb_gemm_bf16_rope": [vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, vp, vp, i32, i32, i32, vp],
@@ -147,19 +146,11 @@ def _declare(lib: ctypes.CDLL) -> None:
         "pb_gemm_allgather": [vp, i32, i32, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, vp],
         "pb_gemm_reduce_scatter": [vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, i32, i32, vp],
         "pb_quantize_mxfp8": [vp, i64, vp, vp, i32, i32, i32, vp],
-        "pb_gemm_mxfp8": [vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, vp],
-        "pb_gemm_mxfp8_set_pair_mode": [i32],
-        "pb_gemm_set_pair_mode": [i32],
+        "pb_gemm_mxfp8": [vp, vp, vp, vp, vp, i32, i32, i32, i32, vp],
         "pb_gemm_set_split_k": [i32],
-        "pb_flash_attn_fwd": [vp, vp, vp, i32, i32, i32, i32, i32, f32, i32, vp],
-        "pb_flash_attn_bwd": [vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, f32, i32, vp],
-        "pb_flash_attn_bwd_set_trace": [vp],
-        "pb_flash_attn_bwd_set_variant": [i32],
-        "pb_flash_attn_fwd_set_variant": [i32],
-        "pb_flash_attn_bwd_rope": [vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, f32, i32, vp, vp, vp],
+        "pb_flash_attn_fwd": [vp, vp, vp, vp, i32, i32, i32, i32, i32, f32, i32, vp],
+        "pb_flash_attn_bwd": [vp, vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, f32, i32, vp, vp, vp],
         "pb_doc_bounds": [vp, i32, i32, i64, vp, vp, vp],
-        "pb_flash_attn_fwd_doc": [vp, vp, vp, vp, i32, i32, i32, i32, i32, f32, vp],
-        "pb_flash_attn_bwd_doc": [vp, vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, f32, vp, vp, vp],
         "pb_ipc_alloc": [ctypes.POINTER(vp), ctypes.c_size_t],
         "pb_ipc_free": [vp],
         "pb_ipc_handle_size": [],
@@ -179,8 +170,6 @@ def _declare(lib: ctypes.CDLL) -> None:
         "pb_set_spin_timeout_ms": [ctypes.c_ulonglong],
         "pb_grad_reduce_segs": [PP, ctypes.POINTER(SegTable), f32, vp, vp, vp, i32, u32, vp, i32, vp],
         "pb_embedding_fwd": [vp, i64, PP, i32, i32, vp, vp],
-        "pb_embedding_bwd": [vp, i64, vp, vp, i32, vp, vp],
-        "pb_embedding_bwd_max_chunk": [],
         "pb_embedding_sort": [vp, i64, vp, vp],
         "pb_embedding_scatter": [vp, i64, vp, vp, i32, vp],
         "pb_allgather_copy": [PP, i64, vp, vp],
@@ -209,9 +198,6 @@ def _declare(lib: ctypes.CDLL) -> None:
             continue
         fn.argtypes = argtypes
         fn.restype = ctypes.c_int
-    if hasattr(lib, "pb_mxfp8_sf_bytes"):
-        lib.pb_mxfp8_sf_bytes.argtypes = [i32, i32]
-        lib.pb_mxfp8_sf_bytes.restype = ctypes.c_int64
 
 
 def load(build_if_missing: bool = True) -> ctypes.CDLL:

@@ -14,7 +14,7 @@ import math
 import torch
 
 from . import _lib
-from .functional import _count, _ptr, _stream
+from .functional import _launch, _ptr, _rope_inplace, _stream
 
 
 def supported_shape(S: int, D: int, H: int, Hkv: int) -> bool:
@@ -41,122 +41,57 @@ def _check_doc(doc, qkv: torch.Tensor, causal: bool) -> None:
             raise ValueError(f"doc bounds must be contiguous int32 [{B}, {S}] tensors on {qkv.device} (ops.document_bounds)")
 
 
-def _fwd(lib, qkv: torch.Tensor, n_heads: int, n_kv_heads: int, causal: bool, doc) -> tuple[torch.Tensor, torch.Tensor, int, float]:
-    B, S, W = qkv.shape
-    D = W // (n_heads + 2 * n_kv_heads)
-    out = torch.empty((B, S, n_heads * D), dtype=qkv.dtype, device=qkv.device)
-    lse2 = torch.empty((B, n_heads, S), dtype=torch.float32, device=qkv.device)
-    scale = 1.0 / math.sqrt(D)
-    if doc is None:
-        rc = lib.pb_flash_attn_fwd(_ptr(qkv), _ptr(out), _ptr(lse2), B, S, n_heads, n_kv_heads, D, scale, int(causal), _stream())
-        _lib.check(rc, "pb_flash_attn_fwd")
-    else:
-        rc = lib.pb_flash_attn_fwd_doc(_ptr(qkv), _ptr(out), _ptr(lse2), _ptr(doc[0]), B, S, n_heads, n_kv_heads, D, scale, _stream())
-        _lib.check(rc, "pb_flash_attn_fwd_doc")
-    _count()
-    return out, lse2, D, scale
+class _FlashAttnFn(torch.autograd.Function):
+    """Attention over the fused QKV activation as ONE autograd node, optionally with RoPE on the Q/K heads (``cos`` / ``sin`` not
+    None). The forward rotates in place on the QKV GEMM output (nobody else reads the un-rotated activation) unless the producer
+    already did (``pre_rotated``); the backward folds the inverse rotation into the dQ / dK epilogues of the attention-backward
+    kernels, so there is neither a copy of the 200 MB gradient (a stand-alone RoPE node may not mutate a gradient it does not own)
+    nor a separate rotation pass over it. ``doc_start`` / ``doc_end``: document masking (both or neither)."""
 
-
-def _bwd_doc(lib, qkv, out, dout, lse2, delta, dqkv, doc_start, doc_end, n_heads, n_kv_heads, D, scale, cos=None, sin=None) -> None:
-    B, S, _ = qkv.shape
-    rc = lib.pb_flash_attn_bwd_doc(_ptr(qkv), _ptr(out), _ptr(dout), _ptr(lse2), _ptr(delta), _ptr(dqkv), _ptr(doc_start), _ptr(doc_end),
-                                   B, S, n_heads, n_kv_heads, D, scale, _ptr(cos), _ptr(sin), _stream())  # fmt: skip
-    _lib.check(rc, "pb_flash_attn_bwd_doc")
-
-
-class _FlashAttnQKVFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, qkv: torch.Tensor, n_heads: int, n_kv_heads: int, causal: bool, doc_start=None, doc_end=None):
-        lib = _lib.load()
-        doc = None if doc_start is None else (doc_start, doc_end)
-        out, lse2, D, scale = _fwd(lib, qkv, n_heads, n_kv_heads, causal, doc)
-        ctx.save_for_backward(qkv, out, lse2, *(doc or ()))
+    def forward(ctx, qkv: torch.Tensor, n_heads: int, n_kv_heads: int, causal: bool, cos=None, sin=None, pre_rotated: bool = False,
+                doc_start=None, doc_end=None):  # fmt: skip
+        B, S, W = qkv.shape
+        D = W // (n_heads + 2 * n_kv_heads)
+        if cos is not None and not pre_rotated:
+            _rope_inplace(qkv, cos, sin, n_heads, n_kv_heads, 1.0)
+        out = torch.empty((B, S, n_heads * D), dtype=qkv.dtype, device=qkv.device)
+        lse2 = torch.empty((B, n_heads, S), dtype=torch.float32, device=qkv.device)
+        scale = 1.0 / math.sqrt(D)
+        _launch("pb_flash_attn_fwd", _ptr(qkv), _ptr(out), _ptr(lse2), _ptr(doc_start), B, S, n_heads, n_kv_heads, D, scale, int(causal),
+                _stream())  # fmt: skip
+        ctx.save_for_backward(qkv, out, lse2, cos, sin, doc_start, doc_end)
         ctx.meta = (n_heads, n_kv_heads, D, scale, causal)
         return out
 
     @staticmethod
     def backward(ctx, dout: torch.Tensor):
-        lib = _lib.load()
-        qkv, out, lse2, *doc = ctx.saved_tensors
+        qkv, out, lse2, cos, sin, doc_start, doc_end = ctx.saved_tensors
         n_heads, n_kv_heads, D, scale, causal = ctx.meta
         B, S, _ = qkv.shape
         dout = dout if dout.is_contiguous() else dout.contiguous()
         dqkv = torch.empty_like(qkv)
         delta = torch.empty_like(lse2)
-        if doc:
-            _bwd_doc(lib, qkv, out, dout, lse2, delta, dqkv, doc[0], doc[1], n_heads, n_kv_heads, D, scale)
-        else:
-            rc = lib.pb_flash_attn_bwd(_ptr(qkv), _ptr(out), _ptr(dout), _ptr(lse2), _ptr(delta), _ptr(dqkv), B, S, n_heads,
-                                       n_kv_heads, D, scale, int(causal), _stream())  # fmt: skip
-            _lib.check(rc, "pb_flash_attn_bwd")
-        _count(3)
-        return dqkv, None, None, None, None, None
+        if cos is not None:
+            # rotation is orthogonal: its backward is the inverse rotation, applied to dQ / dK inside the attention-backward epilogues
+            # (registers → smem → TMA store), so dQKV is written exactly once
+            assert cos.dtype == torch.float32 and cos.is_contiguous() and sin.is_contiguous() and cos.shape[1] == D // 2 and cos.shape[0] >= S
+        _launch("pb_flash_attn_bwd", _ptr(qkv), _ptr(out), _ptr(dout), _ptr(lse2), _ptr(delta), _ptr(dqkv), _ptr(doc_start), _ptr(doc_end),
+                B, S, n_heads, n_kv_heads, D, scale, int(causal), _ptr(cos), _ptr(sin), _stream(), n=3)  # fmt: skip
+        return dqkv, None, None, None, None, None, None, None, None
 
 
 def flash_attention_qkv(qkv: torch.Tensor, n_heads: int, n_kv_heads: int, causal: bool = True, doc: tuple | None = None) -> torch.Tensor:
     """``doc=(doc_start, doc_end)`` (int32 [B, S], :func:`prime_b200.ops.document_bounds`): document-masked causal attention."""
-    if doc is None:
-        return _FlashAttnQKVFn.apply(qkv, n_heads, n_kv_heads, causal)
-    _check_doc(doc, qkv, causal)
-    return _FlashAttnQKVFn.apply(qkv, n_heads, n_kv_heads, causal, doc[0], doc[1])
+    return rope_flash_attention_qkv(qkv, None, None, n_heads, n_kv_heads, causal, doc=doc)
 
 
-def _rope_inplace(lib, t: torch.Tensor, cos, sin, n_heads: int, n_kv_heads: int, D: int, sign: float) -> None:
-    tokens = t.numel() // t.shape[-1]
-    rc = lib.pb_rope_inplace(_ptr(t), _ptr(cos), _ptr(sin), tokens, t.shape[1], n_heads + n_kv_heads, n_heads + 2 * n_kv_heads, D,
-                             sign, _stream())  # fmt: skip
-    _lib.check(rc, "pb_rope_inplace")
-    _count()
-
-
-class _RopeFlashAttnFn(torch.autograd.Function):
-    """RoPE ⊕ attention as ONE autograd node: forward rotates in place on the QKV GEMM output (nobody else reads the un-rotated
-    activation); backward folds the inverse rotation into the dQ / dK epilogues of the attention-backward kernels, so there is
-    neither a copy of the 200 MB gradient (a stand-alone RoPE node may not mutate a gradient it does not own) nor a separate
-    rotation pass over it."""
-
-    @staticmethod
-    def forward(ctx, qkv: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor, n_heads: int, n_kv_heads: int, causal: bool,
-                pre_rotated: bool = False, doc_start=None, doc_end=None):  # fmt: skip
-        lib = _lib.load()
-        B, S, W = qkv.shape
-        D = W // (n_heads + 2 * n_kv_heads)
-        if not pre_rotated:  # otherwise the QKV GEMM epilogue already did it
-            _rope_inplace(lib, qkv, cos, sin, n_heads, n_kv_heads, D, 1.0)
-        doc = None if doc_start is None else (doc_start, doc_end)
-        out, lse2, D, scale = _fwd(lib, qkv, n_heads, n_kv_heads, causal, doc)
-        ctx.save_for_backward(qkv, out, lse2, cos, sin, *(doc or ()))
-        ctx.meta = (n_heads, n_kv_heads, D, scale, causal)
-        return out
-
-    @staticmethod
-    def backward(ctx, dout: torch.Tensor):
-        lib = _lib.load()
-        qkv, out, lse2, cos, sin, *doc = ctx.saved_tensors
-        n_heads, n_kv_heads, D, scale, causal = ctx.meta
-        B, S, _ = qkv.shape
-        dout = dout if dout.is_contiguous() else dout.contiguous()
-        dqkv = torch.empty_like(qkv)
-        delta = torch.empty_like(lse2)
-        # rotation is orthogonal: its backward is the inverse rotation, applied to dQ / dK inside the attention-backward epilogues
-        # (registers → smem → TMA store), so dQKV is written exactly once
-        assert cos.dtype == torch.float32 and cos.is_contiguous() and sin.is_contiguous() and cos.shape[1] == D // 2 and cos.shape[0] >= S
-        if doc:
-            _bwd_doc(lib, qkv, out, dout, lse2, delta, dqkv, doc[0], doc[1], n_heads, n_kv_heads, D, scale, cos, sin)
-        else:
-            rc = lib.pb_flash_attn_bwd_rope(_ptr(qkv), _ptr(out), _ptr(dout), _ptr(lse2), _ptr(delta), _ptr(dqkv), B, S, n_heads,
-                                            n_kv_heads, D, scale, int(causal), _ptr(cos), _ptr(sin), _stream())  # fmt: skip
-            _lib.check(rc, "pb_flash_attn_bwd_rope")
-        _count(3)
-        return dqkv, None, None, None, None, None, None, None, None
-
-
-def rope_flash_attention_qkv(qkv: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor, n_heads: int, n_kv_heads: int,
+def rope_flash_attention_qkv(qkv: torch.Tensor, cos: torch.Tensor | None, sin: torch.Tensor | None, n_heads: int, n_kv_heads: int,
                              causal: bool = True, pre_rotated: bool = False, doc: tuple | None = None) -> torch.Tensor:  # fmt: skip
-    if doc is None:
-        return _RopeFlashAttnFn.apply(qkv, cos, sin, n_heads, n_kv_heads, causal, pre_rotated)
-    _check_doc(doc, qkv, causal)
-    return _RopeFlashAttnFn.apply(qkv, cos, sin, n_heads, n_kv_heads, causal, pre_rotated, doc[0], doc[1])
+    """RoPE (``cos`` / ``sin`` fp32 [S, D/2] tables; None = no rotation) ⊕ attention, see :class:`_FlashAttnFn`."""
+    if doc is not None:
+        _check_doc(doc, qkv, causal)
+    return _FlashAttnFn.apply(qkv, n_heads, n_kv_heads, causal, cos, sin, pre_rotated, *(doc or (None, None)))
 
 
 def document_bounds(tokens: torch.Tensor, eos_id: int) -> tuple[torch.Tensor, torch.Tensor]:
@@ -166,6 +101,5 @@ def document_bounds(tokens: torch.Tensor, eos_id: int) -> tuple[torch.Tensor, to
     assert t.dtype == torch.int64
     doc_start = torch.empty((B, S), dtype=torch.int32, device=t.device)
     doc_end = torch.empty((B, S), dtype=torch.int32, device=t.device)
-    _lib.check(_lib.load().pb_doc_bounds(_ptr(t), B, S, int(eos_id), _ptr(doc_start), _ptr(doc_end), _stream()), "pb_doc_bounds")
-    _count()
+    _launch("pb_doc_bounds", _ptr(t), B, S, int(eos_id), _ptr(doc_start), _ptr(doc_end), _stream())
     return doc_start, doc_end

@@ -38,6 +38,18 @@ def _ptr(t: torch.Tensor | None) -> int | None:
     return None if t is None else t.data_ptr()
 
 
+def _launch(name: str, *args, n: int = 1) -> None:
+    """Call the native launcher ``name``, raise on a non-zero return code and count the ``n`` kernels it launches."""
+    _lib.check(getattr(_lib.load(), name)(*args), name)
+    _count(n)
+
+
+def _rows(t: torch.Tensor) -> torch.Tensor:
+    """``t`` as a 2-D [rows, last dim] matrix with unit strides (a view when the layout allows it)."""
+    t2 = t.reshape(-1, t.shape[-1])
+    return t2 if t2.is_contiguous() else t2.contiguous()
+
+
 # --------------------------------------------------------------------------- GEMM
 
 
@@ -74,20 +86,11 @@ def gemm(
         out = torch.empty((M, N), dtype=out_dtype, device=a.device)
     else:
         assert out.shape == (M, N) and out.stride(1) == 1 and out.dtype in (torch.bfloat16, torch.float32)
-    lib = _lib.load()
-    rc = lib.pb_gemm_bf16(
-        a.data_ptr(), b.data_ptr(), out.data_ptr(), M, N, K, a.stride(0), b.stride(0), out.stride(0),
+    _launch(
+        "pb_gemm_bf16", a.data_ptr(), b.data_ptr(), out.data_ptr(), M, N, K, a.stride(0), b.stride(0), out.stride(0),
         int(a_mn_major), int(b_mn_major), int(out.dtype == torch.float32), int(accumulate), max_ctas, _stream(),
     )  # fmt: skip
-    _lib.check(rc, "pb_gemm_bf16")
-    _count()
     return out
-
-
-def set_gemm_pair_mode(on: bool | None) -> int:
-    """Tile-scheduler selector of the GEMM, kept for API compatibility: on sm_90a every mode runs the one scheduler (one CTA per
-    128×128 tile). ``None`` = re-read ``PB_GEMM_PAIR``. Returns the previous mode."""
-    return int(_lib.load().pb_gemm_set_pair_mode(-1 if on is None else int(bool(on))))
 
 
 def set_gemm_split_k(mode: int) -> int:
@@ -138,6 +141,45 @@ def _full_weight(z, device) -> torch.Tensor:
     return torch.as_tensor(_RawBuffer(z.full_ptr, z.rows * z.cols * 2), device=device).view(torch.bfloat16).view(z.rows, z.cols)
 
 
+def _gemm_epi(a: torch.Tensor, w: torch.Tensor, out: torch.Tensor, *, b_mn_major: bool = False, rope: tuple | None = None,
+              swiglu_h: torch.Tensor | None = None, swiglu_bwd_gu: torch.Tensor | None = None) -> torch.Tensor:  # fmt: skip
+    """The GEMM of :func:`gemm_wgather` and its epilogues on a local weight ``w`` [rows, cols]: C = a·wᵀ (``rope``, ``swiglu_h``) or,
+    with ``b_mn_major``, C = a·w (``swiglu_bwd_gu``). SwiGLU runs as a stand-alone kernel after a plain GEMM where its fused
+    epilogue does not apply (M <= 128, and for the forward hidden % 64 != 0)."""
+    M = a.shape[0]
+    if swiglu_bwd_gu is not None:
+        if M > 128:
+            _launch("pb_gemm_bf16_swiglu_bwd", a.data_ptr(), w.data_ptr(), swiglu_bwd_gu.data_ptr(), out.data_ptr(), M, w.shape[1], w.shape[0],
+                    a.stride(0), w.stride(0), swiglu_bwd_gu.stride(0), out.stride(0), _stream())  # fmt: skip
+        else:
+            dh = gemm(a, w, b_mn_major=True)
+            _launch("pb_swiglu_bwd", swiglu_bwd_gu.data_ptr(), dh.data_ptr(), out.data_ptr(), M, w.shape[1], _stream())
+    elif swiglu_h is not None:
+        FF = w.shape[0] // 2
+        if M > 128 and FF % 64 == 0:
+            _launch("pb_gemm_bf16_swiglu", a.data_ptr(), w.data_ptr(), out.data_ptr(), swiglu_h.data_ptr(), M, FF, w.shape[1], a.stride(0),
+                    w.stride(0), out.stride(0), swiglu_h.stride(0), _stream())  # fmt: skip
+        else:
+            gemm(a, w, out=out)
+            _launch("pb_swiglu_fwd", out.data_ptr(), swiglu_h.data_ptr(), M, FF, _stream())
+    elif rope is not None:
+        cos, sin, seq_len, rot_cols, head_dim = rope
+        assert cos.dtype == torch.float32 and cos.is_contiguous() and sin.is_contiguous() and cos.shape[0] >= seq_len
+        _launch("pb_gemm_bf16_rope", a.data_ptr(), w.data_ptr(), out.data_ptr(), M, w.shape[0], a.shape[1], a.stride(0), w.stride(0),
+                out.stride(0), 0, cos.data_ptr(), sin.data_ptr(), seq_len, rot_cols, head_dim, _stream())  # fmt: skip
+    else:
+        gemm(a, w, b_mn_major=b_mn_major, out=out)
+    return out
+
+
+def _matmul(a: torch.Tensor, weight: torch.Tensor, out: torch.Tensor, **epi) -> torch.Tensor:
+    """:func:`_gemm_epi` on ``weight``, gathered from the peers' shards inside the GEMM when it is ZeRO-3 sharded (``weight.z3``)."""
+    z = getattr(weight, "z3", None)
+    if z is not None:
+        return gemm_wgather(a, z, out=out, **epi)
+    return _gemm_epi(a, weight, out, **epi)
+
+
 def gemm_wgather(a: torch.Tensor, z, *, b_mn_major: bool = False, out: torch.Tensor | None = None, rope: tuple | None = None,
                  swiglu_h: torch.Tensor | None = None, swiglu_bwd_gu: torch.Tensor | None = None) -> torch.Tensor:  # fmt: skip
     """Parameter all-gather ⊕ GEMM (ZeRO-3): ``z`` is the ``RowShard`` of a weight W [rows, cols] sharded by rows over the FSDP group.
@@ -157,8 +199,6 @@ def gemm_wgather(a: torch.Tensor, z, *, b_mn_major: bool = False, out: torch.Ten
     assert a.shape[1] == (z.rows if b_mn_major else z.cols)
     if out is None:
         out = torch.empty((M, 2 * N if swiglu_bwd_gu is not None else N), dtype=torch.bfloat16, device=a.device)
-    lib = _lib.load()
-    epi = 3 if swiglu_bwd_gu is not None else (2 if swiglu_h is not None else (1 if rope is not None else 0))
     own_resident = _resident(z)
     nz = z.next_bwd if b_mn_major else z.next_fwd
     if nz is not None and (nz.full_ptr == 0 or _resident(nz) or nz.n != z.n):
@@ -168,55 +208,23 @@ def gemm_wgather(a: torch.Tensor, z, *, b_mn_major: bool = False, out: torch.Ten
         # gather by peer loads first): the plain kernels
         if not own_resident:
             pp = _lib.PeerPtrs.of(z.peer_ptrs[i] for i in range(z.n))
-            _lib.check(lib.pb_allgather_copy(ctypes.byref(pp), z.rpr * z.cols * 2, z.full_ptr, _stream()), "pb_allgather_copy")
-            _count()
+            _launch("pb_allgather_copy", ctypes.byref(pp), z.rpr * z.cols * 2, z.full_ptr, _stream())
             _mark_resident(z)
-        w = _full_weight(z, a.device)
-        if epi == 3:
-            if M > 128:
-                rc = lib.pb_gemm_bf16_swiglu_bwd(a.data_ptr(), w.data_ptr(), swiglu_bwd_gu.data_ptr(), out.data_ptr(), M, z.cols, z.rows,
-                                                 a.stride(0), w.stride(0), swiglu_bwd_gu.stride(0), out.stride(0), _stream())  # fmt: skip
-                _lib.check(rc, "pb_gemm_bf16_swiglu_bwd")
-                _count()
-            else:
-                dh = gemm(a, w, b_mn_major=True)
-                _lib.check(lib.pb_swiglu_bwd(swiglu_bwd_gu.data_ptr(), dh.data_ptr(), out.data_ptr(), M, z.cols, _stream()), "pb_swiglu_bwd")
-                _count()
-        elif epi == 2:
-            FF = z.rows // 2
-            if M > 128 and FF % 64 == 0:
-                rc = lib.pb_gemm_bf16_swiglu(a.data_ptr(), w.data_ptr(), out.data_ptr(), swiglu_h.data_ptr(), M, FF, z.cols, a.stride(0),
-                                             w.stride(0), out.stride(0), swiglu_h.stride(0), _stream())  # fmt: skip
-                _lib.check(rc, "pb_gemm_bf16_swiglu")
-                _count()
-            else:
-                gemm(a, w, out=out)
-                _lib.check(lib.pb_swiglu_fwd(out.data_ptr(), swiglu_h.data_ptr(), M, FF, _stream()), "pb_swiglu_fwd")
-                _count()
-        elif epi == 1:
-            cos, sin, seq_len, rot_cols, head_dim = rope
-            rc = lib.pb_gemm_bf16_rope(a.data_ptr(), w.data_ptr(), out.data_ptr(), M, N, a.shape[1], a.stride(0), w.stride(0), out.stride(0), 0,
-                                       cos.data_ptr(), sin.data_ptr(), seq_len, rot_cols, head_dim, _stream())  # fmt: skip
-            _lib.check(rc, "pb_gemm_bf16_rope")
-            _count()
-        else:
-            gemm(a, w, b_mn_major=b_mn_major, out=out)
-        return out
+        return _gemm_epi(a, _full_weight(z, a.device), out, b_mn_major=b_mn_major, rope=rope, swiglu_h=swiglu_h, swiglu_bwd_gu=swiglu_bwd_gu)
+    epi = 3 if swiglu_bwd_gu is not None else (2 if swiglu_h is not None else (1 if rope is not None else 0))
     cos = sin = None
     seq_len, rot_cols, head_dim = 1, 0, 64
     if rope is not None:
         cos, sin, seq_len, rot_cols, head_dim = rope
         assert cos.dtype == torch.float32 and cos.is_contiguous() and sin.is_contiguous() and cos.shape[0] >= seq_len
     aux = swiglu_h if swiglu_h is not None else swiglu_bwd_gu
-    rc = lib.pb_gemm_wgather(
-        a.data_ptr(), z.peer_ptrs, z.n, z.rank, z.full_ptr, z.flags.data_ptr(), out.data_ptr(), _ptr(aux), M, z.rows, z.cols,
-        a.stride(0), out.stride(0), aux.stride(0) if aux is not None else 0, int(b_mn_major), epi,
+    _launch(
+        "pb_gemm_wgather", a.data_ptr(), z.peer_ptrs, z.n, z.rank, z.full_ptr, z.flags.data_ptr(), out.data_ptr(), _ptr(aux), M, z.rows,
+        z.cols, a.stride(0), out.stride(0), aux.stride(0) if aux is not None else 0, int(b_mn_major), epi,
         _ptr(cos), _ptr(sin), seq_len, rot_cols, head_dim,
         int(own_resident), nz.peer_ptrs if nz is not None else None, nz.full_ptr if nz is not None else None,
-        nz.rows if nz is not None else 0, nz.cols if nz is not None else 0, _stream(),
+        nz.rows if nz is not None else 0, nz.cols if nz is not None else 0, _stream(), n=1 if own_resident else 2,
     )  # fmt: skip
-    _lib.check(rc, "pb_gemm_wgather")
-    _count(1 if own_resident else 2)
     _mark_resident(z)
     if nz is not None:
         _mark_resident(nz)
@@ -236,45 +244,25 @@ class _LinearFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, x: torch.Tensor, weight: torch.Tensor, rope: tuple | None = None) -> torch.Tensor:
-        x2 = x.reshape(-1, x.shape[-1])
-        if not x2.is_contiguous():
-            x2 = x2.contiguous()
+        x2 = _rows(x)
         ctx.save_for_backward(x2, weight)
         ctx.x_shape = x.shape
         # allocate with the final shape: a Function output must not be a view (RoPE / the loss rotate / overwrite it in place)
         y = torch.empty((*x.shape[:-1], weight.shape[0]), dtype=x.dtype, device=x.device)
-        z = getattr(weight, "z3", None)
-        if z is not None:  # ZeRO-3: the weight is gathered from the peers' shards inside the GEMM
-            gemm_wgather(x2, z, out=y.view(-1, weight.shape[0]), rope=rope)
-        elif rope is None:
-            gemm(x2, weight, out=y.view(-1, weight.shape[0]))
-        else:
-            # fused QKV projection: the GEMM epilogue rotates the Q/K head columns while the tile is in registers. The consumer
-            # (rope_attention_qkv(..., pre_rotated=True)) returns the gradient w.r.t. the UN-rotated activation, so backward below
-            # is the plain linear backward.
-            cos, sin, seq_len, rot_cols, head_dim = rope
-            M, N, K = x2.shape[0], weight.shape[0], x2.shape[1]
-            assert cos.dtype == torch.float32 and cos.is_contiguous() and sin.is_contiguous() and cos.shape[0] >= seq_len
-            rc = _lib.load().pb_gemm_bf16_rope(x2.data_ptr(), weight.data_ptr(), y.data_ptr(), M, N, K, x2.stride(0), weight.stride(0), N, 0,
-                                               cos.data_ptr(), sin.data_ptr(), seq_len, rot_cols, head_dim, _stream())  # fmt: skip
-            _lib.check(rc, "pb_gemm_bf16_rope")
-            _count()
+        # rope: fused QKV projection, the GEMM epilogue rotates the Q/K head columns while the tile is in registers. The consumer
+        # (rope_attention_qkv(..., pre_rotated=True)) returns the gradient w.r.t. the UN-rotated activation, so backward below is the
+        # plain linear backward.
+        _matmul(x2, weight, y.view(-1, weight.shape[0]), rope=rope)
         return y
 
     @staticmethod
     def backward(ctx, dy: torch.Tensor):
         x2, weight = ctx.saved_tensors
-        dy2 = dy.reshape(-1, dy.shape[-1])
-        if not dy2.is_contiguous():
-            dy2 = dy2.contiguous()
+        dy2 = _rows(dy)
         dx = dw = None
         if ctx.needs_input_grad[0]:
             dx = torch.empty(ctx.x_shape, dtype=dy.dtype, device=dy.device)
-            z = getattr(weight, "z3", None)
-            if z is not None:
-                gemm_wgather(dy2, z, b_mn_major=True, out=dx.view(-1, ctx.x_shape[-1]))
-            else:
-                gemm(dy2, weight, b_mn_major=True, out=dx.view(-1, ctx.x_shape[-1]))
+            _matmul(dy2, weight, dx.view(-1, ctx.x_shape[-1]), b_mn_major=True)
         if ctx.needs_input_grad[1]:
             dw = _wgrad(dy2, x2, weight)
         return dx, dw, None
@@ -286,7 +274,6 @@ def linear(x: torch.Tensor, weight: torch.Tensor) -> torch.Tensor:
     return reference.linear(x, weight)
 
 
-# A/B switch for measurements: PB_NO_EPILOGUE_FUSION=1 runs RoPE and SwiGLU as stand-alone kernels again
 # --------------------------------------------------------------------------- block-scaled fp8 (MXFP8)
 
 
@@ -308,14 +295,11 @@ def quantize_mxfp8(x: torch.Tensor, transpose: bool = False) -> tuple[torch.Tens
         return reference.quantize_mxfp8(x, transpose)
     q = torch.empty((rows, k), dtype=torch.uint8, device=x.device)
     sf = torch.empty(mxfp8_sf_bytes(rows, k), dtype=torch.uint8, device=x.device)
-    rc = _lib.load().pb_quantize_mxfp8(x.data_ptr(), x.stride(0), q.data_ptr(), sf.data_ptr(), R, C, int(transpose), _stream())
-    _lib.check(rc, "pb_quantize_mxfp8")
-    _count()
+    _launch("pb_quantize_mxfp8", x.data_ptr(), x.stride(0), q.data_ptr(), sf.data_ptr(), R, C, int(transpose), _stream())
     return q, sf
 
 
-def gemm_mxfp8(aq: torch.Tensor, asf: torch.Tensor, bq: torch.Tensor, bsf: torch.Tensor, out: torch.Tensor | None = None,
-               max_ctas: int = 0) -> torch.Tensor:  # fmt: skip
+def gemm_mxfp8(aq: torch.Tensor, asf: torch.Tensor, bq: torch.Tensor, bsf: torch.Tensor, out: torch.Tensor | None = None) -> torch.Tensor:
     """C[M,N] bf16 = dequant(A)·dequant(B)ᵀ with e4m3 tensor-core MMAs, scaled per 32-element block in registers."""
     M, K = aq.shape
     N, Kb = bq.shape
@@ -329,17 +313,8 @@ def gemm_mxfp8(aq: torch.Tensor, asf: torch.Tensor, bq: torch.Tensor, bsf: torch
     if out is None:
         out = torch.empty((M, N), dtype=torch.bfloat16, device=aq.device)
     assert out.shape == (M, N) and out.dtype == torch.bfloat16 and out.stride(1) == 1
-    rc = _lib.load().pb_gemm_mxfp8(aq.data_ptr(), asf.data_ptr(), bq.data_ptr(), bsf.data_ptr(), out.data_ptr(), M, N, K, out.stride(0),
-                                   max_ctas, _stream())  # fmt: skip
-    _lib.check(rc, "pb_gemm_mxfp8")
-    _count()
+    _launch("pb_gemm_mxfp8", aq.data_ptr(), asf.data_ptr(), bq.data_ptr(), bsf.data_ptr(), out.data_ptr(), M, N, K, out.stride(0), _stream())
     return out
-
-
-def set_mxfp8_pair_mode(on: bool | None) -> int:
-    """Scheduler of the MXFP8 GEMM: ``False`` = one CTA per 128×192 tile, ``True`` = CTA pair (``cta_group::2``) per 256×192 tile,
-    ``None`` = re-read ``PB_MXFP8_PAIR``. Returns the previous mode."""
-    return int(_lib.load().pb_gemm_mxfp8_set_pair_mode(-1 if on is None else int(bool(on))))
 
 
 class _LinearMXFP8Fn(torch.autograd.Function):
@@ -349,9 +324,7 @@ class _LinearMXFP8Fn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, x: torch.Tensor, weight: torch.Tensor) -> torch.Tensor:
-        x2 = x.reshape(-1, x.shape[-1])
-        if not x2.is_contiguous():
-            x2 = x2.contiguous()
+        x2 = _rows(x)
         ctx.save_for_backward(x2, weight)
         ctx.x_shape = x.shape
         xq, xsf = quantize_mxfp8(x2)
@@ -363,9 +336,7 @@ class _LinearMXFP8Fn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dy: torch.Tensor):
         x2, weight = ctx.saved_tensors
-        dy2 = dy.reshape(-1, dy.shape[-1])
-        if not dy2.is_contiguous():
-            dy2 = dy2.contiguous()
+        dy2 = _rows(dy)
         dx = dw = None
         if ctx.needs_input_grad[0]:
             dyq, dysf = quantize_mxfp8(dy2)                     # [M, N], blocks along N
@@ -393,10 +364,8 @@ def linear_mxfp8(x: torch.Tensor, weight: torch.Tensor) -> torch.Tensor:
     return _LinearMXFP8Fn.apply(x, weight)
 
 
+# A/B switch for measurements: PB_NO_EPILOGUE_FUSION=1 runs RoPE and SwiGLU as stand-alone kernels again
 _NO_EPILOGUE_FUSION = bool(int(__import__("os").environ.get("PB_NO_EPILOGUE_FUSION", "0")))
-# SwiGLU backward inside the down-projection's dgrad epilogue (EPI = 3) vs dgrad + stand-alone kernel. Default = what measured faster
-# in the step (DESIGN.md §1.6 has the numbers of both); PB_SWIGLU_BWD_FUSED=0/1 overrides.
-_SWIGLU_BWD_FUSED = bool(int(__import__("os").environ.get("PB_SWIGLU_BWD_FUSED", "1")))
 
 
 def rope_fusable(x: torch.Tensor, n_heads: int, n_kv_heads: int, head_dim: int) -> bool:
@@ -426,7 +395,6 @@ class _EmbeddingFn(torch.autograd.Function):
     def forward(ctx, tokens: torch.Tensor, weight: torch.Tensor) -> torch.Tensor:
         import ctypes
 
-        lib = _lib.load()
         V, dim = weight.shape
         t = tokens.reshape(-1)
         t = t if t.is_contiguous() else t.contiguous()
@@ -438,39 +406,36 @@ class _EmbeddingFn(torch.autograd.Function):
             assert weight.is_contiguous()
             pp, rpr = _lib.PeerPtrs.of([weight.data_ptr()]), V
         out = torch.empty((*tokens.shape, dim), dtype=weight.dtype, device=weight.device)
-        _lib.check(lib.pb_embedding_fwd(t.data_ptr(), t.numel(), ctypes.byref(pp), rpr, dim, out.data_ptr(), _stream()), "pb_embedding_fwd")
-        _count()
+        _launch("pb_embedding_fwd", t.data_ptr(), t.numel(), ctypes.byref(pp), rpr, dim, out.data_ptr(), _stream())
         ctx.weight = weight
         ctx.sorted_ev = None
         if ctx.needs_input_grad[1]:  # (autograd runs forward() with grad mode off: needs_input_grad is the reliable signal)
             # the backward needs the positions sorted by token: a one-CTA kernel (~0.2 ms) that depends only on the token ids, so it
             # runs NOW on a side stream underneath the forward GEMMs instead of on the critical path at the end of the backward
             sorted_keys = torch.empty(t.numel(), dtype=torch.int64, device=weight.device)
+            n_chunks = (t.numel() + 16383) // 16384
             if torch.cuda.is_current_stream_capturing():
-                _lib.check(lib.pb_embedding_sort(t.data_ptr(), t.numel(), sorted_keys.data_ptr(), _stream()), "pb_embedding_sort")
+                _launch("pb_embedding_sort", t.data_ptr(), t.numel(), sorted_keys.data_ptr(), _stream(), n=n_chunks)
             else:
                 side = _side_stream(weight.device)
                 side.wait_stream(torch.cuda.current_stream())
                 with torch.cuda.stream(side):
-                    _lib.check(lib.pb_embedding_sort(t.data_ptr(), t.numel(), sorted_keys.data_ptr(), side.cuda_stream), "pb_embedding_sort")
+                    _launch("pb_embedding_sort", t.data_ptr(), t.numel(), sorted_keys.data_ptr(), side.cuda_stream, n=n_chunks)
                     ctx.sorted_ev = torch.cuda.Event()
                     ctx.sorted_ev.record(side)
                 t.record_stream(side)
                 sorted_keys.record_stream(side)
-            _count((t.numel() + 16383) // 16384)
             ctx.save_for_backward(sorted_keys)
         return out
 
     @staticmethod
     def backward(ctx, dout: torch.Tensor):
-        lib = _lib.load()
         if not ctx.saved_tensors:
             return None, None
         (sorted_keys,) = ctx.saved_tensors
         weight = ctx.weight
         V, dim = weight.shape
-        d2 = dout.reshape(-1, dim)
-        d2 = d2 if d2.is_contiguous() else d2.contiguous()
+        d2 = _rows(dout)
         main_grad = getattr(weight, "main_grad", None)
         if main_grad is not None:
             if _take_fresh(weight):
@@ -482,8 +447,7 @@ class _EmbeddingFn(torch.autograd.Function):
         if ctx.sorted_ev is not None:
             torch.cuda.current_stream().wait_event(ctx.sorted_ev)
         T = sorted_keys.numel()
-        _lib.check(lib.pb_embedding_scatter(sorted_keys.data_ptr(), T, d2.data_ptr(), grad.data_ptr(), dim, _stream()), "pb_embedding_scatter")
-        _count((T + 16383) // 16384)
+        _launch("pb_embedding_scatter", sorted_keys.data_ptr(), T, d2.data_ptr(), grad.data_ptr(), dim, _stream(), n=(T + 16383) // 16384)
         return None, (None if ret is None else ret.to(weight.dtype))
 
 
@@ -507,31 +471,20 @@ def embedding(tokens: torch.Tensor, weight: torch.Tensor) -> torch.Tensor:
 # --------------------------------------------------------------------------- RMSNorm
 
 
-def _accumulate_param_grad(param: torch.Tensor, grad_fp32: torch.Tensor | None):
-    """Helper for ops that produce fp32 weight grads."""
-    return None if grad_fp32 is None else grad_fp32.to(param.dtype)
-
-
 class _RMSNormFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, residual, weight, eps):
-        lib = _lib.load()
-        D = x.shape[-1]
-        x2 = x.reshape(-1, D)
-        x2 = x2 if x2.is_contiguous() else x2.contiguous()
-        R = x2.shape[0]
+        x2 = _rows(x)
+        R, D = x2.shape
         y = torch.empty(x.shape, dtype=x.dtype, device=x.device)
         rstd = torch.empty(R, dtype=torch.float32, device=x.device)
         if residual is not None:
-            r2 = residual.reshape(-1, D)
-            r2 = r2 if r2.is_contiguous() else r2.contiguous()
+            r2 = _rows(residual)
             h = torch.empty(x.shape, dtype=x.dtype, device=x.device)
         else:
             r2, h = None, x2
-        rc = lib.pb_rmsnorm_fwd(_ptr(x2), _ptr(r2), _ptr(weight), _ptr(y), _ptr(h) if residual is not None else None,
-                                _ptr(rstd), R, D, float(eps), _stream())  # fmt: skip
-        _lib.check(rc, "pb_rmsnorm_fwd")
-        _count()
+        _launch("pb_rmsnorm_fwd", _ptr(x2), _ptr(r2), _ptr(weight), _ptr(y), _ptr(h) if residual is not None else None,
+                _ptr(rstd), R, D, float(eps), _stream())  # fmt: skip
         ctx.save_for_backward(h, weight, rstd)
         ctx.has_res = residual is not None
         ctx.shape = x.shape
@@ -539,28 +492,20 @@ class _RMSNormFn(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, dy, dh):
-        lib = _lib.load()
         h, weight, rstd = ctx.saved_tensors
-        D = h.shape[-1]
-        R = h.numel() // D
-        dy2 = dy.reshape(R, D)
-        dy2 = dy2 if dy2.is_contiguous() else dy2.contiguous()
-        dres = None
-        if dh is not None:
-            dres = dh.reshape(R, D)
-            dres = dres if dres.is_contiguous() else dres.contiguous()
+        dy2 = _rows(dy)
+        R, D = dy2.shape
+        dres = None if dh is None else _rows(dh)
         dx = torch.empty(ctx.shape, dtype=h.dtype, device=h.device)
-        grid = lib.pb_rmsnorm_bwd_grid(R)
+        grid = _lib.load().pb_rmsnorm_bwd_grid(R)
         partial = torch.empty((grid, D), dtype=torch.float32, device=h.device)
         main_grad = getattr(weight, "main_grad", None)
         if main_grad is not None:
             dw32, acc = main_grad, 0 if _take_fresh(weight) else 1
         else:
             dw32, acc = torch.empty(D, dtype=torch.float32, device=h.device), 0
-        rc = lib.pb_rmsnorm_bwd(_ptr(dy2), _ptr(h), _ptr(weight), _ptr(rstd), _ptr(dres), _ptr(dx), _ptr(partial),
-                                _ptr(dw32), acc, R, D, _stream())  # fmt: skip
-        _lib.check(rc, "pb_rmsnorm_bwd")
-        _count(2)
+        _launch("pb_rmsnorm_bwd", _ptr(dy2), _ptr(h), _ptr(weight), _ptr(rstd), _ptr(dres), _ptr(dx), _ptr(partial),
+                _ptr(dw32), acc, R, D, _stream(), n=2)  # fmt: skip
         dxv = dx
         dw = None if main_grad is not None else dw32.to(weight.dtype)
         # residual-add backward: gradient flows identically to x and residual
@@ -583,45 +528,39 @@ def add_rmsnorm(x: torch.Tensor, residual: torch.Tensor, weight: torch.Tensor, e
 # --------------------------------------------------------------------------- RoPE (in place on fused QKV)
 
 
+def _rope_inplace(qkv: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor, n_heads: int, n_kv_heads: int, sign: float) -> None:
+    """Rotate (``sign`` 1) or un-rotate (``sign`` -1) the Q and K heads of a contiguous fused [B,S,(H+2Hkv)·D] tensor in place."""
+    total_heads = n_heads + 2 * n_kv_heads
+    _launch("pb_rope_inplace", _ptr(qkv), _ptr(cos), _ptr(sin), qkv.numel() // qkv.shape[-1], qkv.shape[1], n_heads + n_kv_heads,
+            total_heads, qkv.shape[-1] // total_heads, sign, _stream())  # fmt: skip
+
+
 class _RopeQKVFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, qkv, cos, sin, n_heads, n_kv_heads, seq_len):
+    def forward(ctx, qkv, cos, sin, n_heads, n_kv_heads):
         # qkv: [B, S, (H + 2*Hkv) * D] contiguous, produced by the QKV GEMM → rotate in place
-        lib = _lib.load()
-        total_heads = n_heads + 2 * n_kv_heads
-        D = qkv.shape[-1] // total_heads
-        tokens = qkv.numel() // qkv.shape[-1]
         assert qkv.is_contiguous()
-        rc = lib.pb_rope_inplace(_ptr(qkv), _ptr(cos), _ptr(sin), tokens, seq_len, n_heads + n_kv_heads, total_heads, D,
-                                 1.0, _stream())  # fmt: skip
-        _lib.check(rc, "pb_rope_inplace")
-        _count()
+        _rope_inplace(qkv, cos, sin, n_heads, n_kv_heads, 1.0)
         ctx.mark_dirty(qkv)
         ctx.save_for_backward(cos, sin)
-        ctx.meta = (n_heads, n_kv_heads, seq_len, D, total_heads)
+        ctx.meta = (n_heads, n_kv_heads)
         return qkv
 
     @staticmethod
     def backward(ctx, dqkv):
-        lib = _lib.load()
         cos, sin = ctx.saved_tensors
-        n_heads, n_kv_heads, seq_len, D, total_heads = ctx.meta
         # never rotate the incoming gradient in place: autograd may share that tensor with other consumers
         dqkv = dqkv.clone(memory_format=torch.contiguous_format)
-        tokens = dqkv.numel() // dqkv.shape[-1]
         # rotation is orthogonal: the backward is the inverse rotation, applied in place on the incoming grad
-        rc = lib.pb_rope_inplace(_ptr(dqkv), _ptr(cos), _ptr(sin), tokens, seq_len, n_heads + n_kv_heads, total_heads, D,
-                                 -1.0, _stream())  # fmt: skip
-        _lib.check(rc, "pb_rope_inplace(bwd)")
-        _count()
-        return dqkv, None, None, None, None, None
+        _rope_inplace(dqkv, cos, sin, *ctx.meta, -1.0)
+        return dqkv, None, None, None, None
 
 
 def rope_qkv(qkv: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor, n_heads: int, n_kv_heads: int) -> torch.Tensor:
     """Rotate the Q and K heads of a fused [B,S,(H+2Hkv)·D] activation."""
     B, S, W = qkv.shape
     if qkv.is_cuda:
-        return _RopeQKVFn.apply(qkv, cos, sin, n_heads, n_kv_heads, S)
+        return _RopeQKVFn.apply(qkv, cos, sin, n_heads, n_kv_heads)
     D = W // (n_heads + 2 * n_kv_heads)
     x = qkv.view(B, S, n_heads + 2 * n_kv_heads, D)
     rot = reference.rope(x[:, :, : n_heads + n_kv_heads], cos, sin)
@@ -634,28 +573,20 @@ def rope_qkv(qkv: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor, n_heads: i
 class _SwiGLUFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, gate_up):
-        lib = _lib.load()
-        F2 = gate_up.shape[-1]
-        gu = gate_up.reshape(-1, F2)
-        gu = gu if gu.is_contiguous() else gu.contiguous()
-        out = torch.empty((*gate_up.shape[:-1], F2 // 2), dtype=gu.dtype, device=gu.device)
-        rc = lib.pb_swiglu_fwd(_ptr(gu), _ptr(out), gu.shape[0], F2 // 2, _stream())
-        _lib.check(rc, "pb_swiglu_fwd")
-        _count()
+        gu = _rows(gate_up)
+        M, FF = gu.shape[0], gu.shape[1] // 2
+        out = torch.empty((*gate_up.shape[:-1], FF), dtype=gu.dtype, device=gu.device)
+        _launch("pb_swiglu_fwd", _ptr(gu), _ptr(out), M, FF, _stream())
         ctx.save_for_backward(gu)
         ctx.shape = gate_up.shape
         return out
 
     @staticmethod
     def backward(ctx, dout):
-        lib = _lib.load()
         (gu,) = ctx.saved_tensors
-        d2 = dout.reshape(gu.shape[0], -1)
-        d2 = d2 if d2.is_contiguous() else d2.contiguous()
+        d2 = _rows(dout)
         dgu = torch.empty(ctx.shape, dtype=gu.dtype, device=gu.device)
-        rc = lib.pb_swiglu_bwd(_ptr(gu), _ptr(d2), _ptr(dgu), gu.shape[0], gu.shape[1] // 2, _stream())
-        _lib.check(rc, "pb_swiglu_bwd")
-        _count()
+        _launch("pb_swiglu_bwd", _ptr(gu), _ptr(d2), _ptr(dgu), gu.shape[0], gu.shape[1] // 2, _stream())
         return dgu
 
 
@@ -667,50 +598,31 @@ def swiglu(gate_up: torch.Tensor) -> torch.Tensor:
 
 class _LinearSwiGLUFn(torch.autograd.Function):
     """h = silu(x W1ᵀ) · (x W3ᵀ) with W13 = [W1; W3]: ONE GEMM whose epilogue emits both the bf16 gate/up activations (kept for
-    the backward) and h — the separate SwiGLU pass over the 370 MB gate_up tensor disappears from the forward. CTA-pair GEMM:
-    the leader stages 128 gate rows of W13, its partner the matching 128 up rows."""
+    the backward) and h — the separate SwiGLU pass over the 370 MB gate_up tensor disappears from the forward."""
 
     @staticmethod
     def forward(ctx, x: torch.Tensor, w13: torch.Tensor) -> torch.Tensor:
-        lib = _lib.load()
-        x2 = x.reshape(-1, x.shape[-1])
-        if not x2.is_contiguous():
-            x2 = x2.contiguous()
-        M, K = x2.shape
+        x2 = _rows(x)
+        M = x2.shape[0]
         FF = w13.shape[0] // 2
         gate_up = torch.empty((M, 2 * FF), dtype=x.dtype, device=x.device)
         h = torch.empty((*x.shape[:-1], FF), dtype=x.dtype, device=x.device)
-        z = getattr(w13, "z3", None)
-        if z is not None:
-            gemm_wgather(x2, z, out=gate_up, swiglu_h=h.view(M, FF))
-        else:
-            rc = lib.pb_gemm_bf16_swiglu(x2.data_ptr(), w13.data_ptr(), gate_up.data_ptr(), h.data_ptr(), M, FF, K, x2.stride(0), w13.stride(0),
-                                         2 * FF, FF, _stream())  # fmt: skip
-            _lib.check(rc, "pb_gemm_bf16_swiglu")
-            _count()
+        _matmul(x2, w13, gate_up, swiglu_h=h.view(M, FF))
         ctx.save_for_backward(x2, w13, gate_up)
         ctx.x_shape = x.shape
         return h
 
     @staticmethod
     def backward(ctx, dh: torch.Tensor):
-        lib = _lib.load()
         x2, w13, gate_up = ctx.saved_tensors
         M, FF = gate_up.shape[0], gate_up.shape[1] // 2
-        d2 = dh.reshape(M, FF)
-        d2 = d2 if d2.is_contiguous() else d2.contiguous()
+        d2 = _rows(dh)
         dgu = torch.empty_like(gate_up)
-        rc = lib.pb_swiglu_bwd(_ptr(gate_up), _ptr(d2), _ptr(dgu), M, FF, _stream())
-        _lib.check(rc, "pb_swiglu_bwd")
-        _count()
+        _launch("pb_swiglu_bwd", _ptr(gate_up), _ptr(d2), _ptr(dgu), M, FF, _stream())
         dx = dw = None
         if ctx.needs_input_grad[0]:
             dx = torch.empty(ctx.x_shape, dtype=dh.dtype, device=dh.device)
-            z = getattr(w13, "z3", None)
-            if z is not None:
-                gemm_wgather(dgu, z, b_mn_major=True, out=dx.view(-1, ctx.x_shape[-1]))
-            else:
-                gemm(dgu, w13, b_mn_major=True, out=dx.view(-1, ctx.x_shape[-1]))
+            _matmul(dgu, w13, dx.view(-1, ctx.x_shape[-1]), b_mn_major=True)
         if ctx.needs_input_grad[1]:
             dw = _wgrad(dgu, x2, w13)
         return dx, dw
@@ -724,65 +636,29 @@ class _MLPSwiGLUFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, x: torch.Tensor, w13: torch.Tensor, w2: torch.Tensor) -> torch.Tensor:
-        lib = _lib.load()
-        x2 = x.reshape(-1, x.shape[-1])
-        if not x2.is_contiguous():
-            x2 = x2.contiguous()
-        M, K = x2.shape
+        x2 = _rows(x)
+        M = x2.shape[0]
         FF = w13.shape[0] // 2
         gate_up = torch.empty((M, 2 * FF), dtype=x.dtype, device=x.device)
         h = torch.empty((M, FF), dtype=x.dtype, device=x.device)
-        z13, z2 = getattr(w13, "z3", None), getattr(w2, "z3", None)
-        if z13 is not None:
-            gemm_wgather(x2, z13, out=gate_up, swiglu_h=h)
-        else:
-            rc = lib.pb_gemm_bf16_swiglu(x2.data_ptr(), w13.data_ptr(), gate_up.data_ptr(), h.data_ptr(), M, FF, K, x2.stride(0), w13.stride(0),
-                                         2 * FF, FF, _stream())  # fmt: skip
-            _lib.check(rc, "pb_gemm_bf16_swiglu")
-            _count()
+        _matmul(x2, w13, gate_up, swiglu_h=h)
         y = torch.empty((*x.shape[:-1], w2.shape[0]), dtype=x.dtype, device=x.device)
-        if z2 is not None:
-            gemm_wgather(h, z2, out=y.view(M, -1))
-        else:
-            gemm(h, w2, out=y.view(M, -1))
+        _matmul(h, w2, y.view(M, -1))
         ctx.save_for_backward(x2, w13, w2, gate_up, h)
         ctx.x_shape = x.shape
         return y
 
     @staticmethod
     def backward(ctx, dy: torch.Tensor):
-        lib = _lib.load()
         x2, w13, w2, gate_up, h = ctx.saved_tensors
-        M, FF = h.shape
-        dy2 = dy.reshape(M, -1)
-        if not dy2.is_contiguous():
-            dy2 = dy2.contiguous()
+        dy2 = _rows(dy)
         dw2 = _wgrad(dy2, h, w2) if ctx.needs_input_grad[2] else None
         dgu = torch.empty_like(gate_up)
-        z13, z2 = getattr(w13, "z3", None), getattr(w2, "z3", None)
-        if not _SWIGLU_BWD_FUSED:
-            # two kernels: dh = dy·W2 (plain / gather-fused dgrad), then the stand-alone SwiGLU backward (0.82 of the HBM roof)
-            dh = torch.empty((M, FF), dtype=dy.dtype, device=dy.device)
-            if z2 is not None:
-                gemm_wgather(dy2, z2, b_mn_major=True, out=dh)
-            else:
-                gemm(dy2, w2, b_mn_major=True, out=dh)
-            _lib.check(lib.pb_swiglu_bwd(_ptr(gate_up), _ptr(dh), _ptr(dgu), M, FF, _stream()), "pb_swiglu_bwd")
-            _count()
-        elif z2 is not None:
-            gemm_wgather(dy2, z2, b_mn_major=True, out=dgu, swiglu_bwd_gu=gate_up)
-        else:
-            rc = lib.pb_gemm_bf16_swiglu_bwd(dy2.data_ptr(), w2.data_ptr(), gate_up.data_ptr(), dgu.data_ptr(), M, FF, dy2.shape[1],
-                                             dy2.stride(0), w2.stride(0), gate_up.stride(0), dgu.stride(0), _stream())  # fmt: skip
-            _lib.check(rc, "pb_gemm_bf16_swiglu_bwd")
-            _count()
+        _matmul(dy2, w2, dgu, b_mn_major=True, swiglu_bwd_gu=gate_up)
         dx = dw13 = None
         if ctx.needs_input_grad[0]:
             dx = torch.empty(ctx.x_shape, dtype=dy.dtype, device=dy.device)
-            if z13 is not None:
-                gemm_wgather(dgu, z13, b_mn_major=True, out=dx.view(M, -1))
-            else:
-                gemm(dgu, w13, b_mn_major=True, out=dx.view(M, -1))
+            _matmul(dgu, w13, dx.view(-1, ctx.x_shape[-1]), b_mn_major=True)
         if ctx.needs_input_grad[1]:
             dw13 = _wgrad(dgu, x2, w13)
         return dx, dw13, dw2
@@ -810,7 +686,6 @@ def linear_swiglu(x: torch.Tensor, w13: torch.Tensor) -> torch.Tensor:
 class _CrossEntropyFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, logits, targets, ignore_index, grad_scale, unit_upstream, loss_acc):
-        lib = _lib.load()
         V = logits.shape[-1]
         z = logits.reshape(-1, V)
         assert z.is_contiguous()
@@ -820,10 +695,8 @@ class _CrossEntropyFn(torch.autograd.Function):
         work = torch.empty(R + 4, dtype=torch.float32, device=z.device)  # [0:2] scales, [2] loss, [4:] per-row losses
         # valid-target count → gradient scale, the fused row kernel (logits are overwritten with d(mean loss)/d(logits): nothing else
         # needs them afterwards) and a fixed-order sum of the row losses — three native launches, no framework kernel
-        rc = lib.pb_cross_entropy_loss(_ptr(z), _ptr(t), work[4:].data_ptr(), work.data_ptr(), work[2:].data_ptr(), _ptr(loss_acc), R, V,
-                                       ignore_index, float(grad_scale), _stream())  # fmt: skip
-        _lib.check(rc, "pb_cross_entropy_loss")
-        _count(3)
+        _launch("pb_cross_entropy_loss", _ptr(z), _ptr(t), work[4:].data_ptr(), work.data_ptr(), work[2:].data_ptr(), _ptr(loss_acc), R, V,
+                ignore_index, float(grad_scale), _stream(), n=3)  # fmt: skip
         # NOTE: deliberately not mark_dirty(): the logits are consumed, not returned; their storage now holds the gradient
         ctx.save_for_backward(z)
         ctx.shape = logits.shape

@@ -124,3 +124,16 @@ def test_native_launchers_validate_their_arguments_before_touching_the_device():
     assert lib.pb_outer_nesterov(ctypes.byref(pp), ctypes.byref(pp), None, None, None, 1024, ctypes.byref(oa), ctypes.byref(pp), None, None, 0, None, None) == -1  # no bucket table
     assert lib.pb_outer_nesterov_f32(ctypes.byref(pp), None, None, None, 1001, ctypes.byref(oa), ctypes.byref(pp), None, None, 1, None, None) == -1
     assert lib.pb_cast_push(None, 1001, ctypes.byref(pp), 0, None) == -1 and lib.pb_cast_push(None, 1024, ctypes.byref(pp), 3, None) == -1
+
+    doc = ctypes.c_int(0)  # never read: every call below is rejected before a kernel could see it
+    d = ctypes.addressof(doc)
+
+    def attn_fwd(doc_start=None, S=256, causal=1):
+        return lib.pb_flash_attn_fwd(None, None, None, doc_start, 1, S, 4, 2, 128, 0.1, causal, None)
+
+    def attn_bwd(doc_start=None, doc_end=None, S=256, causal=1):
+        return lib.pb_flash_attn_bwd(None, None, None, None, None, None, doc_start, doc_end, 1, S, 4, 2, 128, 0.1, causal, None, None, None)
+
+    assert attn_fwd(doc_start=d, causal=0) == -1 and attn_bwd(doc_start=d, doc_end=d, causal=0) == -1  # document masking is causal
+    assert attn_bwd(doc_start=d) == -1 and attn_bwd(doc_end=d) == -1  # the backward needs both bounds or neither
+    assert attn_fwd(S=200) == -1 and attn_bwd(S=200) == -1  # 128-row query / key blocks

@@ -288,7 +288,7 @@ def test_native_document_masked_attention_matches_reference(B, S, H, Hkv, D, lay
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("B,S,H,Hkv,D", [(2, 512, 4, 2, 128), (1, 1024, 8, 8, 64)])
+@pytest.mark.parametrize("B,S,H,Hkv,D", [(2, 512, 4, 2, 128), (1, 1024, 8, 8, 64), (1, 256, 4, 1, 128), (3, 384, 2, 2, 64)])
 def test_single_document_is_bitwise_causal(B, S, H, Hkv, D):
     """A row without EOS is one document: output, lse2 and gradients of the masked kernels equal the causal kernels' bit for bit."""
     import math
@@ -306,8 +306,8 @@ def test_single_document_is_bitwise_causal(B, S, H, Hkv, D):
     scale = 1.0 / math.sqrt(D)
     o1, o2 = (torch.empty(B, S, H * D, dtype=torch.bfloat16, device=_dev()) for _ in range(2))
     l1, l2 = (torch.empty(B, H, S, dtype=torch.float32, device=_dev()) for _ in range(2))
-    _lib.check(lib.pb_flash_attn_fwd(_ptr(qkv), _ptr(o1), _ptr(l1), B, S, H, Hkv, D, scale, 1, _stream()), "fwd")
-    _lib.check(lib.pb_flash_attn_fwd_doc(_ptr(qkv), _ptr(o2), _ptr(l2), _ptr(doc[0]), B, S, H, Hkv, D, scale, _stream()), "fwd_doc")
+    _lib.check(lib.pb_flash_attn_fwd(_ptr(qkv), _ptr(o1), _ptr(l1), None, B, S, H, Hkv, D, scale, 1, _stream()), "fwd")
+    _lib.check(lib.pb_flash_attn_fwd(_ptr(qkv), _ptr(o2), _ptr(l2), _ptr(doc[0]), B, S, H, Hkv, D, scale, 1, _stream()), "fwd doc")
     torch.cuda.synchronize()
     assert torch.equal(o1, o2) and torch.equal(l1, l2)
     dout = torch.randn(B, S, H * D, device=_dev()).to(torch.bfloat16)

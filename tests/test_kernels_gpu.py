@@ -298,7 +298,8 @@ def test_trainer_loss_decreases_on_gpu():
 
 
 # ------------------------------------------------------------------ native flash attention
-@pytest.mark.parametrize("B,S,H,Hkv,D", [(2, 256, 4, 4, 128), (1, 512, 4, 2, 128), (2, 384, 8, 8, 64), (1, 128, 2, 1, 64), (1, 1024, 2, 2, 128)])
+@pytest.mark.parametrize("B,S,H,Hkv,D", [(2, 256, 4, 4, 128), (1, 512, 4, 2, 128), (2, 384, 8, 8, 64), (1, 128, 2, 1, 64), (1, 1024, 2, 2, 128),
+                                         (3, 768, 2, 1, 128)])  # fmt: skip
 @pytest.mark.parametrize("causal", [True, False])
 def test_flash_attention_fwd_bwd(B, S, H, Hkv, D, causal):
     from prime_b200.ops import attention_native as A
@@ -321,34 +322,6 @@ def test_flash_attention_fwd_bwd(B, S, H, Hkv, D, causal):
     assert _rel_err(g[:, :, :H], gr[:, :, :H]) < 3e-2, f"dQ rel err {_rel_err(g[:, :, :H], gr[:, :, :H])}"
     assert _rel_err(g[:, :, H : H + Hkv], gr[:, :, H : H + Hkv]) < 3e-2, "dK"
     assert _rel_err(g[:, :, H + Hkv :], gr[:, :, H + Hkv :]) < 3e-2, "dV"
-
-
-@pytest.mark.parametrize("causal", [True, False])
-@pytest.mark.parametrize("B,S,H,Hkv,D", [(2, 256, 4, 4, 128), (1, 512, 4, 2, 128), (1, 1024, 2, 2, 128), (3, 768, 2, 1, 128)])
-def test_flash_attention_fwd_two_tile_kernel(B, S, H, Hkv, D, causal):
-    """Forward with the kernel-variant selector set to 2 (sm_90a has one forward kernel) against the same fp32 reference."""
-    from prime_b200.ops import _lib
-
-    lib = _lib.load()
-    old = lib.pb_flash_attn_fwd_set_variant(2)
-    try:
-        test_flash_attention_fwd_bwd(B, S, H, Hkv, D, causal)
-    finally:
-        lib.pb_flash_attn_fwd_set_variant(old)
-
-
-@pytest.mark.parametrize("variant", [0, 1, 2])
-@pytest.mark.parametrize("B,S,H,Hkv,D", [(1, 512, 4, 2, 128), (2, 384, 8, 8, 64)])
-def test_flash_attention_bwd_dkdv_variants(B, S, H, Hkv, D, variant):
-    """Every value of the dK/dV variant selector (sm_90a has one backward kernel) gives the reference gradients."""
-    from prime_b200.ops import _lib
-
-    lib = _lib.load()
-    old = lib.pb_flash_attn_bwd_set_variant(variant)
-    try:
-        test_flash_attention_fwd_bwd(B, S, H, Hkv, D, True)
-    finally:
-        lib.pb_flash_attn_bwd_set_variant(old)
 
 
 @pytest.mark.parametrize("H,Hkv,D", [(4, 4, 128), (8, 2, 64)])
@@ -375,46 +348,54 @@ def test_rope_attention_fused_node_matches_reference(H, Hkv, D):
     assert _rel_err(base.grad, ref_in.grad) < 3e-2
 
 
-@pytest.mark.parametrize("pair", [False, True])
+def _out_buffer(M, N, dtype, padded):
+    """(output view [M, N], full buffer): with ``padded`` the view is the first N columns of an [M, N + 8] buffer (row pitch
+    N + 8), so a kernel that ignores the output's row stride, or stores past column N, fails the caller's checks."""
+    full = torch.full((M, N + 8 if padded else N), 7.0, device=_dev(), dtype=dtype)
+    return full[:, :N], full
+
+
+@pytest.mark.parametrize("out_layout", ["dense_out", "padded_out"])
 @pytest.mark.parametrize("M,N,K,a_mn,b_mn", [(256, 256, 64, False, False), (384, 1000, 136, False, True), (640, 264, 4096, True, True), (4096, 4096, 1024, True, False)])
-def test_gemm_pair_and_single_schedulers_agree(pair, M, N, K, a_mn, b_mn):
-    """Both values of the tile-scheduler selector (sm_90a has one scheduler) give the reference result."""
+def test_gemm_transposed_layouts_at_larger_shapes(M, N, K, a_mn, b_mn, out_layout):
+    """Every K-major / MN-major operand combination against the fp32 reference, with ragged N and K and up to 4096² outputs, written
+    into a dense output or into the first N columns of a wider buffer (whose padding must stay untouched)."""
     from prime_b200 import ops
 
-    old = ops.set_gemm_pair_mode(pair)
-    try:
-        torch.manual_seed(M + N)
-        A = torch.randn(M, K, device=_dev(), dtype=torch.bfloat16) * 0.1
-        B = torch.randn(N, K, device=_dev(), dtype=torch.bfloat16) * 0.1
-        a = A.t().contiguous() if a_mn else A
-        b = B.t().contiguous() if b_mn else B
-        out = ops.gemm(a, b, a_mn_major=a_mn, b_mn_major=b_mn)
-        torch.cuda.synchronize()
-        assert _rel_err(out, A.float() @ B.float().t()) < 1e-2
-    finally:
-        ops.set_gemm_pair_mode(bool(old))
+    torch.manual_seed(M + N)
+    A = torch.randn(M, K, device=_dev(), dtype=torch.bfloat16) * 0.1
+    B = torch.randn(N, K, device=_dev(), dtype=torch.bfloat16) * 0.1
+    a = A.t().contiguous() if a_mn else A
+    b = B.t().contiguous() if b_mn else B
+    out, full = _out_buffer(M, N, torch.bfloat16, out_layout == "padded_out")
+    ops.gemm(a, b, a_mn_major=a_mn, b_mn_major=b_mn, out=out)
+    torch.cuda.synchronize()
+    assert _rel_err(out, A.float() @ B.float().t()) < 1e-2
+    assert bool((full[:, N:] == 7.0).all()), "store past column N"
 
 
+@pytest.mark.parametrize("out_layout", ["dense_out", "padded_out"])
 @pytest.mark.parametrize("split", [-1, 2, 3, 8])
-@pytest.mark.parametrize("pair", [False, True])
-def test_gemm_split_k_reduce_add(split, pair):
-    """Weight-gradient pattern: fp32 C += AᵀB with K sliced across work items, every slice TMA-reduce-adding its partial tile.
-    K = 17·64 + 8 is not divisible by any split (ragged last slice, and with split 8 an empty one)."""
+def test_gemm_split_k_reduce_add(split, out_layout):
+    """Weight-gradient pattern: fp32 C += AᵀB with K sliced across work items, every slice adding its partial tile into C.
+    K = 17·64 + 8 is not divisible by any split (ragged last slice, and with split 8 an empty one). C is dense or the first N
+    columns of a wider buffer, whose padding must stay untouched."""
     from prime_b200 import ops
 
-    old_p, old_s = ops.set_gemm_pair_mode(pair), ops.set_gemm_split_k(split)
+    old_s = ops.set_gemm_split_k(split)
     try:
         torch.manual_seed(3)
         M, N, K = 512, 768, 17 * 64 + 8
         A = torch.randn(K, M, device=_dev(), dtype=torch.bfloat16)
         B = torch.randn(K, N, device=_dev(), dtype=torch.bfloat16)
-        C = torch.randn(M, N, device=_dev(), dtype=torch.float32)
+        C, full = _out_buffer(M, N, torch.float32, out_layout == "padded_out")
+        C.copy_(torch.randn(M, N, device=_dev(), dtype=torch.float32))
         ref = C + A.float().t() @ B.float()
         ops.gemm(A, B, a_mn_major=True, b_mn_major=True, out=C, accumulate=True)
         torch.cuda.synchronize()
         assert _rel_err(C, ref) < 2e-3
+        assert bool((full[:, N:] == 7.0).all()), "store past column N"
     finally:
-        ops.set_gemm_pair_mode(bool(old_p))
         ops.set_gemm_split_k(old_s)
 
 
@@ -454,8 +435,7 @@ def test_qkv_gemm_rope_epilogue_and_attention_unrotate(H, Hkv, D):
 
 @pytest.mark.parametrize("M,FF,K", [(512, 1024, 256), (640, 5632, 2048), (384, 192, 136)])
 def test_gemm_swiglu_epilogue(M, FF, K):
-    """gate/up projection with SwiGLU in the epilogue (CTA pair: leader stages gate rows, partner the matching up rows) vs the
-    unfused linear → swiglu path, forward and gradients."""
+    """gate/up projection with SwiGLU in the epilogue vs the unfused linear → swiglu path, forward and gradients."""
     from prime_b200 import ops
 
     torch.manual_seed(M + FF)
@@ -495,20 +475,11 @@ def test_quantize_mxfp8_matches_reference(R, C, transpose):
     assert _rel_err(deq, tgt) < 0.04
 
 
-@pytest.mark.parametrize("pair", [False, True])
+@pytest.mark.parametrize("out_layout", ["dense_out", "padded_out"])
 @pytest.mark.parametrize("M,N,K", [(128, 192, 128), (256, 384, 512), (300, 520, 256), (1024, 2112, 1024), (4096, 3072, 2048), (136, 8, 128)])
-def test_gemm_mxfp8_matches_dequantized_reference(M, N, K, pair):
-    from prime_b200 import ops
-    from prime_b200.ops import reference as Rf
-
-    old = ops.set_mxfp8_pair_mode(pair)
-    try:
-        _check_gemm_mxfp8(M, N, K)
-    finally:
-        ops.set_mxfp8_pair_mode(None if old < 0 else bool(old))
-
-
-def _check_gemm_mxfp8(M, N, K):
+def test_gemm_mxfp8_matches_dequantized_reference(M, N, K, out_layout):
+    """``dense_out``: the op allocates C. ``padded_out``: C is the first N columns of a wider buffer, whose padding must stay
+    untouched."""
     from prime_b200 import ops
     from prime_b200.ops import reference as Rf
 
@@ -519,11 +490,16 @@ def _check_gemm_mxfp8(M, N, K):
     A[:, K // 2 :] *= 4  # and across K blocks
     aq, asf = ops.quantize_mxfp8(A)
     bq, bsf = ops.quantize_mxfp8(B)
-    out = ops.gemm_mxfp8(aq, asf, bq, bsf)
+    if out_layout == "padded_out":
+        out, full = _out_buffer(M, N, torch.bfloat16, True)
+        ops.gemm_mxfp8(aq, asf, bq, bsf, out=out)
+    else:
+        out = full = ops.gemm_mxfp8(aq, asf, bq, bsf)
     torch.cuda.synchronize()
     ref = Rf.dequantize_mxfp8(aq, asf) @ Rf.dequantize_mxfp8(bq, bsf).t()
     assert _rel_err(out, ref) < 6e-3, f"rel err {_rel_err(out, ref)}"
     assert _rel_err(out, A.float() @ B.float().t()) < 0.06  # and the quantisation itself is sane
+    assert bool((full[:, N:] == 7.0).all()), "store past column N"
 
 
 def test_linear_mxfp8_autograd():

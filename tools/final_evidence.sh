@@ -8,7 +8,6 @@ python bench.py --steps 10 --warmup 3 2>gpurun_out/bench_final.err | tee gpurun_
 python bench.py --steps 6 --warmup 3 --no-fused-comm --attn sdpa 2>/dev/null | tee gpurun_out/bench_b0_sdpa_nccl.json | cut -c1-160
 python tools/attn_bench.py > gpurun_out/attn_bench_final.json 2>/dev/null
 python tools/op_bench.py > gpurun_out/op_bench_final.json 2>/dev/null
-python tools/attn_trace.py > gpurun_out/attn_trace_final.json 2>/dev/null
 bash tools/profile.sh 2>&1 | tail -6
 bash tools/sanitize.sh 2>&1 | tail -8
 du -sh gpurun_out

@@ -41,9 +41,6 @@ def main():
         out = torch.empty(M, N, device=dev, dtype=torch.bfloat16)
         aq, asf = ops.quantize_mxfp8(a)
         bq, bsf = ops.quantize_mxfp8(b)
-        ops.set_mxfp8_pair_mode(False)
-        t_fp8_single = timeit(lambda: ops.gemm_mxfp8(aq, asf, bq, bsf, out=out), flush)
-        ops.set_mxfp8_pair_mode(True)
         t_fp8 = timeit(lambda: ops.gemm_mxfp8(aq, asf, bq, bsf, out=out), flush)
         t_bf16 = timeit(lambda: ops.gemm(a, b, out=out), flush)
         t_qa = timeit(lambda: ops.quantize_mxfp8(a), flush)
@@ -51,7 +48,6 @@ def main():
         t_qbt = timeit(lambda: ops.quantize_mxfp8(b, transpose=True), flush) if N % 128 == 0 else None
         fl = 2.0 * M * N * K
         rows.append({"shape": name, "M": M, "N": N, "K": K, "mxfp8_ms": round(t_fp8, 4), "mxfp8_tflops": round(fl / t_fp8 / 1e9, 1),
-                     "mxfp8_single_cta_ms": round(t_fp8_single, 4), "mxfp8_single_cta_tflops": round(fl / t_fp8_single / 1e9, 1),
                      "bf16_ms": round(t_bf16, 4), "bf16_tflops": round(fl / t_bf16 / 1e9, 1), "speedup": round(t_bf16 / t_fp8, 3),
                      "quantize_act_ms": round(t_qa, 4), "quantize_act_GBps": round(M * K * 3 / t_qa / 1e6, 1),
                      "quantize_w_ms": round(t_qb, 4), "quantize_w_transposed_ms": None if t_qbt is None else round(t_qbt, 4)})  # fmt: skip

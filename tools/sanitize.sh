@@ -12,9 +12,9 @@ run() { # tool, pytest -k expression, tag
 : > gpurun_out/sanitizer_summary.txt
 run memcheck  "rmsnorm or swiglu or rope_qkv or cross_entropy" memcheck_elementwise
 run memcheck  "gemm_layouts or gemm_fp32 or split_k" memcheck_gemm
-run memcheck  "flash_attention or rope_attention or two_tile or dkdv_variants" memcheck_attention
+run memcheck  "flash_attention or rope_attention" memcheck_attention
 run racecheck "rmsnorm or cross_entropy" racecheck_elementwise
-run synccheck "gemm_pair or flash_attention or rope_attention or qkv_gemm_rope or two_tile or dkdv_variants" synccheck_tc
+run synccheck "gemm_transposed or flash_attention or rope_attention or qkv_gemm_rope" synccheck_tc
 run memcheck  "mxfp8" memcheck_mxfp8
 run synccheck "mxfp8 or swiglu_epilogue" synccheck_mxfp8
 cat gpurun_out/sanitizer_summary.txt
