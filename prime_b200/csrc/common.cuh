@@ -16,8 +16,6 @@
 
 namespace pb {
 
-constexpr int kWarp = 32;
-
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
@@ -127,9 +125,6 @@ __device__ __forceinline__ void red_add_release_gpu_u32(uint32_t* p, uint32_t v)
 }
 __device__ __forceinline__ void st_release_sys_u32(uint32_t* p, uint32_t v) {
   asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
-}
-__device__ __forceinline__ void red_add_release_sys_u32(uint32_t* p, uint32_t v) {
-  asm volatile("red.release.sys.global.add.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
 }
 
 }  // namespace pb

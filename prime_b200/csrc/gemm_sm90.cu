@@ -16,12 +16,22 @@
 // the producer already fills the ring for the next tile.
 #include <cuda.h>
 
-#include <mutex>
-#include <unordered_map>
-
 #include "common.cuh"
 #include "tc_common.cuh"
 #include "tmap.h"
+
+// Fused epilogue of pb_gemm_bf16 / pb_gemm_wgather; a null descriptor means plain. Mirrored by ops/_lib.py: GemmEpilogue.
+struct GemmEpilogue {
+  int kind;  // 0 plain, 1 RoPE, 2 SwiGLU, 3 SwiGLU backward
+  // RoPE (the fused QKV projection): output columns [0, rope_cols) are heads of width rope_D (64 | 128); output row r is token r
+  // of a [B, rope_S] batch; cos / sin are fp32 [>= rope_S, rope_D/2]
+  const float* rope_cos;
+  const float* rope_sin;
+  int rope_S, rope_cols, rope_D;
+  // SwiGLU: h [M, FF] (written); SwiGLU backward: the saved gate_up [M, 2·FF] (read)
+  void* aux;
+  int ld_aux;
+};
 
 namespace {
 
@@ -583,9 +593,11 @@ int choose_split_k(int tiles, int units, int num_kb) {
 
 int g_split_k_mode = -1;  // -1 auto, 0/1 off, n>1 forced
 
-template <int A_MN, int B_MN, int EPI = 0, int IO = 0>
-int launch(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, int max_ctas, cudaStream_t stream,
-           const PeerMaps* pmp = nullptr, const CUtensorMap* tgp = nullptr, const CUtensorMap* tg2p = nullptr) {
+const GemmEpilogue kPlain = {};
+
+template <int A_MN, int B_MN, int EPI, int IO>
+int launch(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, cudaStream_t stream, const PeerMaps* pmp,
+           const CUtensorMap* tgp, const CUtensorMap* tg2p) {
   static const PeerMaps kNoPeers = {};
   const PeerMaps& pm = pmp ? *pmp : kNoPeers;
   const CUtensorMap& tg = tgp ? *tgp : ta;
@@ -600,7 +612,6 @@ int launch(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, in
   }
   if (g_num_sms == 0) g_num_sms = pbhost::num_sms();
   int grid = g_num_sms;
-  if (max_ctas > 0 && max_ctas < grid) grid = max_ctas;
   const int tiles_n = EPI == 2 ? p.swiglu_ff / 64 : (p.N + BN - 1) / BN;
   const int tiles = ((p.M + BM - 1) / BM) * tiles_n * p.split_k;
   // IO = 1 / 3 need every CTA resident at once (tiles wait on flags other CTAs publish): the grid never exceeds the SM count
@@ -608,6 +619,89 @@ int launch(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, in
   gemm_bf16_kernel<A_MN, B_MN, EPI, IO><<<grid, kThreads, G::kSmemBytes, stream>>>(ta, tb, tg, tg2, p, pm);
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? 0 : (int)e;
+}
+
+constexpr int variant(int io, int epi, int a_mn, int b_mn) { return io << 4 | epi << 2 | a_mn << 1 | b_mn; }
+
+// (I/O mode, epilogue, operand layouts) → kernel. These 16 instantiations are all the entry points accept: every layout for the
+// plain local GEMM, RoPE / SwiGLU on K-major B, SwiGLU backward on MN-major B, and K-major A for the collective modes.
+int dispatch(int io, int epi, const GemmParams& p, const CUtensorMap& ta, const CUtensorMap& tb, cudaStream_t stream,
+             const PeerMaps* pm = nullptr, const CUtensorMap* tg = nullptr, const CUtensorMap* tg2 = nullptr) {
+  switch (variant(io, epi, p.a_mn, p.b_mn)) {
+#define PB_GEMM_VARIANT(IO, EPI, A_MN, B_MN) \
+  case variant(IO, EPI, A_MN, B_MN):         \
+    return launch<A_MN, B_MN, EPI, IO>(ta, tb, p, stream, pm, tg, tg2);
+    PB_GEMM_VARIANT(0, 0, 0, 0)
+    PB_GEMM_VARIANT(0, 0, 0, 1)
+    PB_GEMM_VARIANT(0, 0, 1, 0)
+    PB_GEMM_VARIANT(0, 0, 1, 1)
+    PB_GEMM_VARIANT(0, 1, 0, 0)
+    PB_GEMM_VARIANT(0, 2, 0, 0)
+    PB_GEMM_VARIANT(0, 3, 0, 1)
+    PB_GEMM_VARIANT(1, 0, 0, 0)
+    PB_GEMM_VARIANT(1, 0, 0, 1)
+    PB_GEMM_VARIANT(2, 0, 0, 0)
+    PB_GEMM_VARIANT(2, 0, 0, 1)
+    PB_GEMM_VARIANT(3, 0, 0, 0)
+    PB_GEMM_VARIANT(3, 0, 0, 1)
+    PB_GEMM_VARIANT(3, 1, 0, 0)
+    PB_GEMM_VARIANT(3, 2, 0, 0)
+    PB_GEMM_VARIANT(3, 3, 0, 1)
+#undef PB_GEMM_VARIANT
+    default:
+      return -7;
+  }
+}
+
+// Argument rules of the fused epilogues, for both entry points; N is the N of the product A·Bᵀ (2·FF for SwiGLU, FF for SwiGLU
+// backward). -7: the epilogue does not exist for this layout / output; -3 / -4: RoPE tables / geometry; -5: SwiGLU geometry.
+int check_epilogue(const GemmEpilogue& e, int M, int N, int a_mn, int b_mn, int c_fp32, int accumulate) {
+  if (e.kind == 0) return 0;
+  if (e.kind < 0 || e.kind > 3 || a_mn || b_mn != (e.kind == 3) || c_fp32 || accumulate) return -7;
+  if (e.kind == 1) {
+    if (e.rope_cos == nullptr || e.rope_sin == nullptr || e.rope_S <= 0 || M % e.rope_S != 0) return -3;
+    if ((e.rope_D != 64 && e.rope_D != 128) || e.rope_cols % e.rope_D != 0 || e.rope_cols > N) return -4;
+    return 0;
+  }
+  // a tile covers 64 features; aux rows are read / written as 16-byte aligned bf16 pairs
+  if (N % (e.kind == 2 ? 128 : 64) != 0 || e.aux == nullptr || (e.ld_aux % 8) || (reinterpret_cast<uintptr_t>(e.aux) & 15)) return -5;
+  if (e.kind == 3 && M <= BM) return -5;
+  return 0;
+}
+
+GemmParams make_params(void* C, int M, int N, int K, int ldc, int a_mn, int b_mn, int c_fp32, int accumulate, const GemmEpilogue& e) {
+  GemmParams p = {};
+  p.M = M;
+  p.N = N;
+  p.K = K;
+  p.ldc = ldc;
+  p.a_mn = a_mn != 0;
+  p.b_mn = b_mn != 0;
+  p.c_fp32 = c_fp32;
+  p.accumulate = accumulate;
+  p.split_k = 1;
+  p.C = C;
+  p.rope_cos = e.rope_cos;
+  p.rope_sin = e.rope_sin;
+  p.rope_S = e.rope_S;
+  p.rope_cols = e.rope_cols;
+  p.rope_D = e.rope_D;
+  if (e.kind == 2) {
+    p.swiglu_ff = N / 2;
+    p.H = e.aux;
+    p.ldh = e.ld_aux;
+  } else if (e.kind == 3) {
+    p.swiglu_ff = N;
+    p.aux = e.aux;
+    p.ld_aux = e.ld_aux;
+  }
+  return p;
+}
+
+// A / B operand tensor maps: K-major {64 k, rows} boxes, MN-major {64 mn, 64 k} boxes.
+int operand_tmap(CUtensorMap* m, const void* ptr, int mn, int K, int ld, int mn_major, int box_rows) {
+  return mn_major ? pbhost::cached_tmap(m, ptr, (uint64_t)K, (uint64_t)mn, (uint64_t)ld, 64, BK)
+                  : pbhost::cached_tmap(m, ptr, (uint64_t)mn, (uint64_t)K, (uint64_t)ld, BK, box_rows);
 }
 
 }  // namespace
@@ -619,79 +713,32 @@ PB_EXPORT int pb_gemm_set_split_k(int mode) {
   return old;
 }
 
-// A / B operand tensor maps: K-major {64 k, rows} boxes, MN-major {64 mn, 64 k} boxes.
-static int operand_tmap(CUtensorMap* m, const void* ptr, int mn, int K, int ld, int mn_major, int box_rows) {
-  return mn_major ? pbhost::cached_tmap(m, ptr, (uint64_t)K, (uint64_t)mn, (uint64_t)ld, 64, BK)
-                  : pbhost::cached_tmap(m, ptr, (uint64_t)mn, (uint64_t)K, (uint64_t)ld, BK, box_rows);
-}
-
+// C[M, N] (bf16 | fp32, += with `accumulate`) = A·Bᵀ, optionally with a fused epilogue (null `epi` = plain).
 // lda/ldb: row stride (elements) of the matrix AS STORED (see header comment).
-static int gemm_impl(const void* A, const void* B, void* C, int M, int N, int K, int lda, int ldb, int ldc, int a_mn_major,
-                     int b_mn_major, int c_fp32, int accumulate, int max_ctas, const float* rope_cos, const float* rope_sin,
-                     int rope_S, int rope_cols, int rope_D, cudaStream_t stream, void* H = nullptr, int ldh = 0, int swiglu_ff = 0) {
+//   RoPE:            y = x·Wᵀ with the Q/K head columns rotated (the fused QKV projection)
+//   SwiGLU:          gate_up = x·W13ᵀ [M, N = 2·FF] with W13 = [gate rows | up rows] into C, and h = silu(gate)·up into epi->aux
+//   SwiGLU backward: dh = dy·W2 [M, N = FF] never leaves registers: C = d_gate_up [M, 2·FF] from dh and the saved gate_up (epi->aux)
+// RoPE and SwiGLU take K-major operands, SwiGLU backward K-major A and MN-major B; all three write bf16 without accumulating.
+PB_EXPORT int pb_gemm_bf16(const void* A, const void* B, void* C, int M, int N, int K, int lda, int ldb, int ldc, int a_mn_major,
+                           int b_mn_major, int c_fp32, int accumulate, const GemmEpilogue* epi, cudaStream_t stream) {
+  const GemmEpilogue& e = epi ? *epi : kPlain;
+  int rc;
+  if ((rc = check_epilogue(e, M, N, a_mn_major, b_mn_major, c_fp32, accumulate))) return rc;
   if (M <= 0 || N <= 0 || K <= 0) return 0;
   if ((lda % 8) || (ldb % 8) || (ldc % (c_fp32 ? 4 : 8))) return -1;
   if ((reinterpret_cast<uintptr_t>(A) | reinterpret_cast<uintptr_t>(B) | reinterpret_cast<uintptr_t>(C)) & 15) return -2;
   CUtensorMap ta, tb;
-  int rc;
   if ((rc = operand_tmap(&ta, A, M, K, lda, a_mn_major, BM))) return rc;
-  if ((rc = operand_tmap(&tb, B, N, K, ldb, b_mn_major, swiglu_ff > 0 ? 64 : BN))) return rc;
-  GemmParams p{M, N, K, ldc, a_mn_major, b_mn_major, c_fp32, accumulate, 1, C, rope_cos, rope_sin, rope_S, rope_cols, rope_D, swiglu_ff,
-               0, nullptr, 0, H, ldh};
+  if ((rc = operand_tmap(&tb, B, N, K, ldb, b_mn_major, e.kind == 2 ? 64 : BN))) return rc;
+  GemmParams p = make_params(C, M, N, K, ldc, a_mn_major, b_mn_major, c_fp32, accumulate, e);
   if (c_fp32 && accumulate && g_split_k_mode != 0 && g_split_k_mode != 1) {
     if (g_num_sms == 0) g_num_sms = pbhost::num_sms();
-    const int units = (max_ctas > 0 && max_ctas < g_num_sms) ? max_ctas : g_num_sms;
+    const int units = g_num_sms > 0 ? g_num_sms : 1;
     const int tiles = ((M + BM - 1) / BM) * ((N + BN - 1) / BN);
     const int num_kb = (K + BK - 1) / BK;
-    p.split_k = g_split_k_mode > 1 ? (num_kb / g_split_k_mode >= 1 ? g_split_k_mode : 1) : choose_split_k(tiles, units > 0 ? units : 1, num_kb);
+    p.split_k = g_split_k_mode > 1 ? (num_kb / g_split_k_mode >= 1 ? g_split_k_mode : 1) : choose_split_k(tiles, units, num_kb);
   }
-  if (swiglu_ff > 0) return launch<0, 0, 2>(ta, tb, p, max_ctas, stream);
-  if (rope_cos != nullptr) return launch<0, 0, 1>(ta, tb, p, max_ctas, stream);
-  if (!a_mn_major && !b_mn_major) return launch<0, 0>(ta, tb, p, max_ctas, stream);
-  if (!a_mn_major && b_mn_major) return launch<0, 1>(ta, tb, p, max_ctas, stream);
-  if (a_mn_major && !b_mn_major) return launch<1, 0>(ta, tb, p, max_ctas, stream);
-  return launch<1, 1>(ta, tb, p, max_ctas, stream);
-}
-
-PB_EXPORT int pb_gemm_bf16(const void* A, const void* B, void* C, int M, int N, int K, int lda, int ldb, int ldc,
-                           int a_mn_major, int b_mn_major, int c_fp32, int accumulate, int max_ctas,
-                           cudaStream_t stream) {
-  return gemm_impl(A, B, C, M, N, K, lda, ldb, ldc, a_mn_major, b_mn_major, c_fp32, accumulate, max_ctas, nullptr, nullptr, 1, 0, 64,
-                   stream);
-}
-
-// y = x·Wᵀ with RoPE applied to output columns [0, rope_cols) in the epilogue (the fused QKV projection). Row r of the output is
-// token r of a [B, S] batch (position r % S); heads are rope_D wide; cos/sin are fp32 [>=S, rope_D/2]. bf16 output, K-major operands.
-PB_EXPORT int pb_gemm_bf16_rope(const void* A, const void* B, void* C, int M, int N, int K, int lda, int ldb, int ldc, int max_ctas,
-                                const float* rope_cos, const float* rope_sin, int rope_S, int rope_cols, int rope_D,
-                                cudaStream_t stream) {
-  if (rope_cos == nullptr || rope_sin == nullptr || rope_S <= 0 || M % rope_S != 0) return -3;
-  if ((rope_D != 64 && rope_D != 128) || rope_cols % rope_D != 0 || rope_cols > N) return -4;
-  return gemm_impl(A, B, C, M, N, K, lda, ldb, ldc, 0, 0, 0, 0, max_ctas, rope_cos, rope_sin, rope_S, rope_cols, rope_D, stream);
-}
-
-// gate_up = x·W13ᵀ (kept for the backward) AND h = silu(gate)·up in ONE kernel: see GemmParams::swiglu_ff.
-//   x [M, K], W13 [2·FF, K] = [gate rows | up rows], gate_up [M, 2·FF], h [M, FF]; all bf16, unit inner stride.
-PB_EXPORT int pb_gemm_bf16_swiglu(const void* A, const void* W13, void* gate_up, void* H, int M, int FF, int K, int lda, int ldb,
-                                  int ld_gu, int ld_h, cudaStream_t stream) {
-  if (FF % 64 != 0 || (ld_h % 8) || (reinterpret_cast<uintptr_t>(H) & 15)) return -5;
-  return gemm_impl(A, W13, gate_up, M, 2 * FF, K, lda, ldb, ld_gu, 0, 0, 0, 0, 0, nullptr, nullptr, 1, 0, 64, stream, H, ld_h, FF);
-}
-
-// d_gate_up = swiglu'(gate_up) ⊙ (dy·W2) in ONE kernel (EPI = 3): dy [M, K=dim], W2 [dim, FF] (MN-major B: the contraction runs over
-// its rows), gate_up [M, 2·FF] saved by the forward, d_gate_up [M, 2·FF]. bf16, unit inner strides, M > 128.
-PB_EXPORT int pb_gemm_bf16_swiglu_bwd(const void* dY, const void* W2, const void* gate_up, void* d_gate_up, int M, int FF, int K,
-                                      int lda, int ldb, int ld_gu, int ld_dgu, cudaStream_t stream) {
-  if (M <= BM || FF % 64 != 0) return -5;
-  if ((lda % 8) || (ldb % 8) || (ld_gu % 8) || (ld_dgu % 8)) return -1;
-  if ((reinterpret_cast<uintptr_t>(dY) | reinterpret_cast<uintptr_t>(W2) | reinterpret_cast<uintptr_t>(gate_up) |
-       reinterpret_cast<uintptr_t>(d_gate_up)) & 15) return -2;
-  CUtensorMap ta, tb;
-  int rc;
-  if ((rc = operand_tmap(&ta, dY, M, K, lda, 0, BM))) return rc;
-  if ((rc = operand_tmap(&tb, W2, FF, K, ldb, 1, BN))) return rc;
-  GemmParams p{M, FF, K, ld_dgu, 0, 1, 0, 0, 1, d_gate_up, nullptr, nullptr, 1, 0, 64, FF, 0, gate_up, ld_gu, nullptr, 0};
-  return launch<0, 1, 3>(ta, tb, p, 0, stream);
+  return dispatch(0, e.kind, p, ta, tb, stream);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------------
@@ -729,8 +776,7 @@ PB_EXPORT int pb_gemm_allgather(const void* const* a_peers, int n, int rank, con
   CUtensorMap tfull, tb;
   if ((rc = pbhost::cached_tmap(&tfull, a_full, (uint64_t)M, (uint64_t)K, (uint64_t)K, BK, BM))) return rc;
   if ((rc = operand_tmap(&tb, B, N, K, ldb, b_mn_major, BN))) return rc;
-  GemmParams p{M, N, K, ldc, 0, b_mn_major, 0, 0, 1, C, nullptr, nullptr, 1, 0, 64, 0, 0, nullptr, 0, nullptr, 0};
-  return b_mn_major ? launch<0, 1, 0, 1>(tfull, tb, p, 0, stream, &pm) : launch<0, 0, 0, 1>(tfull, tb, p, 0, stream, &pm);
+  return dispatch(1, 0, make_params(C, M, N, K, ldc, 0, b_mn_major, 0, 0, kPlain), tfull, tb, stream, &pm);
 }
 
 // GEMM ⊕ reduce-scatter:  every rank holds a K-shard (A [M, K_local], B [N, K_local]); rank r ends up with rows
@@ -746,40 +792,30 @@ PB_EXPORT int pb_gemm_reduce_scatter(const void* A, const void* B, float* const*
   for (int r = 0; r < n; ++r) pm.c[r] = c_peers[r];
   int rc;
   CUtensorMap ta, tb;
-  if ((rc = pbhost::cached_tmap(&ta, A, (uint64_t)M, (uint64_t)K, (uint64_t)lda, BK, BM))) return rc;
+  if ((rc = operand_tmap(&ta, A, M, K, lda, 0, BM))) return rc;
   if ((rc = operand_tmap(&tb, B, N, K, ldb, b_mn_major, BN))) return rc;
-  GemmParams p{M, N, K, ldc, 0, b_mn_major, 1, 1, 1, c_peers[rank], nullptr, nullptr, 1, 0, 64, 0, 0, nullptr, 0, nullptr, 0};
-  return b_mn_major ? launch<0, 1, 0, 2>(ta, tb, p, 0, stream, &pm) : launch<0, 0, 0, 2>(ta, tb, p, 0, stream, &pm);
+  return dispatch(2, 0, make_params(c_peers[rank], M, N, K, ldc, 0, b_mn_major, 1, 1, kPlain), ta, tb, stream, &pm);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------------
 // parameter all-gather ⊕ GEMM (IO = 3; ZeRO-3 / train.reshard_after_forward): the weight W [rowsW, colsW] is sharded by rows
 // over n ranks (rank r: rows [r·rowsW/n, (r+1)·rowsW/n) at w_peers[r], the address AS MAPPED IN THIS PROCESS). The kernel gathers
 // it into w_full (local, [rowsW, colsW]) tile by tile WHILE it multiplies; no collective, no barrier (shards are read-only here).
-//   b_mn_major = 0 (forward)        C[M, rowsW] = A[M, colsW] · Wᵀ          epi: 0 plain | 1 RoPE on the leading columns | 2 SwiGLU
-//   b_mn_major = 1 (input gradient) C[M, colsW] = A[M, rowsW] · W           epi 0 only
-// SwiGLU: W = W13 [2·FF, colsW] = [gate rows | up rows], C = gate_up [M, 2·FF], H = silu(gate)·up [M, FF].
-// flags: n·4 uint32 in local memory (zeroed here, on the stream). bf16 everywhere, M > 128.
-// epi = 3 (with b_mn_major = 1): SwiGLU-backward epilogue, W = W2 [dim, FF]; H = the saved gate_up [M, 2·FF] (read), C = d_gate_up.
+//   b_mn_major = 0 (forward)        C[M, rowsW] = A[M, colsW] · Wᵀ          epilogue: plain | RoPE | SwiGLU (W = W13, N = 2·FF)
+//   b_mn_major = 1 (input gradient) C[M, colsW] = A[M, rowsW] · W           epilogue: plain | SwiGLU backward (W = W2, N = FF)
+// `epi` as for pb_gemm_bf16. flags: n·4 uint32 in local memory (zeroed here, on the stream). bf16 everywhere, M > 128.
 // own_resident = 1: W is already complete in w_full (gathered ahead by the previous kernel): no gather, no gating.
 // next_peers != nullptr: additionally gather the weight [next_rows, next_cols] (same n ranks) the NEXT GEMM will consume into
 // next_full — un-gated, complete when this kernel retires.
-PB_EXPORT int pb_gemm_wgather(const void* A, const void* const* w_peers, int n, int rank, void* w_full, uint32_t* flags, void* C,
-                              void* H, int M, int rowsW, int colsW, int lda, int ldc, int ldh, int b_mn_major, int epi,
-                              const float* rope_cos, const float* rope_sin, int rope_S, int rope_cols, int rope_D,
-                              int own_resident, const void* const* next_peers, void* next_full, int next_rows, int next_cols,
-                              cudaStream_t stream) {
+PB_EXPORT int pb_gemm_wgather(const void* A, const void* const* w_peers, int n, int rank, void* w_full, uint32_t* flags, void* C, int M,
+                              int rowsW, int colsW, int lda, int ldc, int b_mn_major, const GemmEpilogue* epi, int own_resident,
+                              const void* const* next_peers, void* next_full, int next_rows, int next_cols, cudaStream_t stream) {
+  const GemmEpilogue& e = epi ? *epi : kPlain;
   if (n < 1 || n > 8 || rank < 0 || rank >= n || rowsW % n != 0 || colsW % 64 != 0) return -6;
   if ((lda % 8) || (ldc % 8)) return -1;
-  if ((epi == 1 || epi == 2) && b_mn_major) return -7;
-  if (epi == 3 && !b_mn_major) return -7;
   const int N = b_mn_major ? colsW : rowsW, K = b_mn_major ? rowsW : colsW;
-  const int FF = epi == 2 ? rowsW / 2 : (epi == 3 ? colsW : 0);
-  if ((epi == 2 || epi == 3) && (FF % 64 != 0 || H == nullptr || (ldh % 8))) return -5;
-  if (epi == 1) {
-    if (rope_cos == nullptr || rope_sin == nullptr || rope_S <= 0 || M % rope_S != 0) return -3;
-    if ((rope_D != 64 && rope_D != 128) || rope_cols % rope_D != 0 || rope_cols > N) return -4;
-  }
+  int rc;
+  if ((rc = check_epilogue(e, M, N, 0, b_mn_major, 0, 0))) return rc;
   if (M <= BM) return -8;  // training shapes only; tiny M goes through an explicit gather on the host side
   const int rpr = rowsW / n;
   PeerMaps pm = {};
@@ -800,13 +836,12 @@ PB_EXPORT int pb_gemm_wgather(const void* A, const void* const* w_peers, int n, 
     pm.ncpr = (nrpr + 127) / 128;
     pm.ncol_chunks = next_cols / 64;
     for (int t = 0; t < n; ++t) pm.norder[t] = (rank + 1 + t) % n;  // remote blocks first (they take longest), own block last
-    int rc2;
     for (int r = 0; r < n; ++r)
-      if ((rc2 = pbhost::cached_tmap(&pm.nm[r], next_peers[r], (uint64_t)nrpr, (uint64_t)next_cols, (uint64_t)next_cols, BK, 128))) return rc2;
-    if ((rc2 = pbhost::cached_tmap_blocks(&tg2, next_full, (uint64_t)nrpr, (uint64_t)next_cols, (uint64_t)n, BK, 128))) return rc2;
+      if ((rc = pbhost::cached_tmap(&pm.nm[r], next_peers[r], (uint64_t)nrpr, (uint64_t)next_cols, (uint64_t)next_cols, BK, 128))) return rc;
+    if ((rc = pbhost::cached_tmap_blocks(&tg2, next_full, (uint64_t)nrpr, (uint64_t)next_cols, (uint64_t)n, BK, 128))) return rc;
     have_next = true;
   }
-  if (epi == 2 && n % 2 == 0) {
+  if (e.kind == 2 && n % 2 == 0) {
     // a tile needs gate rows (blocks < n/2) and the matching up rows (blocks >= n/2): fetch them pairwise, own pair first
     const int h = n / 2, g0 = rank % h;
     for (int t = 0; t < h; ++t) {
@@ -817,32 +852,25 @@ PB_EXPORT int pb_gemm_wgather(const void* A, const void* const* w_peers, int n, 
     pm.start = (g0 * rpr) / 64;  // tiles are 64 features wide
   } else {
     for (int t = 0; t < n; ++t) pm.order[t] = (rank + t) % n;
-    if (epi == 2) pm.start = 0;
+    if (e.kind == 2) pm.start = 0;
     else pm.start = b_mn_major ? (rank * rpr) / BK : (rank * rpr) / BN;
   }
   if (!own_resident) {
-    cudaError_t e = cudaMemsetAsync(flags, 0, sizeof(uint32_t) * (size_t)(n * kGatherSub), stream);
-    if (e != cudaSuccess) return (int)e;
+    cudaError_t err = cudaMemsetAsync(flags, 0, sizeof(uint32_t) * (size_t)(n * kGatherSub), stream);
+    if (err != cudaSuccess) return (int)err;
   }
-  int rc;
   for (int r = 0; r < n; ++r)
     if ((rc = pbhost::cached_tmap(&pm.m[r], w_peers[r], (uint64_t)rpr, (uint64_t)colsW, (uint64_t)colsW, BK, 128))) return rc;
   CUtensorMap tg, ta, tb;
   if ((rc = pbhost::cached_tmap_blocks(&tg, w_full, (uint64_t)rpr, (uint64_t)colsW, (uint64_t)n, BK, 128))) return rc;
-  if ((rc = pbhost::cached_tmap(&ta, A, (uint64_t)M, (uint64_t)K, (uint64_t)lda, BK, BM))) return rc;
-  if (!b_mn_major) rc = pbhost::cached_tmap(&tb, w_full, (uint64_t)rowsW, (uint64_t)colsW, (uint64_t)colsW, BK, epi == 2 ? 64 : BN);
-  else rc = pbhost::cached_tmap(&tb, w_full, (uint64_t)rowsW, (uint64_t)colsW, (uint64_t)colsW, 64, BK);
-  if (rc) return rc;
+  if ((rc = operand_tmap(&ta, A, M, K, lda, 0, BM))) return rc;
+  if ((rc = operand_tmap(&tb, w_full, N, K, colsW, b_mn_major, e.kind == 2 ? 64 : BN))) return rc;
   static int group_m = -1;
   if (group_m < 0) {
     const char* ev = getenv("PB_WG_GROUP_M");
     group_m = ev ? atoi(ev) : 0;
   }
-  GemmParams p{M, epi == 2 ? 2 * FF : N, K, ldc, 0, b_mn_major, 0, 0, 1, C, rope_cos, rope_sin, rope_S, rope_cols, rope_D, FF, group_m,
-               epi == 3 ? H : nullptr, epi == 3 ? ldh : 0, epi == 2 ? H : nullptr, epi == 2 ? ldh : 0};
-  const CUtensorMap* tg2p = have_next ? &tg2 : nullptr;
-  if (epi == 3) return launch<0, 1, 3, 3>(ta, tb, p, 0, stream, &pm, &tg, tg2p);
-  if (epi == 2) return launch<0, 0, 2, 3>(ta, tb, p, 0, stream, &pm, &tg, tg2p);
-  if (epi == 1) return launch<0, 0, 1, 3>(ta, tb, p, 0, stream, &pm, &tg, tg2p);
-  return b_mn_major ? launch<0, 1, 0, 3>(ta, tb, p, 0, stream, &pm, &tg, tg2p) : launch<0, 0, 0, 3>(ta, tb, p, 0, stream, &pm, &tg, tg2p);
+  GemmParams p = make_params(C, M, N, K, ldc, 0, b_mn_major, 0, 0, e);
+  p.group_m = group_m;
+  return dispatch(3, e.kind, p, ta, tb, stream, &pm, &tg, have_next ? &tg2 : nullptr);
 }

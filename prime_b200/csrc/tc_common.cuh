@@ -31,21 +31,6 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// Non-blocking probe (try_wait may suspend the thread for a hardware time slice; test_wait never does): use it for the
-// "is there something useful I could do meanwhile?" checks inside a polling loop.
-__device__ __forceinline__ bool mbar_test_wait(uint64_t* bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n"
-      "selp.u32 %0, 1, 0, p;\n"
-      "}\n"
-      : "=r"(ok)
-      : "r"(smem_u32(bar)), "r"(parity)
-      : "memory");
-  return ok != 0;
-}
 // Bounded wait: a protocol bug traps (kernel error) after ~4 s instead of hanging the GPU.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
@@ -74,7 +59,6 @@ struct SpinGuard {
   }
 };
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 // all state spaces: orders generic-proxy accesses (flags) against async-proxy (TMA) accesses to GLOBAL memory
 __device__ __forceinline__ void fence_proxy_async_all() { asm volatile("fence.proxy.async;" ::: "memory"); }
 
@@ -85,22 +69,11 @@ __device__ __forceinline__ void tma_load_2d(const CUtensorMap* map, uint64_t* ba
       "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
       : "memory");
 }
-__device__ __forceinline__ void tma_load_3d(const CUtensorMap* map, uint64_t* bar, void* smem, int c0, int c1, int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];" ::"r"(
-          smem_u32(smem)),
-      "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
-// pull a tile into L2 ahead of the TMA load that will consume it (no smem, no barrier)
-__device__ __forceinline__ void tma_prefetch_l2_2d(const CUtensorMap* map, int c0, int c1) {
-  asm volatile("cp.async.bulk.prefetch.tensor.2d.L2.global [%0, {%1, %2}];" ::"l"(map), "r"(c0), "r"(c1) : "memory");
-}
 __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
 }
 
-// smem → global tensor store / reduce-add (bulk async-group completion)
+// smem → global tensor store (bulk async-group completion)
 __device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, const void* smem, int c0, int c1) {
   asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(map),
                "r"(smem_u32(smem)), "r"(c0), "r"(c1)
@@ -111,11 +84,6 @@ __device__ __forceinline__ void tma_store_3d(const CUtensorMap* map, const void*
                "r"(smem_u32(smem)), "r"(c0), "r"(c1), "r"(c2)
                : "memory");
 }
-__device__ __forceinline__ void tma_reduce_add_2d(const CUtensorMap* map, const void* smem, int c0, int c1) {
-  asm volatile("cp.reduce.async.bulk.tensor.2d.global.shared::cta.add.bulk_group [%0, {%2, %3}], [%1];" ::"l"(map),
-               "r"(smem_u32(smem)), "r"(c0), "r"(c1)
-               : "memory");
-}
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void bulk_wait_read() {
@@ -123,18 +91,6 @@ __device__ __forceinline__ void bulk_wait_read() {
 }
 // full completion (the writes/reductions themselves, not just the smem reads) of every bulk group of this thread
 __device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-__device__ __forceinline__ void st_shared_v4(uint32_t saddr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
-  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(saddr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
-}
-__device__ __forceinline__ uint4 ld_shared_v4(uint32_t saddr) {
-  uint4 r;
-  asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "r"(saddr) : "memory");
-  return r;
-}
-__device__ __forceinline__ uint32_t pack_bf16x2(uint32_t lo_f32_bits, uint32_t hi_f32_bits) {
-  const __nv_bfloat162 v = __floats2bfloat162_rn(__uint_as_float(lo_f32_bits), __uint_as_float(hi_f32_bits));
-  return *reinterpret_cast<const uint32_t*>(&v);
-}
 
 // ---------------------------------------------------------------------------------------------- wgmma (sm_90a)
 // Shared-memory matrix descriptor, SWIZZLE_128B (layout type 1 in bits 62-63).

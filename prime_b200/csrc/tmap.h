@@ -1,17 +1,13 @@
 // Host-side TMA tensor-map construction (cuTensorMapEncodeTiled through the runtime's driver entry point) with a
-// process-wide cache keyed by (pointer, shape, stride, box, element size).
+// process-wide cache keyed by (pointer, shape, stride, box). Every map is bf16 with 128B-swizzled boxes; 0 = success.
 #pragma once
 #include <cuda.h>
 #include <stdint.h>
 
 namespace pbhost {
-// rows x cols matrix (cols contiguous), row stride `ld` elements, 128B-swizzled boxes of box_cols x box_rows.
-// esize: 1 = fp8 (bytes), 2 = bf16, 4 = fp32.  Returns 0 on success.
-int cached_tmap(CUtensorMap* out, const void* ptr, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_cols,
-                uint32_t box_rows, int esize = 2);
-// {64 columns, rows, cols/64 chunks} view with boxes of {64, box_rows, chunks}: one TMA instruction per multi-chunk operand tile.
-int cached_tmap3(CUtensorMap* out, const void* ptr, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows, uint32_t chunks);
-// dense [blocks][rows][cols] bf16 view, boxes {box_cols, box_rows, 1} (rows clipped per block)
+// rows x cols matrix (cols contiguous), row stride `ld` elements, boxes of box_cols x box_rows.
+int cached_tmap(CUtensorMap* out, const void* ptr, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_cols, uint32_t box_rows);
+// dense [blocks][rows][cols] view, boxes {box_cols, box_rows, 1} (rows clipped per block)
 int cached_tmap_blocks(CUtensorMap* out, const void* ptr, uint64_t rows, uint64_t cols, uint64_t blocks, uint32_t box_cols, uint32_t box_rows);
 int num_sms();
 }  // namespace pbhost

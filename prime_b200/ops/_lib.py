@@ -128,10 +128,19 @@ class OuterArgs(ctypes.Structure):
     _fields_ = [("lr", ctypes.c_float), ("momentum", ctypes.c_float), ("inv_workers", ctypes.c_float), ("nesterov", ctypes.c_int)]
 
 
-def _declare(lib: ctypes.CDLL) -> None:
+class GemmEpilogue(ctypes.Structure):
+    """Fused epilogue of ``pb_gemm_bf16`` / ``pb_gemm_wgather`` (csrc/gemm_sm90.cu). ``kind``: 0 plain, 1 RoPE, 2 SwiGLU (``aux`` = h,
+    written), 3 SwiGLU backward (``aux`` = the saved gate_up, read)."""
+
+    _fields_ = [("kind", ctypes.c_int), ("rope_cos", ctypes.c_void_p), ("rope_sin", ctypes.c_void_p), ("rope_S", ctypes.c_int),
+                ("rope_cols", ctypes.c_int), ("rope_D", ctypes.c_int), ("aux", ctypes.c_void_p), ("ld_aux", ctypes.c_int)]  # fmt: skip
+
+
+def _sigs() -> dict:
+    """Argument types of every exported ``pb_*`` launcher (all return int)."""
     vp, i32, i64, f32, u32 = ctypes.c_void_p, ctypes.c_int, ctypes.c_int64, ctypes.c_float, ctypes.c_uint32
     PP = ctypes.POINTER(PeerPtrs)
-    sigs = {
+    return {
         "pb_rmsnorm_fwd": [vp, vp, vp, vp, vp, vp, i64, i32, f32, vp],
         "pb_rmsnorm_bwd_grid": [i64],
         "pb_rmsnorm_bwd": [vp, vp, vp, vp, vp, vp, vp, vp, i32, i64, i32, vp],
@@ -139,10 +148,7 @@ def _declare(lib: ctypes.CDLL) -> None:
         "pb_swiglu_fwd": [vp, vp, i64, i32, vp],
         "pb_swiglu_bwd": [vp, vp, vp, i64, i32, vp],
         "pb_cross_entropy_loss": [vp, vp, vp, vp, vp, vp, i64, i32, i64, f32, vp],
-        "pb_gemm_bf16": [vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, i32, i32, i32, i32, vp],
-        "pb_gemm_bf16_rope": [vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, vp, vp, i32, i32, i32, vp],
-        "pb_gemm_bf16_swiglu": [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, vp],
-        "pb_gemm_bf16_swiglu_bwd": [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, vp],
+        "pb_gemm_bf16": [vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, i32, i32, i32, ctypes.POINTER(GemmEpilogue), vp],
         "pb_gemm_allgather": [vp, i32, i32, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, vp],
         "pb_gemm_reduce_scatter": [vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, i32, i32, vp],
         "pb_quantize_mxfp8": [vp, i64, vp, vp, i32, i32, i32, vp],
@@ -173,8 +179,8 @@ def _declare(lib: ctypes.CDLL) -> None:
         "pb_embedding_sort": [vp, i64, vp, vp],
         "pb_embedding_scatter": [vp, i64, vp, vp, i32, vp],
         "pb_allgather_copy": [PP, i64, vp, vp],
-        "pb_gemm_wgather": [vp, ctypes.POINTER(vp), i32, i32, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, i32, vp, vp, i32, i32, i32,
-                            i32, ctypes.POINTER(vp), vp, i32, i32, vp],
+        "pb_gemm_wgather": [vp, ctypes.POINTER(vp), i32, i32, vp, vp, vp, i32, i32, i32, i32, i32, i32, ctypes.POINTER(GemmEpilogue), i32,
+                            ctypes.POINTER(vp), vp, i32, i32, vp],
         "pb_cast_push": [vp, i64, PP, i64, vp],
         # NVLS: VMM allocations shared by fd, multicast objects, multimem kernels (csrc/multicast.cu)
         "pb_mc_supported": [i32],
@@ -192,10 +198,11 @@ def _declare(lib: ctypes.CDLL) -> None:
         "pb_mc_all_reduce": [vp, i64, i32, vp, vp, i32, i32, u32, vp, vp],
         "pb_mc_grad_reduce": [vp, i64, i64, f32, vp, vp, vp, i32, u32, i32, vp, i32, vp],
     }
-    for name, argtypes in sigs.items():
-        fn = getattr(lib, name, None)
-        if fn is None:
-            continue
+
+
+def _declare(lib: ctypes.CDLL) -> None:
+    for name, argtypes in _sigs().items():
+        fn = getattr(lib, name)  # a declared launcher the library lacks is a stale build or a stale declaration: fail here
         fn.argtypes = argtypes
         fn.restype = ctypes.c_int
 

@@ -23,10 +23,8 @@ def supported_shape(S: int, D: int, H: int, Hkv: int) -> bool:
 
 def supported(qkv: torch.Tensor, n_heads: int, n_kv_heads: int) -> bool:
     try:
-        lib = _lib.load()
+        _lib.load()
     except Exception:
-        return False
-    if getattr(lib, "pb_flash_attn_fwd", None) is None:
         return False
     D = qkv.shape[-1] // (n_heads + 2 * n_kv_heads)
     return qkv.dtype == torch.bfloat16 and qkv.is_contiguous() and supported_shape(qkv.shape[1], D, n_heads, n_kv_heads)

@@ -62,13 +62,18 @@ def gemm(
     out: torch.Tensor | None = None,
     out_dtype: torch.dtype = torch.bfloat16,
     accumulate: bool = False,
-    max_ctas: int = 0,
+    rope: tuple | None = None,
+    swiglu_h: torch.Tensor | None = None,
+    swiglu_bwd_gu: torch.Tensor | None = None,
 ) -> torch.Tensor:
     """C[M,N] (+)= A·Bᵀ on the wgmma kernel.
 
     ``a``: [M,K] (K-major) or, if ``a_mn_major``, stored [K,M].
     ``b``: [N,K] (K-major) or, if ``b_mn_major``, stored [K,N].
     Both must be 2-D bf16 with unit inner stride.
+    Fused epilogues (:func:`_epilogue`; K-major ``a``, bf16 output): ``rope`` rotates the Q/K head columns, ``swiglu_h`` receives
+    silu(gate)·up of C = gate_up [M, 2·FF], ``swiglu_bwd_gu`` (MN-major ``b``, M > 128) turns the product dh [M, FF] into
+    C = d_gate_up [M, 2·FF] from the saved gate_up.
     """
     assert a.dtype == torch.bfloat16 and b.dtype == torch.bfloat16
     assert a.dim() == 2 and b.dim() == 2 and a.stride(1) == 1 and b.stride(1) == 1
@@ -81,16 +86,33 @@ def gemm(
     else:
         N, Kb = b.shape
     assert K == Kb, f"contraction mismatch {K} vs {Kb}"
+    out_n = 2 * N if swiglu_bwd_gu is not None else N
     if out is None:
         assert not accumulate
-        out = torch.empty((M, N), dtype=out_dtype, device=a.device)
+        out = torch.empty((M, out_n), dtype=out_dtype, device=a.device)
     else:
-        assert out.shape == (M, N) and out.stride(1) == 1 and out.dtype in (torch.bfloat16, torch.float32)
+        assert out.shape == (M, out_n) and out.stride(1) == 1 and out.dtype in (torch.bfloat16, torch.float32)
     _launch(
         "pb_gemm_bf16", a.data_ptr(), b.data_ptr(), out.data_ptr(), M, N, K, a.stride(0), b.stride(0), out.stride(0),
-        int(a_mn_major), int(b_mn_major), int(out.dtype == torch.float32), int(accumulate), max_ctas, _stream(),
+        int(a_mn_major), int(b_mn_major), int(out.dtype == torch.float32), int(accumulate),
+        _epilogue(rope, swiglu_h, swiglu_bwd_gu), _stream(),
     )  # fmt: skip
     return out
+
+
+def _epilogue(rope: tuple | None, swiglu_h: torch.Tensor | None, swiglu_bwd_gu: torch.Tensor | None) -> _lib.GemmEpilogue | None:
+    """The native epilogue descriptor of a GEMM launch, None for a plain GEMM. ``rope`` = (cos, sin, seq_len, rotated columns,
+    head_dim) with fp32 [>= seq_len, head_dim/2] tables; ``swiglu_h`` = h [M, FF]; ``swiglu_bwd_gu`` = the saved gate_up [M, 2·FF]."""
+    if swiglu_bwd_gu is not None:
+        return _lib.GemmEpilogue(kind=3, aux=swiglu_bwd_gu.data_ptr(), ld_aux=swiglu_bwd_gu.stride(0))
+    if swiglu_h is not None:
+        return _lib.GemmEpilogue(kind=2, aux=swiglu_h.data_ptr(), ld_aux=swiglu_h.stride(0))
+    if rope is not None:
+        cos, sin, seq_len, rot_cols, head_dim = rope
+        assert cos.dtype == torch.float32 and cos.is_contiguous() and sin.is_contiguous() and cos.shape[0] >= seq_len
+        return _lib.GemmEpilogue(kind=1, rope_cos=cos.data_ptr(), rope_sin=sin.data_ptr(), rope_S=seq_len, rope_cols=rot_cols,
+                                 rope_D=head_dim)  # fmt: skip
+    return None
 
 
 def set_gemm_split_k(mode: int) -> int:
@@ -147,28 +169,14 @@ def _gemm_epi(a: torch.Tensor, w: torch.Tensor, out: torch.Tensor, *, b_mn_major
     with ``b_mn_major``, C = a·w (``swiglu_bwd_gu``). SwiGLU runs as a stand-alone kernel after a plain GEMM where its fused
     epilogue does not apply (M <= 128, and for the forward hidden % 64 != 0)."""
     M = a.shape[0]
-    if swiglu_bwd_gu is not None:
-        if M > 128:
-            _launch("pb_gemm_bf16_swiglu_bwd", a.data_ptr(), w.data_ptr(), swiglu_bwd_gu.data_ptr(), out.data_ptr(), M, w.shape[1], w.shape[0],
-                    a.stride(0), w.stride(0), swiglu_bwd_gu.stride(0), out.stride(0), _stream())  # fmt: skip
-        else:
-            dh = gemm(a, w, b_mn_major=True)
-            _launch("pb_swiglu_bwd", swiglu_bwd_gu.data_ptr(), dh.data_ptr(), out.data_ptr(), M, w.shape[1], _stream())
-    elif swiglu_h is not None:
-        FF = w.shape[0] // 2
-        if M > 128 and FF % 64 == 0:
-            _launch("pb_gemm_bf16_swiglu", a.data_ptr(), w.data_ptr(), out.data_ptr(), swiglu_h.data_ptr(), M, FF, w.shape[1], a.stride(0),
-                    w.stride(0), out.stride(0), swiglu_h.stride(0), _stream())  # fmt: skip
-        else:
-            gemm(a, w, out=out)
-            _launch("pb_swiglu_fwd", out.data_ptr(), swiglu_h.data_ptr(), M, FF, _stream())
-    elif rope is not None:
-        cos, sin, seq_len, rot_cols, head_dim = rope
-        assert cos.dtype == torch.float32 and cos.is_contiguous() and sin.is_contiguous() and cos.shape[0] >= seq_len
-        _launch("pb_gemm_bf16_rope", a.data_ptr(), w.data_ptr(), out.data_ptr(), M, w.shape[0], a.shape[1], a.stride(0), w.stride(0),
-                out.stride(0), 0, cos.data_ptr(), sin.data_ptr(), seq_len, rot_cols, head_dim, _stream())  # fmt: skip
+    if swiglu_bwd_gu is not None and M <= 128:
+        dh = gemm(a, w, b_mn_major=True)
+        _launch("pb_swiglu_bwd", swiglu_bwd_gu.data_ptr(), dh.data_ptr(), out.data_ptr(), M, w.shape[1], _stream())
+    elif swiglu_h is not None and (M <= 128 or (w.shape[0] // 2) % 64 != 0):
+        gemm(a, w, out=out)
+        _launch("pb_swiglu_fwd", out.data_ptr(), swiglu_h.data_ptr(), M, w.shape[0] // 2, _stream())
     else:
-        gemm(a, w, b_mn_major=b_mn_major, out=out)
+        gemm(a, w, b_mn_major=b_mn_major, out=out, rope=rope, swiglu_h=swiglu_h, swiglu_bwd_gu=swiglu_bwd_gu)
     return out
 
 
@@ -211,17 +219,9 @@ def gemm_wgather(a: torch.Tensor, z, *, b_mn_major: bool = False, out: torch.Ten
             _launch("pb_allgather_copy", ctypes.byref(pp), z.rpr * z.cols * 2, z.full_ptr, _stream())
             _mark_resident(z)
         return _gemm_epi(a, _full_weight(z, a.device), out, b_mn_major=b_mn_major, rope=rope, swiglu_h=swiglu_h, swiglu_bwd_gu=swiglu_bwd_gu)
-    epi = 3 if swiglu_bwd_gu is not None else (2 if swiglu_h is not None else (1 if rope is not None else 0))
-    cos = sin = None
-    seq_len, rot_cols, head_dim = 1, 0, 64
-    if rope is not None:
-        cos, sin, seq_len, rot_cols, head_dim = rope
-        assert cos.dtype == torch.float32 and cos.is_contiguous() and sin.is_contiguous() and cos.shape[0] >= seq_len
-    aux = swiglu_h if swiglu_h is not None else swiglu_bwd_gu
     _launch(
-        "pb_gemm_wgather", a.data_ptr(), z.peer_ptrs, z.n, z.rank, z.full_ptr, z.flags.data_ptr(), out.data_ptr(), _ptr(aux), M, z.rows,
-        z.cols, a.stride(0), out.stride(0), aux.stride(0) if aux is not None else 0, int(b_mn_major), epi,
-        _ptr(cos), _ptr(sin), seq_len, rot_cols, head_dim,
+        "pb_gemm_wgather", a.data_ptr(), z.peer_ptrs, z.n, z.rank, z.full_ptr, z.flags.data_ptr(), out.data_ptr(), M, z.rows, z.cols,
+        a.stride(0), out.stride(0), int(b_mn_major), _epilogue(rope, swiglu_h, swiglu_bwd_gu),
         int(own_resident), nz.peer_ptrs if nz is not None else None, nz.full_ptr if nz is not None else None,
         nz.rows if nz is not None else 0, nz.cols if nz is not None else 0, _stream(), n=1 if own_resident else 2,
     )  # fmt: skip
@@ -631,7 +631,8 @@ class _LinearSwiGLUFn(torch.autograd.Function):
 class _MLPSwiGLUFn(torch.autograd.Function):
     """y = (silu(x W1ᵀ)·(x W3ᵀ)) W2ᵀ as ONE autograd node so that the backward can fuse across the two projections:
     the down-projection's input-gradient GEMM (dh = dy·W2) applies the SwiGLU derivative in its epilogue and writes d_gate_up
-    directly (``pb_gemm_bf16_swiglu_bwd``) — dh is never stored or re-read and the stand-alone swiglu_bwd pass is gone.
+    directly (the SwiGLU-backward epilogue of ``pb_gemm_bf16``) — dh is never stored or re-read and the stand-alone swiglu_bwd
+    pass is gone.
     Forward: gate/up GEMM with the SwiGLU epilogue, then the down projection. Saves exactly what the two separate nodes saved."""
 
     @staticmethod

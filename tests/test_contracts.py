@@ -2,9 +2,13 @@
 metrics helpers."""
 
 import json
+import re
+import shutil
 import subprocess
 import sys
 from pathlib import Path
+
+import pytest
 
 ROOT = Path(__file__).resolve().parents[1]
 
@@ -94,7 +98,7 @@ def test_nvlink_counters_decode_and_delta():
     assert NvlinkCounters(0, nvml=Broken()).read() is None
 
 
-def test_native_launchers_validate_their_arguments_before_touching_the_device():
+def test_native_launchers_reject_impossible_arguments_before_touching_the_device():
     """The C-ABI launchers are called with shapes that come from user configs: impossible ones must come back as error codes, on any
     machine — the checks run before the first CUDA call, so this needs no GPU (the library itself loads wherever libcudart is)."""
     import ctypes
@@ -110,7 +114,8 @@ def test_native_launchers_validate_their_arguments_before_touching_the_device():
     oa = _lib.OuterArgs(0.7, 0.9, 1.0, 1)
 
     def wgather(n=2, rank=0, M=1024, rows=1024, cols=1024, lda=1024, ldc=1024, ldh=0, b_mn=0, epi=0, H=None):
-        return lib.pb_gemm_wgather(None, peers, n, rank, None, None, None, H, M, rows, cols, lda, ldc, ldh, b_mn, epi, None, None, 1, 0, 64, 0, None, None, 0, 0, None)
+        e = _lib.GemmEpilogue(kind=epi, aux=H, ld_aux=ldh)
+        return lib.pb_gemm_wgather(None, peers, n, rank, None, None, None, M, rows, cols, lda, ldc, b_mn, e, 0, None, None, 0, 0, None)
 
     assert wgather(n=0) == -6 and wgather(n=9) == -6 and wgather(rank=2) == -6  # group size / rank out of range
     assert wgather(rows=1023) == -6 and wgather(cols=1000) == -6  # rows must divide over the ranks, columns come in 64-wide TMA boxes
@@ -119,6 +124,22 @@ def test_native_launchers_validate_their_arguments_before_touching_the_device():
     assert wgather(epi=2, ldh=1024) == -5  # SwiGLU epilogue without an output for h
     assert wgather(epi=1) == -3  # RoPE without tables
     assert wgather(M=128) == -8  # below one CTA-pair tile: the host gathers explicitly instead
+
+    aux = 1 << 20  # a 16-byte aligned address that is never dereferenced: every call below is rejected first
+
+    def gemm(M=1024, N=1024, lda=1024, a_mn=0, b_mn=0, c_fp32=0, acc=0, epi=None):
+        return lib.pb_gemm_bf16(None, None, None, M, N, 1024, lda, 1024, 1024, a_mn, b_mn, c_fp32, acc, epi, None)
+
+    rope = _lib.GemmEpilogue(kind=1, rope_cos=aux, rope_sin=aux, rope_S=256, rope_cols=512, rope_D=128)
+    swiglu = _lib.GemmEpilogue(kind=2, aux=aux, ld_aux=512)
+    swiglu_bwd = _lib.GemmEpilogue(kind=3, aux=aux, ld_aux=2048)
+    assert gemm(lda=1001) == -1  # 16-byte row pitch
+    assert gemm(epi=_lib.GemmEpilogue(kind=1)) == -3  # RoPE without tables
+    assert gemm(N=1088, epi=swiglu) == -5 and gemm(epi=_lib.GemmEpilogue(kind=2)) == -5  # SwiGLU: 64-feature tiles, an output for h
+    assert gemm(M=128, b_mn=1, epi=swiglu_bwd) == -5  # the SwiGLU backward runs on training shapes only
+    assert gemm(a_mn=1, epi=rope) == -7 and gemm(c_fp32=1, epi=rope) == -7  # RoPE / SwiGLU: K-major operands, bf16 output
+    assert gemm(epi=swiglu_bwd) == -7  # SwiGLU backward: MN-major B (the input-gradient GEMM)
+    assert gemm(epi=_lib.GemmEpilogue(kind=4)) == -7  # no such epilogue
     assert lib.pb_pseudograd_quant(None, None, None, None, 1000, None) == -1  # int8 blocks are 1024 elements
     assert lib.pb_outer_nesterov(ctypes.byref(pp), ctypes.byref(pp), None, None, None, 1000, ctypes.byref(oa), ctypes.byref(pp), None, None, 1, None, None) == -1
     assert lib.pb_outer_nesterov(ctypes.byref(pp), ctypes.byref(pp), None, None, None, 1024, ctypes.byref(oa), ctypes.byref(pp), None, None, 0, None, None) == -1  # no bucket table
@@ -137,3 +158,27 @@ def test_native_launchers_validate_their_arguments_before_touching_the_device():
     assert attn_fwd(doc_start=d, causal=0) == -1 and attn_bwd(doc_start=d, doc_end=d, causal=0) == -1  # document masking is causal
     assert attn_bwd(doc_start=d) == -1 and attn_bwd(doc_end=d) == -1  # the backward needs both bounds or neither
     assert attn_fwd(S=200) == -1 and attn_bwd(S=200) == -1  # 128-row query / key blocks
+
+
+def test_ctypes_declarations_match_the_exported_prototypes():
+    """Every exported ``pb_*`` launcher is declared in ``_lib`` and nothing else is, with as many ctypes argument types as its
+    ``PB_EXPORT`` prototype has parameters: a declaration that drifts by one passes garbage into a kernel."""
+    from prime_b200.ops import _lib
+
+    if shutil.which("nm") is None:
+        pytest.skip("nm not installed")
+    try:
+        _lib.load()
+    except Exception as e:  # noqa: BLE001
+        pytest.skip(f"native library not loadable here: {e}")
+    nm = subprocess.run(["nm", "-D", "--defined-only", str(_lib.LIB_PATH)], capture_output=True, text=True, check=True).stdout
+    exported = {line.split()[-1] for line in nm.splitlines() if line.split() and line.split()[-1].startswith("pb_")}
+    sigs = _lib._sigs()
+    assert exported == set(sigs), (sorted(exported - set(sigs)), sorted(set(sigs) - exported))
+    protos = {}
+    for src in sorted(_lib.CSRC.glob("*.cu")):
+        for name, params in re.findall(r"PB_EXPORT\s+int\s+(pb_\w+)\s*\(([^)]*)\)", src.read_text()):
+            params = params.strip()
+            protos[name] = 0 if params in ("", "void") else params.count(",") + 1
+    assert set(protos) == exported
+    assert {n: len(a) for n, a in sigs.items()} == protos

@@ -94,12 +94,7 @@ def main():
             out = torch.empty(T, rowsW, dtype=torch.bfloat16, device=dev)
             h = torch.empty(T, rowsW // 2, dtype=torch.bfloat16, device=dev)
             kw = {"swiglu_h": h}
-            lib = ops.functional._lib.load()
-
-            def local():
-                rc = lib.pb_gemm_bf16_swiglu(x.data_ptr(), full.data_ptr(), out.data_ptr(), h.data_ptr(), T, rowsW // 2, colsW, x.stride(0), colsW,
-                                             rowsW, rowsW // 2, torch.cuda.current_stream().cuda_stream)  # fmt: skip
-                assert rc == 0
+            local = lambda: ops.functional._gemm_epi(x, full, out, swiglu_h=h)  # noqa: E731
         else:  # dgrad: dx = dy · W
             x = (torch.randn(T, rowsW, device=dev) * 0.5).to(torch.bfloat16)
             out = torch.empty(T, colsW, dtype=torch.bfloat16, device=dev)
