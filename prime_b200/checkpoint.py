@@ -423,11 +423,13 @@ def assemble_full_model(path: str | Path, name_model: str, type_model: str = "ll
     1/F slice of the fp32 master weights, cut either as contiguous bucket slices (replicated-parameter mode) or as one row block
     per weight (ZeRO-3). The layout is recomputed with the engine's own planner, so there is one source of truth.
     Used by ``python -m prime_b200.models.hf export`` and ``examples/inspect_checkpoint.py``; DiLoCo workers are identical after
-    an outer step, the first worker's shards are taken."""
+    an outer step, the first worker's shards are taken. The sliding window is taken from the run's recorded config (the bucket
+    layout does not depend on it), so a windowed model is never rebuilt with full attention."""
     from .models.llama import build_model
 
     d = Path(path)
     meta = json.loads((d / "meta.json").read_text())
+    overrides.setdefault("sliding_window", (meta.get("config") or {}).get("sliding_window"))
     shards: dict[int, torch.Tensor] = {}
     extra0: dict[str, Any] | None = None
     for r in range(int(meta["world_size"])):

@@ -129,6 +129,9 @@ ModelName = Literal["debugmodel", "10M", "150M", "271M", "1B", "7B", "10B", "13B
 class Config(_Section):
     name_model: ModelName = "150M"
     type_model: Literal["llama2", "llama3"] = "llama2"
+    # sliding-window attention in every layer (as in Mistral): a query attends only its W most recent keys, itself included; it
+    # composes with data.document_mask. Part of the model's definition, so checkpoints record it. None = full causal attention
+    sliding_window: int | None = Field(default=None, ge=1)
     project: str = "prime_b200"
     run_id: str | None = None
     seed: int = 42

@@ -14,8 +14,11 @@
 // With dS = P ∘ (dP·scale − delta·scale) the results need no further scaling; P is recomputed from lse2.
 // Optional RoPE backward (non-null rope_cos / rope_sin of pb_flash_attn_bwd): the inverse rotation is applied to dQ / dK in registers
 // before the store.
-// Optional document masking of packed rows (kDoc, selected by a non-null doc_start with the bounds of pb_doc_bounds): key tiles that
-// lie before a query block's first document are skipped, not masked.
+// Optional lower-bounded causal masking (kDoc, selected by a non-null doc_start): query q of row b sees key k iff
+// lo[q] <= k <= q, where lo = doc_start is any int32 [B, S] array that never decreases along a row and has lo[q] <= q, and
+// end = doc_end is its matching upper bound (end[k] = one past the last query that sees key k). pb_doc_bounds builds them for
+// documents of packed rows, a sliding window of W keys (lo[q] = q - W + 1), or both. Key tiles below a query block's first
+// visible key are skipped, not masked.
 #include "common.cuh"
 
 namespace {
@@ -109,14 +112,14 @@ struct AttnParams {
   int causal;
   const float* rope_cos;  // backward only: fp32 [S, D/2] tables of the forward rotation, nullptr = no RoPE
   const float* rope_sin;
-  const int* doc_start;  // kDoc kernels only: int32 [B, S] first position of the document holding s (pb_doc_bounds)
-  const int* doc_end;    //                     int32 [B, S] one past its last position
+  const int* doc_start;  // kDoc kernels only: int32 [B, S] lo[s], the first key query s sees (non-decreasing, <= s)
+  const int* doc_end;    //                     int32 [B, S] end[s], one past the last query that sees key s
 };
 
 // ------------------------------------------------------------------------------------------------------------------ forward
-// kDoc: document masking (always causal). Query q sees key k iff doc_start[b, q] <= k <= q. doc_start never decreases along a
-// row, so the key loop starts at the tile of doc_start[b, q0]; only tiles below doc_start[b, q0 + BQ - 1] and the diagonal tile
-// need a mask, the others take the plain path.
+// kDoc: lower-bounded causal masking. Query q sees key k iff lo[q] <= k <= q (lo = doc_start). lo never decreases along a row,
+// so the key loop starts at the tile of lo[q0]; only tiles below lo[q0 + BQ - 1] and the diagonal tile need a mask, the others
+// take the plain path.
 template <int D, bool kDoc>
 __global__ void __launch_bounds__(kThreads) flash_fwd_kernel(const AttnParams p) {
   extern __shared__ __align__(128) uint8_t smem[];
@@ -206,7 +209,7 @@ __global__ void __launch_bounds__(kThreads) flash_fwd_kernel(const AttnParams p)
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
       if constexpr (kDoc) {
-        // a row whose document starts later in the block can meet tiles in which every key is masked; while its maximum is
+        // a row whose lower bound lies later in the block can meet tiles in which every key is masked; while its maximum is
         // still -inf, subtract 0 so that exp2 gives 0 instead of exp2(-inf - -inf) = NaN (m is reset to -inf below)
         const float mref = mx[r] == -INFINITY ? 0.f : mx[r];
         corr[r] = fast_exp2(m[r] - mref);
@@ -324,8 +327,8 @@ __device__ __forceinline__ void store_rows(__nv_bfloat16* dst, int64_t ld, int r
   }
 }
 
-// kDoc: the query-tile loop stops at the tile holding doc_end[b, k0 + BKV - 1] (no later query sees a key of this block) and
-// Pᵀ is zero unless doc_start[q] <= key <= q; the tile's doc_start values are staged in shared memory after lse2 and delta.
+// kDoc: the query-tile loop stops at the tile holding end[b, k0 + BKV - 1] (end never decreases, so no later query sees a key of
+// this block) and Pᵀ is zero unless lo[q] <= key <= q; the tile's lo values are staged in shared memory after lse2 and delta.
 template <int D, bool kDoc>
 __global__ void __launch_bounds__(kThreads) bwd_dkdv_kernel(const AttnParams p) {
   extern __shared__ __align__(128) uint8_t smem[];
@@ -432,7 +435,7 @@ __global__ void __launch_bounds__(kThreads) bwd_dkdv_kernel(const AttnParams p) 
   store_rows<D>(dst + (p.H + p.Hkv + hk) * D, W, k0 + warp * 16, k0 + warp * 16, dv, p, false);
 }
 
-// kDoc: key tiles from doc_start[b, q0] / BKV to the diagonal, masks as in the forward
+// kDoc: key tiles from lo[b, q0] / BKV to the diagonal, masks as in the forward
 template <int D, bool kDoc>
 __global__ void __launch_bounds__(kThreads) bwd_dq_kernel(const AttnParams p) {
   extern __shared__ __align__(128) uint8_t smem[];
@@ -560,8 +563,9 @@ int launch_bwd(const AttnParams& p, cudaStream_t stream) {
 
 // Document bounds of packed rows: one CTA per row. Every thread owns a contiguous run of positions; a block-wide exclusive
 // max-scan of the last document start per run (and min-scan, from the right, of the first EOS end) gives each run its carry-in.
+// The window (1 <= window <= S; S = none) clamps both bounds as they are written.
 constexpr int kBoundsThreads = 256;
-__global__ void __launch_bounds__(kBoundsThreads) doc_bounds_kernel(const int64_t* __restrict__ tokens, int S, int64_t eos,
+__global__ void __launch_bounds__(kBoundsThreads) doc_bounds_kernel(const int64_t* __restrict__ tokens, int S, int64_t eos, int window,
                                                                     int* __restrict__ doc_start, int* __restrict__ doc_end) {
   constexpr int kWarps = kBoundsThreads / 32;
   __shared__ int s_lo[kWarps], s_hi[kWarps];
@@ -591,19 +595,19 @@ __global__ void __launch_bounds__(kBoundsThreads) doc_bounds_kernel(const int64_
   for (int w = warp + 1; w < kWarps; ++w) cur_hi = min(cur_hi, s_hi[w]);
   for (int s = s0; s < s1; ++s) {
     if (s > 0 && tokens[row + s - 1] == eos) cur_lo = s;
-    doc_start[row + s] = cur_lo;
+    doc_start[row + s] = max(cur_lo, s - window + 1);
   }
   for (int s = s1 - 1; s >= s0; --s) {
     if (tokens[row + s] == eos) cur_hi = s + 1;
-    doc_end[row + s] = cur_hi;
+    doc_end[row + s] = min(cur_hi, s + window);
   }
 }
 
 }  // namespace
 
 // qkv [B, S, (H+2Hkv)·D] → out [B, S, H·D], lse2 [B, H, S].  S % 128 == 0, D ∈ {64, 128}.
-// doc_start: null, or the int32 [B, S] document starts of pb_doc_bounds for document-masked causal attention (causal != 0): query q
-// attends key k iff doc_start[b, q] <= k <= q.
+// doc_start: null, or an int32 [B, S] lower bound lo (non-decreasing along a row, lo[q] <= q; pb_doc_bounds builds it for documents
+// and / or a sliding window) for masked causal attention (causal != 0): query q attends key k iff doc_start[b, q] <= k <= q.
 PB_EXPORT int pb_flash_attn_fwd(const void* qkv, void* out, float* lse2, const int* doc_start, int B, int S, int H, int Hkv, int D,
                                 float scale, int causal, cudaStream_t stream) {
   if (S % 128 != 0 || H % Hkv != 0 || (doc_start != nullptr && !causal)) return -1;
@@ -620,7 +624,7 @@ PB_EXPORT int pb_flash_attn_fwd(const void* qkv, void* out, float* lse2, const i
 }
 
 // delta: [B, H, S] fp32 scratch.  dqkv: [B, S, (H+2Hkv)·D] bf16, fully overwritten.
-// doc_start / doc_end: both null, or both the forward's document bounds (causal != 0).
+// doc_start / doc_end: both null, or both the forward's lower bound and its matching upper bound (causal != 0).
 // rope_cos / rope_sin: null, or the fp32 [S, D/2] tables of a forward rotation, whose inverse is fused into the dQ / dK stores.
 PB_EXPORT int pb_flash_attn_bwd(const void* qkv, const void* out, const void* dout, const float* lse2, float* delta, void* dqkv,
                                 const int* doc_start, const int* doc_end, int B, int S, int H, int Hkv, int D, float scale, int causal,
@@ -638,11 +642,15 @@ PB_EXPORT int pb_flash_attn_bwd(const void* qkv, const void* out, const void* do
   return -2;
 }
 
-// tokens int64 [B, S] → doc_start, doc_end int32 [B, S]: position s starts a document when s == 0 or tokens[b, s-1] == eos;
-// doc_start = first position of the document holding s, doc_end = one past its last position (after its EOS, or S).
-PB_EXPORT int pb_doc_bounds(const int64_t* tokens, int B, int S, int64_t eos, int* doc_start, int* doc_end, cudaStream_t stream) {
-  if (B <= 0 || S <= 0) return -1;
-  doc_bounds_kernel<<<B, kBoundsThreads, 0, stream>>>(tokens, S, eos, doc_start, doc_end);
+// tokens int64 [B, S] → doc_start, doc_end int32 [B, S], the lo / end bounds of pb_flash_attn_fwd / _bwd. Position s starts a
+// document when s == 0 or tokens[b, s-1] == eos; eos < 0 means no documents (token ids are never negative). window: 0 = none,
+// else query s sees only the `window` most recent keys, itself included. Query s attends key k iff lo[s] <= k <= s with
+// lo[s] = max(first position of the document holding s, s - window + 1), and end[s] = min(one past the document's last position
+// (after its EOS, or S), s + window) is one past the last query that sees key s.
+PB_EXPORT int pb_doc_bounds(const int64_t* tokens, int B, int S, int64_t eos, int window, int* doc_start, int* doc_end,
+                            cudaStream_t stream) {
+  if (B <= 0 || S <= 0 || window < 0) return -1;
+  doc_bounds_kernel<<<B, kBoundsThreads, 0, stream>>>(tokens, S, eos, window == 0 || window > S ? S : window, doc_start, doc_end);
   PB_CHECK_LAUNCH();
   return 0;
 }

@@ -12,6 +12,8 @@ Layout differences handled here (checked against ``transformers`` on CPU in ``te
 * **Fused projections.** ``wqkv`` = [q; k; v] rows, ``w13`` = [gate; up] rows.
 * **Untied head only.** ``tie_word_embeddings`` checkpoints are imported by copying the embedding into the head; exporting always
   writes an untied head. RoPE scaling variants (``rope_scaling`` ≠ null) are refused rather than silently ignored.
+* **Sliding window.** A model with ``ModelArgs.sliding_window`` is exported as a ``MistralForCausalLM`` (same tensors and names,
+  ``sliding_window`` in the config). Import stays Llama-only.
 """
 
 from __future__ import annotations
@@ -70,7 +72,9 @@ def args_from_hf_config(cfg: dict) -> ModelArgs:
 
 
 def hf_config_from_args(a: ModelArgs, dtype: torch.dtype = torch.bfloat16) -> dict:
-    return {
+    """``config.json`` of :func:`save_hf_dir`. A model with a sliding window is a ``MistralForCausalLM``: the same tensors, names and
+    RoPE layout as Llama, with the window in every layer."""
+    cfg = {
         "architectures": ["LlamaForCausalLM"],
         "model_type": "llama",
         "hidden_size": a.dim,
@@ -90,6 +94,9 @@ def hf_config_from_args(a: ModelArgs, dtype: torch.dtype = torch.bfloat16) -> di
         "tie_word_embeddings": False,
         "torch_dtype": str(dtype).replace("torch.", ""),
     }
+    if a.sliding_window is not None:
+        cfg.update(architectures=["MistralForCausalLM"], model_type="mistral", sliding_window=a.sliding_window)
+    return cfg
 
 
 @torch.no_grad()

@@ -37,6 +37,8 @@ class ModelArgs:
     max_seq_len: int = 2048
     depth_init: bool = True
     intermediate_size: int | None = None  # explicit FFN width (imported checkpoints); None = derived from dim / multiple_of
+    # sliding-window attention in every layer (Mistral): query q attends only keys q - W + 1 .. q. None = full causal attention
+    sliding_window: int | None = None
 
     @property
     def head_dim(self) -> int:
@@ -106,7 +108,8 @@ class Attention(nn.Module):
         self.fp8 = False  # train.fp8: MXFP8 forward / input-gradient GEMMs (Transformer.set_fp8)
 
     def forward(self, x: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor, attn_impl: str = "auto", doc: tuple | None = None) -> torch.Tensor:
-        """``doc``: (doc_start, doc_end) of ``ops.document_bounds`` for document-masked attention, None = plain causal."""
+        """``doc``: (doc_start, doc_end) of ``ops.document_bounds`` for document-masked and / or sliding-window attention, None =
+        plain causal."""
         B, S, _ = x.shape
         H, Hkv, D = self.n_heads, self.n_kv_heads, self.head_dim
         if self.fp8:
@@ -214,8 +217,9 @@ class Transformer(nn.Module):
         B, S = tokens.shape
         cos, sin = self.rope_tables(S, tokens.device)
         h = ops.embedding(tokens, self.tok_embeddings.weight)
-        # computed once per micro-batch, read by every layer
-        doc = ops.document_bounds(tokens, self.doc_eos_id) if self.doc_eos_id is not None else None
+        # computed once per micro-batch, read by every layer: documents and / or the sliding window bound the keys a query sees
+        win = self.args.sliding_window
+        doc = ops.document_bounds(tokens, self.doc_eos_id, win) if self.doc_eos_id is not None or win is not None else None
         delta = None
         ac = self.ac_ckpt if torch.is_grad_enabled() else False
         for i, layer in enumerate(self.layers):
@@ -247,10 +251,12 @@ class Transformer(nn.Module):
         return n
 
     def flops_per_token(self, seq_len: int) -> float:
-        """Training FLOPs/token (fwd+bwd): 6·N (matmul params) + causal attention 6·L·S·dim."""
+        """Training FLOPs/token (fwd+bwd): 6·N (matmul params) + causal attention 6·L·S·dim, times the share of the causal
+        (query, key) pairs a sliding window W keeps: (W·S - W²/2) / (S²/2) = 1 - (1 - W/S)²."""
         a = self.args
         n_mm = self.num_params(exclude_embedding=True)
-        return 6.0 * n_mm + 6.0 * a.n_layers * seq_len * a.dim
+        kept = 1.0 if a.sliding_window is None else 1.0 - (1.0 - min(a.sliding_window, seq_len) / seq_len) ** 2
+        return 6.0 * n_mm + 6.0 * a.n_layers * seq_len * a.dim * kept
 
 
 # ---------------------------------------------------------------------- checkpoint naming interchange

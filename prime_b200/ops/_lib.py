@@ -156,7 +156,7 @@ def _sigs() -> dict:
         "pb_gemm_set_split_k": [i32],
         "pb_flash_attn_fwd": [vp, vp, vp, vp, i32, i32, i32, i32, i32, f32, i32, vp],
         "pb_flash_attn_bwd": [vp, vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, f32, i32, vp, vp, vp],
-        "pb_doc_bounds": [vp, i32, i32, i64, vp, vp, vp],
+        "pb_doc_bounds": [vp, i32, i32, i64, i32, vp, vp, vp],
         "pb_ipc_alloc": [ctypes.POINTER(vp), ctypes.c_size_t],
         "pb_ipc_free": [vp],
         "pb_ipc_handle_size": [],

@@ -92,12 +92,14 @@ def rope_flash_attention_qkv(qkv: torch.Tensor, cos: torch.Tensor | None, sin: t
     return _FlashAttnFn.apply(qkv, n_heads, n_kv_heads, causal, cos, sin, pre_rotated, *(doc or (None, None)))
 
 
-def document_bounds(tokens: torch.Tensor, eos_id: int) -> tuple[torch.Tensor, torch.Tensor]:
-    """Native ``pb_doc_bounds``: int64 [B, S] CUDA tokens → (doc_start, doc_end) int32 [B, S]."""
+def document_bounds(tokens: torch.Tensor, eos_id: int | None, window: int | None = None) -> tuple[torch.Tensor, torch.Tensor]:
+    """Native ``pb_doc_bounds``: int64 [B, S] CUDA tokens → (doc_start, doc_end) int32 [B, S]. ``eos_id`` None = no documents
+    (passed as -1, which no token id equals), ``window`` None = no window (passed as 0)."""
     B, S = tokens.shape
     t = tokens if tokens.is_contiguous() else tokens.contiguous()
     assert t.dtype == torch.int64
     doc_start = torch.empty((B, S), dtype=torch.int32, device=t.device)
     doc_end = torch.empty((B, S), dtype=torch.int32, device=t.device)
-    _launch("pb_doc_bounds", _ptr(t), B, S, int(eos_id), _ptr(doc_start), _ptr(doc_end), _stream())
+    eos = -1 if eos_id is None else int(eos_id)
+    _launch("pb_doc_bounds", _ptr(t), B, S, eos, int(window or 0), _ptr(doc_start), _ptr(doc_end), _stream())
     return doc_start, doc_end

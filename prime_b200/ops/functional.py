@@ -743,15 +743,19 @@ def cross_entropy(
 # --------------------------------------------------------------------------- attention
 
 
-def document_bounds(tokens: torch.Tensor, eos_id: int) -> tuple[torch.Tensor, torch.Tensor]:
+def document_bounds(tokens: torch.Tensor, eos_id: int | None, window: int | None = None) -> tuple[torch.Tensor, torch.Tensor]:
     """Documents of packed token rows [B, S] → (doc_start, doc_end), int32 [B, S] each: the ``doc`` argument of the attention ops.
-    Position s starts a document when s == 0 or tokens[b, s-1] == eos_id. One native kernel on CUDA; it reads only ``tokens``, so
-    it can be captured in a CUDA graph over a static token buffer."""
+    Position s starts a document when s == 0 or tokens[b, s-1] == eos_id (None = no documents). ``window`` W (None = none): query q
+    also sees only the W most recent keys, itself included, so q attends k iff max(doc_start, q - W + 1) <= k <= q (see
+    :func:`reference.document_bounds`). One native kernel on CUDA; it reads only ``tokens``, so it can be captured in a CUDA graph
+    over a static token buffer."""
+    if window is not None and window < 1:
+        raise ValueError(f"window must be >= 1 (or None for no window), got {window}")
     if tokens.is_cuda:
         from . import attention_native as native
 
-        return native.document_bounds(tokens, eos_id)
-    return reference.document_bounds(tokens, eos_id)
+        return native.document_bounds(tokens, eos_id, window)
+    return reference.document_bounds(tokens, eos_id, window)
 
 
 def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, causal: bool = True, doc: tuple | None = None) -> torch.Tensor:

@@ -56,19 +56,24 @@ def swiglu(gate_up: torch.Tensor) -> torch.Tensor:
     return (F.silu(g) * u).to(gate_up.dtype)
 
 
-def document_bounds(tokens: torch.Tensor, eos_id: int) -> tuple[torch.Tensor, torch.Tensor]:
+def document_bounds(tokens: torch.Tensor, eos_id: int | None, window: int | None = None) -> tuple[torch.Tensor, torch.Tensor]:
     """Documents of packed rows, tokens [B, S] → (doc_start, doc_end) int32 [B, S].
 
-    Position s starts a document when s == 0 or tokens[b, s-1] == eos_id (the EOS belongs to the document it ends).
-    ``doc_start[b, s]`` is the first position of the document holding s, ``doc_end[b, s]`` one past its last position."""
+    Position s starts a document when s == 0 or tokens[b, s-1] == eos_id (the EOS belongs to the document it ends); ``eos_id``
+    None = the whole row is one document. ``doc_start[b, s]`` is the first position of the document holding s, ``doc_end[b, s]``
+    one past its last position. With a sliding ``window`` W, query s sees only the W most recent keys, itself included:
+    doc_start = max(doc_start, s - W + 1) and doc_end = min(doc_end, s + W), one past the last query that sees key s."""
     B, S = tokens.shape
-    is_eos = tokens == eos_id
+    is_eos = tokens == eos_id if eos_id is not None else torch.zeros((B, S), dtype=torch.bool, device=tokens.device)
     starts = torch.zeros((B, S), dtype=torch.bool, device=tokens.device)
     starts[:, 0] = True
     starts[:, 1:] = is_eos[:, :-1]
     pos = torch.arange(S, device=tokens.device).expand(B, S)
     doc_start = torch.where(starts, pos, 0).cummax(1).values  # latest start at or before s
     doc_end = torch.where(is_eos, pos + 1, S).flip(1).cummin(1).values.flip(1)  # first EOS at or after s, plus one
+    if window is not None:
+        doc_start = torch.maximum(doc_start, pos - window + 1)
+        doc_end = torch.minimum(doc_end, pos + window)
     return doc_start.int(), doc_end.int()
 
 

@@ -51,6 +51,7 @@ class Trainer:
         doc_eos_id = document_eos_id(cfg.data)  # before any allocation: a missing EOS id is a configuration error
         overrides = dict(model_overrides or {})
         overrides.setdefault("max_seq_len", max(cfg.data.seq_length, 128))
+        overrides.setdefault("sliding_window", cfg.sliding_window)
         self.memory_plan = self._plan_memory(cfg, mesh, overrides) if cuda else None  # refuse what cannot fit BEFORE allocating
         # identical init on every rank (same seed) — workers start from the same θ₀
         self.model: Transformer = build_model(cfg.name_model, cfg.type_model, device=self.device, dtype=dtype, seed=cfg.seed, **overrides)

@@ -2,9 +2,12 @@
 
     python tools/attn_bench.py                                         # the default Llama shapes
     python tools/attn_bench.py --shape 4,4096,16,16,128 --doc-len 256  # + document-masked kernels, 256-token documents
+    python tools/attn_bench.py --shape 4,8192,16,16,128 --window 1024  # + sliding-window attention over 1024 keys
 
 ``--doc-len N`` packs every row with documents of N tokens (EOS every N positions) and also times the document-masked kernels
-(``native_doc_*``) in the same process, so masked and plain causal attention are compared on one shape in one invocation."""
+(``native_doc_*``) in the same process, so masked and plain causal attention are compared on one shape in one invocation.
+``--window W`` does the same for sliding-window attention (``native_win_*``) and reports the ratio of tiles the kernels visit,
+counted from the bounds: key tiles of the forward / dQ kernels, query tiles of the dK/dV kernel."""
 
 import argparse
 import json
@@ -36,10 +39,20 @@ def timeit(fn, iters=10, warm=3, flush=None):
     return ts[len(ts) // 2]
 
 
+def tile_counts(lo: torch.Tensor, end: torch.Tensor) -> tuple[int, int]:
+    """Tiles the kernels visit for int32 [B, S] bounds, summed over rows: (64-key tiles of the forward / dQ kernels, 32-query tiles
+    of the dK/dV kernel). Per (b, head); the same loop bounds as csrc/attention_sm90.cu."""
+    blk = torch.arange(lo.shape[1] // 64, device=lo.device)
+    fwd = (blk - lo[:, ::64].long() // 64 + 1).sum()
+    dkdv = ((end[:, 63::64].long() + 31) // 32 - 2 * blk).sum()
+    return int(fwd), int(dkdv)
+
+
 def main():
     ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
     ap.add_argument("--shape", action="append", default=None, metavar="B,S,H,Hkv,D", help="shape to time (repeatable); default: Llama shapes")
     ap.add_argument("--doc-len", type=int, default=0, help="also time document-masked attention with documents of this many tokens")
+    ap.add_argument("--window", type=int, default=0, help="also time sliding-window attention over this many keys")
     a = ap.parse_args()
     shapes = [("1B mb16", 16, 1024, 16, 16, 128), ("7B-like", 8, 2048, 32, 32, 128), ("150M", 16, 1024, 16, 16, 64)]
     if a.shape:
@@ -98,6 +111,22 @@ def main():
             dboth = timeit(dfb, flush=flush)
             rows[-1].update({"doc_len": a.doc_len, "native_doc_fwd_ms": round(dfwd, 4), "native_doc_bwd_ms": round(dboth - dfwd, 4),
                              "doc_fwd_speedup": round(fwd / dfwd, 2), "doc_bwd_speedup": round((both - fwd) / (dboth - dfwd), 2)})  # fmt: skip
+        if a.window:
+            tok = torch.zeros((B, S), dtype=torch.int64, device=dev)
+            win = ops.document_bounds(tok, None, a.window)
+            wfwd = timeit(lambda: A.flash_attention_qkv(qkv, H, Hkv, True, win), flush=flush)
+
+            def wfb():
+                qkv.grad = None
+                A.flash_attention_qkv(qkv, H, Hkv, True, win).backward(dout)
+
+            wboth = timeit(wfb, flush=flush)
+            (cf, cb), (wf, wb) = tile_counts(*ops.document_bounds(tok, None)), tile_counts(*win)
+            rows[-1].update({"window": a.window, "native_win_fwd_ms": round(wfwd, 4), "native_win_bwd_ms": round(wboth - wfwd, 4),
+                             "win_fwd_speedup": round(fwd / wfwd, 2), "win_bwd_speedup": round((both - fwd) / (wboth - wfwd), 2),
+                             "win_fwd_tiles_per_bh": wf // B, "causal_fwd_tiles_per_bh": cf // B, "win_fwd_tile_ratio": round(cf / wf, 2),
+                             "win_dkdv_tiles_per_bhkv": wb // B, "causal_dkdv_tiles_per_bhkv": cb // B,
+                             "win_dkdv_tile_ratio": round(cb / wb, 2)})  # fmt: skip
         print(rows[-1], flush=True)
     (ROOT / "gpurun_out").mkdir(exist_ok=True)
     (ROOT / "gpurun_out" / "attn_bench.json").write_text(json.dumps({"rows": rows, "clocks": sampler.finish(),
