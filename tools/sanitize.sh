@@ -4,8 +4,8 @@
 # so each tool gets a focused subset; summaries land in gpurun_out/sanitizer_*.txt (copy to profiles/).
 set -u
 SAN=compute-sanitizer
-run() { # tool, pytest -k expression, tag
-  timeout 600 $SAN --tool "$1" --print-limit 5 --error-exitcode 9 python -m pytest tests/test_kernels_gpu.py -q -k "$2" -p no:cacheprovider \
+run() { # tool, pytest -k expression, tag[, test file]
+  timeout 600 $SAN --tool "$1" --print-limit 5 --error-exitcode 9 python -m pytest "${4:-tests/test_kernels_gpu.py}" -q -k "$2" -p no:cacheprovider \
     > gpurun_out/sanitizer_$3.log 2>&1
   echo "$1 [$2]: exit $? — $(grep -E 'ERROR SUMMARY|passed|failed' gpurun_out/sanitizer_$3.log | tr '\n' ' ')" | tee -a gpurun_out/sanitizer_summary.txt
 }
@@ -16,5 +16,7 @@ run memcheck  "flash_attention or rope_attention" memcheck_attention
 run racecheck "rmsnorm or cross_entropy" racecheck_elementwise
 run synccheck "gemm_transposed or flash_attention or rope_attention or qkv_gemm_rope" synccheck_tc
 run memcheck  "mxfp8" memcheck_mxfp8
+# tail rows, last vectors and partial tiles of the elementwise kernels and GEMM epilogues (the largest shapes are left to the plain run)
+run memcheck  "gpu and not 16384 and not 128256 and not 14336" memcheck_edges tests/test_kernel_edges_gpu.py
 run synccheck "mxfp8 or swiglu_epilogue" synccheck_mxfp8
 cat gpurun_out/sanitizer_summary.txt
