@@ -7,9 +7,10 @@
 
 The model is rebuilt on one device from the per-rank optimizer shards (``checkpoint.assemble_full_model``) or from a Hugging
 Face directory (``models.hf.load_hf_dir``); the forward runs through the same ops as training (native kernels on an H100, the
-reference ops on the CPU).  Generation recomputes the whole prefix for every token — there is no KV cache in a training engine —
-and pads the sequence to a multiple of 128 on CUDA (causal attention makes right padding invisible to the position that is read),
-which is fine for inspecting a checkpoint and not a serving path.
+reference ops on the CPU).  Generation runs on a KV cache (``inference.py``): one prefill of the prompt, padded to a multiple of 128
+on CUDA, then one decode step per token (the split-KV decode-attention kernel, the step replayed from a CUDA graph on the GPU), so
+T new tokens cost one prompt forward and T single-token steps instead of T full forwards. ``generate_batch`` samples ragged
+prompt lists together. Sliding windows and document masking (``Transformer.doc_eos_id``) behave as in the full forward.
 """
 
 from __future__ import annotations
@@ -22,6 +23,7 @@ import torch
 import torch.nn.functional as F
 
 from .data import MemmapTokenDataset
+from .inference import generate_batch, sample
 from .models.llama import Transformer
 
 
@@ -41,10 +43,17 @@ def perplexity(model: Transformer, dataset, *, batches: int, batch_size: int, de
     return {"loss": loss, "perplexity": math.exp(min(loss, 50.0)), "tokens": n}
 
 
-@torch.no_grad()
 def generate(model: Transformer, prompt: list[int], *, max_new: int, temperature: float = 0.0, top_k: int = 0, seed: int = 0,
              eos_id: int | None = None) -> list[int]:  # fmt: skip
     """Greedy (temperature 0) or top-k / temperature sampling; returns prompt + continuation."""
+    return generate_batch(model, [prompt], max_new=max_new, temperature=temperature, top_k=top_k, seed=seed, eos_id=eos_id)[0]
+
+
+@torch.no_grad()
+def _generate_recompute(model: Transformer, prompt: list[int], *, max_new: int, temperature: float = 0.0, top_k: int = 0, seed: int = 0,
+                        eos_id: int | None = None) -> list[int]:  # fmt: skip
+    """:func:`generate` without a cache: the whole prefix is run again for every token (padded to a multiple of 128 on CUDA). The
+    oracle of the cached path and the baseline of its speed-up."""
     model.eval()
     dev = next(model.parameters()).device
     ids = list(prompt)
@@ -56,14 +65,7 @@ def generate(model: Transformer, prompt: list[int], *, max_new: int, temperature
             break
         padded = ids + [0] * ((-n) % pad_to)
         logits = model(torch.tensor([padded], dtype=torch.int64, device=dev))[0, n - 1].float().cpu()
-        if temperature <= 0:
-            nxt = int(logits.argmax())
-        else:
-            logits = logits / temperature
-            if top_k > 0:
-                kth = torch.topk(logits, min(top_k, logits.numel())).values[-1]
-                logits = logits.masked_fill(logits < kth, float("-inf"))
-            nxt = int(torch.multinomial(torch.softmax(logits, -1), 1, generator=gen))
+        nxt = sample(logits, temperature, top_k, gen)
         ids.append(nxt)
         if eos_id is not None and nxt == eos_id:
             break

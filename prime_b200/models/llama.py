@@ -107,23 +107,43 @@ class Attention(nn.Module):
         self.wo = nn.Parameter(torch.empty(args.dim, self.n_heads * self.head_dim))
         self.fp8 = False  # train.fp8: MXFP8 forward / input-gradient GEMMs (Transformer.set_fp8)
 
-    def forward(self, x: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor, attn_impl: str = "auto", doc: tuple | None = None) -> torch.Tensor:
+    def forward(self, x: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor, attn_impl: str = "auto", doc: tuple | None = None,
+                kv=None) -> torch.Tensor:  # fmt: skip
         """``doc``: (doc_start, doc_end) of ``ops.document_bounds`` for document-masked and / or sliding-window attention, None =
-        plain causal."""
+        plain causal. ``kv``: this layer's handle of an ``inference.KVCache``, None outside generation. When prefilling, the rotated
+        K|V columns of every position are also copied into the cache; when decoding, ``x`` is [B, 1, dim], the new token is appended
+        to the cache and attends over it."""
         B, S, _ = x.shape
         H, Hkv, D = self.n_heads, self.n_kv_heads, self.head_dim
+        if kv is not None and kv.decoding:
+            qkv = ops.linear(x, self.wqkv).view(B, -1)  # M = B: the new token of every row
+            ops.kv_append(qkv, kv.kv, kv.cache.len, cos, sin, H, Hkv)
+            out = ops.decode_attention(qkv, kv.kv, kv.cache.len, kv.cache.lo, kv.cache.window, H, Hkv)
+            return ops.linear(out.view(B, 1, H * D), self.wo)
         if self.fp8:
             qkv = ops.linear_mxfp8(x, self.wqkv)
-            out = ops.rope_attention_qkv(qkv, cos, sin, H, Hkv, causal=True, impl=attn_impl, doc=doc)
+            out = self._prefill_attention(qkv, cos, sin, attn_impl, doc, kv)
             return ops.linear_mxfp8(out, self.wo)
         if attn_impl in ("auto", "native") and ops.rope_fusable(x, H, Hkv, D):
             # RoPE rides in the QKV GEMM epilogue (forward) and in the dQ/dK epilogues of the attention backward: no rotation pass
             qkv = ops.linear_qkv_rope(x, self.wqkv, cos, sin, H, Hkv)  # [B, S, (H+2Hkv)·D], Q/K heads rotated
+            if kv is not None:
+                kv.store(qkv, H * D)
             out = ops.rope_attention_qkv(qkv, cos, sin, H, Hkv, causal=True, impl=attn_impl, pre_rotated=True, doc=doc)
         else:
             qkv = ops.linear(x, self.wqkv)  # [B, S, (H+2Hkv)·D]
-            out = ops.rope_attention_qkv(qkv, cos, sin, H, Hkv, causal=True, impl=attn_impl, doc=doc)  # [B, S, H·D], no layout shuffles
+            out = self._prefill_attention(qkv, cos, sin, attn_impl, doc, kv)  # [B, S, H·D], no layout shuffles
         return ops.linear(out, self.wo)
+
+    def _prefill_attention(self, qkv: torch.Tensor, cos, sin, attn_impl: str, doc: tuple | None, kv) -> torch.Tensor:
+        """RoPE ⊕ attention of the un-rotated fused QKV. With a cache handle the rotation runs as its own op (``rope_qkv``: in place
+        on CUDA, a new tensor on the CPU), so that the rotated K|V can be copied into the cache before the attention reads them."""
+        H, Hkv = self.n_heads, self.n_kv_heads
+        if kv is None:
+            return ops.rope_attention_qkv(qkv, cos, sin, H, Hkv, causal=True, impl=attn_impl, doc=doc)
+        qkv = ops.rope_qkv(qkv, cos, sin, H, Hkv)
+        kv.store(qkv, H * self.head_dim)
+        return ops.attention_qkv(qkv, H, Hkv, causal=True, impl=attn_impl, doc=doc)
 
 
 class FeedForward(nn.Module):
@@ -151,13 +171,14 @@ class TransformerBlock(nn.Module):
         self.eps = args.norm_eps
         self.init_std = 0.02 / math.sqrt(2 * (layer_id + 1)) if args.depth_init else 0.02 / math.sqrt(2 * args.n_layers)
 
-    def forward(self, h: torch.Tensor, delta: torch.Tensor | None, cos, sin, attn_impl: str = "auto", doc: tuple | None = None):
-        """``h`` = residual stream, ``delta`` = output of the previous sub-block not yet added, ``doc`` = document bounds or None."""
+    def forward(self, h: torch.Tensor, delta: torch.Tensor | None, cos, sin, attn_impl: str = "auto", doc: tuple | None = None, kv=None):
+        """``h`` = residual stream, ``delta`` = output of the previous sub-block not yet added, ``doc`` = document bounds or None,
+        ``kv`` = this layer's KV-cache handle or None (see :meth:`Attention.forward`)."""
         if delta is None:
             x = ops.rmsnorm(h, self.attention_norm.weight, self.eps)
         else:
             x, h = ops.add_rmsnorm(delta, h, self.attention_norm.weight, self.eps)
-        a = self.attention(x, cos, sin, attn_impl, doc)
+        a = self.attention(x, cos, sin, attn_impl, doc, kv)
         y, h = ops.add_rmsnorm(a, h, self.ffn_norm.weight, self.eps)
         return h, self.feed_forward(y)
 
@@ -213,7 +234,8 @@ class Transformer(nn.Module):
         return self._rope
 
     # ------------------------------------------------------------------ forward
-    def forward_hidden(self, tokens: torch.Tensor) -> torch.Tensor:
+    def forward_hidden(self, tokens: torch.Tensor, cache=None) -> torch.Tensor:
+        """Final hidden states [B, S, dim]. ``cache``: an ``inference.KVCache`` that receives every layer's rotated K|V (prefill)."""
         B, S = tokens.shape
         cos, sin = self.rope_tables(S, tokens.device)
         h = ops.embedding(tokens, self.tok_embeddings.weight)
@@ -230,12 +252,25 @@ class Transformer(nn.Module):
 
                 h, delta = checkpoint(layer, h, delta, cos, sin, self.attn_impl, doc, use_reentrant=False)
             else:
-                h, delta = layer(h, delta, cos, sin, self.attn_impl, doc)
+                h, delta = layer(h, delta, cos, sin, self.attn_impl, doc, None if cache is None else cache.layer(i))
         x, _ = ops.add_rmsnorm(delta, h, self.norm.weight, self.args.norm_eps)
         return x
 
     def forward(self, tokens: torch.Tensor) -> torch.Tensor:
         return ops.linear(self.forward_hidden(tokens), self.output)
+
+    def decode_step(self, tokens: torch.Tensor, cache) -> torch.Tensor:
+        """One generation step over a filled ``inference.KVCache``: ``tokens`` int64 [B], the next token of every row → logits [B, V]
+        of the token after it. The same blocks run on [B, 1, dim]; only attention appends to the cache and reads it. Every input that
+        changes between steps is on the device, so the step can be captured in a CUDA graph over a static token buffer."""
+        B = tokens.shape[0]
+        ops.decode_advance(tokens, cache.len, cache.lo, cache.last_tok, self.doc_eos_id)
+        h = ops.embedding(tokens.view(B, 1), self.tok_embeddings.weight)
+        delta = None
+        for i, layer in enumerate(self.layers):
+            h, delta = layer(h, delta, cache.cos, cache.sin, self.attn_impl, None, cache.layer(i, decoding=True))
+        x, _ = ops.add_rmsnorm(delta, h, self.norm.weight, self.args.norm_eps)
+        return ops.linear(x.view(B, -1), self.output)
 
     def loss(self, tokens: torch.Tensor, targets: torch.Tensor, *, grad_scale: float = 1.0, loss_acc: torch.Tensor | None = None) -> torch.Tensor:
         """Mean next-token loss; gradient (not value) is scaled by ``grad_scale``; call ``.backward()`` on it. ``loss_acc``: fp32

@@ -157,6 +157,11 @@ def _sigs() -> dict:
         "pb_flash_attn_fwd": [vp, vp, vp, vp, i32, i32, i32, i32, i32, f32, i32, vp],
         "pb_flash_attn_bwd": [vp, vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, f32, i32, vp, vp, vp],
         "pb_doc_bounds": [vp, i32, i32, i64, i32, vp, vp, vp],
+        # KV-cache decoding (csrc/decode_sm90.cu)
+        "pb_decode_advance": [vp, i64, vp, vp, vp, i32, vp],
+        "pb_kv_append": [vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, vp],
+        "pb_decode_attn": [vp, vp, vp, vp, i32, vp, vp, i32, i32, i32, i32, i32, i32, f32, vp],
+        "pb_decode_attn_splits": [i32, i32, i32],
         "pb_ipc_alloc": [ctypes.POINTER(vp), ctypes.c_size_t],
         "pb_ipc_free": [vp],
         "pb_ipc_handle_size": [],

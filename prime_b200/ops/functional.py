@@ -8,6 +8,7 @@ native library on the *current* torch stream (so they compose with streams and C
 
 from __future__ import annotations
 
+import math
 
 import torch
 
@@ -814,3 +815,88 @@ def rope_attention_qkv(qkv: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor, 
     if pre_rotated:
         raise RuntimeError("pre_rotated=True needs the native attention path (its backward undoes the rotation)")
     return attention_qkv(rope_qkv(qkv, cos, sin, n_heads, n_kv_heads), n_heads, n_kv_heads, causal, impl, doc)
+
+
+# --------------------------------------------------------------------------- KV-cache decoding
+
+
+def _decode_native(qkv: torch.Tensor, kv: torch.Tensor, n_heads: int, n_kv_heads: int) -> bool:
+    """Shapes and layouts the decode kernels (csrc/decode_sm90.cu) take: bf16, contiguous, D in {64, 128}, H % Hkv == 0."""
+    D = qkv.shape[-1] // (n_heads + 2 * n_kv_heads)
+    return (qkv.is_cuda and qkv.dtype == torch.bfloat16 and kv.dtype == torch.bfloat16 and qkv.is_contiguous() and kv.is_contiguous()
+            and D in (64, 128) and n_heads % n_kv_heads == 0)  # fmt: skip
+
+
+def decode_attn_splits(batch: int, n_kv_heads: int, capacity: int) -> int:
+    """The native split policy of :func:`decode_attention`: a function of the cache geometry only (never of the lengths), so one
+    captured decode step stays valid at every position."""
+    n = int(_lib.load().pb_decode_attn_splits(batch, n_kv_heads, capacity))
+    _lib.check(min(n, 0), "pb_decode_attn_splits")
+    return n
+
+
+def decode_advance(tokens: torch.Tensor, length: torch.Tensor, lo: torch.Tensor, last_tok: torch.Tensor, eos_id: int | None) -> None:
+    """Per-row bookkeeping at the start of a decode step, in place: pos = len; lo = pos if last_tok == eos_id; len = pos + 1;
+    last_tok = tokens. ``tokens`` / ``last_tok`` int64 [B], ``length`` / ``lo`` int32 [B]; ``eos_id`` None = no documents."""
+    if tokens.is_cuda:
+        assert tokens.dtype == last_tok.dtype == torch.int64 and length.dtype == lo.dtype == torch.int32
+        assert tokens.is_contiguous() and length.is_contiguous() and lo.is_contiguous() and last_tok.is_contiguous()
+        _launch("pb_decode_advance", tokens.data_ptr(), -1 if eos_id is None else int(eos_id), length.data_ptr(), lo.data_ptr(),
+                last_tok.data_ptr(), tokens.shape[0], _stream())  # fmt: skip
+        return
+    if eos_id is not None:
+        lo.copy_(torch.where(last_tok == eos_id, length, lo))
+    length.add_(1)
+    last_tok.copy_(tokens)
+
+
+def kv_append(qkv: torch.Tensor, kv: torch.Tensor, length: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor, n_heads: int,
+              n_kv_heads: int) -> torch.Tensor:  # fmt: skip
+    """The new token of every row, un-rotated fused QKV [B, (H+2Hkv)·D], at position len[b] - 1: rotates its Q heads in place and
+    writes its rotated K heads and its V heads into row len[b] - 1 of the layer's cache ``kv`` [B, capacity, 2·Hkv·D]. Rows whose
+    position is outside the cache are left alone. Returns ``qkv``."""
+    B = qkv.shape[0]
+    H, Hkv = n_heads, n_kv_heads
+    D = qkv.shape[-1] // (H + 2 * Hkv)
+    cap = kv.shape[1]
+    if _decode_native(qkv, kv, H, Hkv):
+        assert length.dtype == torch.int32 and cos.dtype == torch.float32 and cos.is_contiguous() and sin.is_contiguous()
+        assert cos.shape[0] >= cap and cos.shape[1] == D // 2
+        _launch("pb_kv_append", qkv.data_ptr(), kv.data_ptr(), length.data_ptr(), cos.data_ptr(), sin.data_ptr(), B, H, Hkv, D, cap,
+                _stream())  # fmt: skip
+        return qkv
+    pos = length.long() - 1
+    ok = (pos >= 0) & (pos < cap)
+    p = pos.clamp(0, cap - 1)
+    x = qkv.view(B, H + 2 * Hkv, D)
+    rot = reference.rope_at(x[:, : H + Hkv], cos[p], sin[p])
+    # no host synchronisation (no nonzero / item): on CUDA this fallback is captured in the decode step's graph as well
+    flat = kv.view(B * cap, -1)
+    idx = torch.arange(B, device=kv.device) * cap + p
+    new = torch.cat((rot[:, H:], x[:, H + Hkv :]), dim=1).reshape(B, -1)
+    flat.index_copy_(0, idx, torch.where(ok.view(B, 1), new, flat.index_select(0, idx)))
+    x[:, :H] = torch.where(ok.view(B, 1, 1), rot[:, :H], x[:, :H])
+    return qkv
+
+
+def decode_attention(qkv: torch.Tensor, kv: torch.Tensor, length: torch.Tensor, lo: torch.Tensor | None, window: int | None,
+                     n_heads: int, n_kv_heads: int, splits: int | None = None) -> torch.Tensor:  # fmt: skip
+    """Attention of the one (rotated) query per row in ``qkv`` [B, (H+2Hkv)·D] over the layer's cache ``kv`` [B, capacity, 2·Hkv·D]
+    → [B, H·D]. Row b sees keys max(lo[b], len[b] - window) <= k < len[b] (``lo`` None = 0, ``window`` None = none). On CUDA the
+    split-KV kernel (one launch, or two with the combine when ``splits`` > 1; None = :func:`decode_attn_splits`), else the fp32
+    :func:`reference.decode_attention`."""
+    B = qkv.shape[0]
+    H, Hkv = n_heads, n_kv_heads
+    D = qkv.shape[-1] // (H + 2 * Hkv)
+    cap = kv.shape[1]
+    if _decode_native(qkv, kv, H, Hkv):
+        assert length.dtype == torch.int32 and (lo is None or lo.dtype == torch.int32)
+        if splits is None:
+            splits = decode_attn_splits(B, Hkv, cap)
+        out = torch.empty((B, H * D), dtype=qkv.dtype, device=qkv.device)
+        part = torch.empty((B, H, splits, D + 2), dtype=torch.float32, device=qkv.device) if splits > 1 else None
+        _launch("pb_decode_attn", qkv.data_ptr(), kv.data_ptr(), length.data_ptr(), _ptr(lo), int(window or 0), out.data_ptr(), _ptr(part),
+                B, H, Hkv, D, cap, splits, 1.0 / math.sqrt(D), _stream(), n=1 if splits == 1 else 2)  # fmt: skip
+        return out
+    q = qkv.view(B, H + 2 * Hkv, D)[:, :H]
+    return reference.decode_attention(q, kv, length, lo, window).reshape(B, H * D).to(qkv.dtype)

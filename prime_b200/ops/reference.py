@@ -104,6 +104,37 @@ def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, causal: bool = 
     return out.transpose(1, 2).to(q.dtype)
 
 
+def rope_at(x: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor) -> torch.Tensor:
+    """x: [B, heads, D] of one token per row; cos / sin: that token's table rows [B, D/2]. Interleaved pairs, as :func:`rope`."""
+    B, Hh, D = x.shape
+    xf = x.float().reshape(B, Hh, D // 2, 2)
+    c, s = cos.view(B, 1, D // 2), sin.view(B, 1, D // 2)
+    x0, x1 = xf[..., 0], xf[..., 1]
+    return torch.stack((x0 * c - x1 * s, x0 * s + x1 * c), dim=-1).reshape(B, Hh, D).to(x.dtype)
+
+
+def decode_attention(q: torch.Tensor, kv: torch.Tensor, length: torch.Tensor, lo: torch.Tensor | None = None,
+                     window: int | None = None) -> torch.Tensor:  # fmt: skip
+    """One query per row over a KV cache, in fp32: q [B, H, D] (rotated), kv [B, capacity, 2·Hkv·D] (rotated K heads, then V heads)
+    → [B, H, D]. Row b sees keys max(lo[b], len[b] - window) <= k < len[b] (``lo`` None = 0, ``window`` None or 0 = none): the rule
+    of :func:`document_bounds` for the query at position len[b] - 1. A row that sees no key gets zeros."""
+    B, H, D = q.shape
+    cap = kv.shape[1]
+    Hkv = kv.shape[2] // (2 * D)
+    kf = kv[..., : Hkv * D].float().reshape(B, cap, Hkv, D).repeat_interleave(H // Hkv, dim=2)
+    vf = kv[..., Hkv * D :].float().reshape(B, cap, Hkv, D).repeat_interleave(H // Hkv, dim=2)
+    L = length.long().clamp(max=cap).view(B, 1)
+    start = torch.zeros_like(L) if lo is None else lo.long().view(B, 1)
+    if window:
+        start = torch.maximum(start, L - window)
+    k = torch.arange(cap, device=q.device).view(1, cap)
+    visible = (k >= start) & (k < L)
+    scores = torch.einsum("bhd,bkhd->bhk", q.float(), kf) / math.sqrt(D)
+    p = scores.masked_fill(~visible.unsqueeze(1), float("-inf")).softmax(-1).nan_to_num(0.0)
+    # rows nobody may read (beyond len, or never written) can hold anything, NaN included: 0·NaN must not reach the output
+    return torch.einsum("bhk,bkhd->bhd", p, vf.masked_fill(~visible.view(B, cap, 1, 1), 0.0))
+
+
 def cross_entropy(logits: torch.Tensor, targets: torch.Tensor, ignore_index: int = -100) -> torch.Tensor:
     return F.cross_entropy(logits.float().view(-1, logits.shape[-1]), targets.view(-1), ignore_index=ignore_index)
 

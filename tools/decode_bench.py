@@ -1,0 +1,171 @@
+"""KV-cache decoding on one GPU: the split-KV decode-attention kernel against SDPA, and end-to-end generation.
+
+    python tools/decode_bench.py [--out results.json] [--skip-e2e]
+
+Kernel section: ``ops.decode_attention`` (pb_decode_attn, split policy of pb_decode_attn_splits) at 1B heads (H = Hkv = 16) and
+Llama-3-8B heads (H = 32, Hkv = 8), D = 128, B ∈ {1, 8, 32} × context ∈ {1 K, 8 K, 32 K}, plus one windowed case; every row sees
+the whole context. CUDA events around one call, median of 20 with a 256 MB L2 flush before each. Bytes read = the visible K and V
+rows (2·Hkv·D·2 bytes each) plus Q and the output; the share of bandwidth is against the 3.35 TB/s of the H100 SXM data sheet.
+The comparison arm is ``F.scaled_dot_product_attention`` with a one-token query over the same cache (strided views, GQA), in the
+same process.
+
+End-to-end section: a random-init Llama-2 1B, prompt 512, 256 new tokens, greedy, B ∈ {1, 8}: tokens/s of cached generation with
+CUDA graphs, cached generation eager, and the recompute loop (``eval._generate_recompute``, one row at a time). Also the share of
+one eager decode step's kernel time spent in the M = B GEMMs (torch.profiler, a separate pass).
+"""
+
+from __future__ import annotations
+
+import argparse
+import json
+import statistics
+import subprocess
+import sys
+import time
+from pathlib import Path
+
+import torch
+import torch.nn.functional as F
+
+sys.path.insert(0, str(Path(__file__).resolve().parent.parent))
+
+from prime_b200 import eval as ev  # noqa: E402
+from prime_b200 import inference, ops  # noqa: E402
+from prime_b200.models.llama import build_model  # noqa: E402
+
+HBM_BPS = 3.35e12
+
+
+def card() -> dict:
+    out = {"name": torch.cuda.get_device_name(0)}
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
+                           capture_output=True, text=True, timeout=30).stdout.strip()  # fmt: skip
+        out["power_limit"], out["max_sm_clock"] = (x.strip() for x in q.split(","))
+    except Exception as e:  # noqa: BLE001
+        out["power_limit"] = f"unread: {e}"
+    return out
+
+
+def timed(fn, flush: torch.Tensor, reps: int = 20) -> float:
+    """Median ms of ``fn`` over ``reps`` calls, each after an L2 flush, CUDA events around the call only."""
+    fn()
+    torch.cuda.synchronize()
+    ts = []
+    for _ in range(reps):
+        flush.zero_()
+        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        a.record()
+        fn()
+        b.record()
+        b.synchronize()
+        ts.append(a.elapsed_time(b))
+    return statistics.median(ts)
+
+
+def kernel_section(flush) -> list[dict]:
+    rows = []
+    D = 128
+    cases = [(H, Hkv, B, ctx, None) for (H, Hkv) in ((16, 16), (32, 8)) for B in (1, 8, 32) for ctx in (1024, 8192, 32768)]
+    cases.append((32, 8, 8, 32768, 4096))
+    for H, Hkv, B, ctx, window in cases:
+        dev = torch.device("cuda", 0)
+        kv = torch.randn(B, ctx, 2 * Hkv * D, device=dev, dtype=torch.bfloat16)
+        qkv = torch.randn(B, (H + 2 * Hkv) * D, device=dev, dtype=torch.bfloat16)
+        length = torch.full((B,), ctx, dtype=torch.int32, device=dev)
+        ms = timed(lambda: ops.decode_attention(qkv, kv, length, None, window, H, Hkv), flush)
+        vis = min(ctx, window or ctx)
+        nbytes = B * vis * 2 * Hkv * D * 2 + 2 * B * H * D * 2
+        r = {"heads": f"{H}/{Hkv}", "B": B, "context": ctx, "window": window, "splits": ops.decode_attn_splits(B, Hkv, ctx), "ms": round(ms, 4),
+             "bytes": nbytes, "GB_s": round(nbytes / ms / 1e6, 1), "share_of_3.35TB_s": round(nbytes / ms / 1e-3 / HBM_BPS, 3)}  # fmt: skip
+        q = qkv[:, : H * D].view(B, H, 1, D)
+        k = kv[..., : Hkv * D].view(B, ctx, Hkv, D).transpose(1, 2)
+        v = kv[..., Hkv * D :].view(B, ctx, Hkv, D).transpose(1, 2)
+        mask = None
+        if window:
+            mask = torch.zeros(1, 1, 1, ctx, dtype=torch.bool, device=dev)
+            mask[..., ctx - window :] = True
+        try:
+            sd = timed(lambda: F.scaled_dot_product_attention(q, k, v, attn_mask=mask, enable_gqa=H != Hkv), flush)
+            r["sdpa_ms"] = round(sd, 4)
+            r["speedup_vs_sdpa"] = round(sd / ms, 2)
+        except Exception as e:  # noqa: BLE001
+            r["sdpa_ms"] = f"failed: {type(e).__name__}"
+        print(json.dumps(r), flush=True)
+        rows.append(r)
+        del kv, qkv
+        torch.cuda.empty_cache()
+    return rows
+
+
+def e2e_section(prompt_len: int = 512, new: int = 256) -> list[dict]:
+    model = build_model("1B", device="cuda", dtype=torch.bfloat16, seed=0).eval()
+    g = torch.Generator().manual_seed(0)
+    rows = []
+    for B in (1, 8):
+        prompts = [torch.randint(0, model.args.vocab_size, (prompt_len,), generator=g).tolist() for _ in range(B)]
+        r = {"B": B, "prompt": prompt_len, "new_tokens": new}
+        for name, graphs in (("cached_graphs", True), ("cached_eager", False)):
+            ev.generate_batch(model, prompts, max_new=8, graphs=graphs)  # warm-up: library, kernel attributes
+            torch.cuda.synchronize()
+            t = time.perf_counter()
+            out = ev.generate_batch(model, prompts, max_new=new, graphs=graphs)
+            torch.cuda.synchronize()
+            dt = time.perf_counter() - t
+            r[f"{name}_tok_s"] = round(sum(len(o) - prompt_len for o in out) / dt, 1)
+        if B == 1:
+            ev._generate_recompute(model, prompts[0], max_new=4)
+            torch.cuda.synchronize()
+            t = time.perf_counter()
+            out = ev._generate_recompute(model, prompts[0], max_new=new)
+            torch.cuda.synchronize()
+            r["recompute_tok_s"] = round((len(out) - prompt_len) / (time.perf_counter() - t), 1)
+        r["gemm_share_of_decode_step"] = gemm_share(model, prompts, prompt_len + new)
+        print(json.dumps(r), flush=True)
+        rows.append(r)
+    return rows
+
+
+@torch.no_grad()
+def gemm_share(model, prompts, capacity: int) -> float:
+    """Share of one eager decode step's CUDA kernel time in the GEMM kernels (QKV, output, gate/up, down projections, LM head)."""
+    from torch.profiler import ProfilerActivity, profile
+
+    _, cache = inference.prefill(model, prompts, inference.cache_capacity(model.args.max_seq_len, [len(p) for p in prompts], capacity))
+    tok = torch.zeros(len(prompts), dtype=torch.int64, device="cuda")
+    for _ in range(3):
+        model.decode_step(tok, cache)
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(5):
+            model.decode_step(tok, cache)
+        torch.cuda.synchronize()
+    tot = gemm = 0.0
+    for e in prof.key_averages():
+        t = e.device_time_total
+        tot += t
+        if "gemm" in e.key.lower():
+            gemm += t
+    return round(gemm / tot, 3) if tot else float("nan")
+
+
+def main() -> None:
+    ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
+    ap.add_argument("--out", default=None, help="also write the results as JSON here")
+    ap.add_argument("--skip-e2e", action="store_true")
+    a = ap.parse_args()
+    if not torch.cuda.is_available():
+        raise SystemExit("decode_bench needs a CUDA device")
+    info = card()
+    print(json.dumps({"card": info}), flush=True)
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")
+    res = {"card": info, "kernel": kernel_section(flush)}
+    if not a.skip_e2e:
+        res["e2e"] = e2e_section()
+    if a.out:
+        Path(a.out).parent.mkdir(parents=True, exist_ok=True)
+        Path(a.out).write_text(json.dumps(res, indent=1))
+
+
+if __name__ == "__main__":
+    main()

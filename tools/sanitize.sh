@@ -19,4 +19,6 @@ run memcheck  "mxfp8" memcheck_mxfp8
 # tail rows, last vectors and partial tiles of the elementwise kernels and GEMM epilogues (the largest shapes are left to the plain run)
 run memcheck  "gpu and not 16384 and not 128256 and not 14336" memcheck_edges tests/test_kernel_edges_gpu.py
 run synccheck "mxfp8 or swiglu_epilogue" synccheck_mxfp8
+# decode kernels: KV append, step bookkeeping and split-KV attention at the small shapes (the 32 K-key fp64 sweep is left to the plain run)
+run memcheck  "gpu and (kv_append or decode_advance or graph_replay or generate_on_cuda)" memcheck_decode tests/test_kv_cache.py
 cat gpurun_out/sanitizer_summary.txt
