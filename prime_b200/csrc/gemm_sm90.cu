@@ -10,9 +10,11 @@
 //     dx = dy W       : A=dy (K-major)   B=W  (MN-major)
 //     dW = dyᵀ x      : A=dy (MN-major)  B=x  (MN-major)     (fp32 accumulate into main_grad)
 //
-// Tile 128 x 128 x 64, 6-stage TMA ring (32 KB / stage; 5 stages when the weight-gather copier takes 32 KB).
+// Tile 128 x BN x 64. BN = 128: 6-stage TMA ring (32 KB / stage; 5 stages when the weight-gather copier takes 32 KB).
+// BN = 256 (local GEMMs only, IO = 0): 4 stages of 48 KB; the producer warpgroup drops to 40 registers and the consumer
+// warpgroups rise to 232 (setmaxnreg) to hold 128 fp32 accumulators per thread. tile_policy() picks BN from the shape.
 // Warp roles: warpgroup 0 = w0 TMA producer (1 lane), w3 gather copier (IO = 1 / 3); warpgroups 1 and 2 = consumers, each
-// issuing m64n128k16 wgmma for 64 rows of the tile and running the epilogue of those rows straight from its registers, while
+// issuing m64nBNk16 wgmma for 64 rows of the tile and running the epilogue of those rows straight from its registers, while
 // the producer already fills the ring for the next tile.
 #include <cuda.h>
 
@@ -35,24 +37,26 @@ struct GemmEpilogue {
 
 namespace {
 
-constexpr int BM = 128, BN = 128, BK = 64;
+constexpr int BM = 128, BN = 128, BK = 64;  // BN: the narrow tile, the only one of the collective variants
+constexpr int kWideBN = 256;
 constexpr int kThreads = 384;
 constexpr int kConsumerWarps = 8;
 constexpr uint32_t kABytes = BM * BK * 2;  // 16 KB
-constexpr uint32_t kBBytes = BN * BK * 2;  // 16 KB
-constexpr uint32_t kStageBytes = kABytes + kBBytes;
 constexpr int kGroupM = 16;  // raster: super-rows of 16 M-tiles keep the A slab L2-resident
 
 constexpr uint32_t kCopyChunkBytes = 128 * BK * 2;  // IO = 3 weight-gather copier: one {64 col, 128 row} box = 16 KB
 constexpr int kCopyBufs = 2;
 constexpr int kGatherSub = 4;  // IO = 3: readiness flags per rank block (a block is released to the MMA tiles in quarters)
 
-template <int IO>
+template <int IO, int TBN>
 struct Geo {
-  static constexpr int kStages = IO == 3 ? 5 : 6;
+  static constexpr int kStages = TBN == kWideBN ? 4 : IO == 3 ? 5 : 6;
+  static constexpr uint32_t kBBytes = TBN * BK * 2;  // 16 | 32 KB
+  static constexpr uint32_t kStageBytes = kABytes + kBBytes;
   static constexpr uint32_t kCopyBytes = IO == 3 ? kCopyBufs * kCopyChunkBytes : 0;
   static constexpr uint32_t kSmemBytes = kStages * kStageBytes + kCopyBytes + 1024 /*align slack*/ + 512 /*barriers*/;
 };
+static_assert(Geo<0, kWideBN>::kSmemBytes <= 227 * 1024, "wide tile ring exceeds the shared memory of an SM");
 
 using namespace tc;
 
@@ -189,13 +193,18 @@ __device__ __forceinline__ uint32_t bf16x2_bits(float lo, float hi) {
 // EPI: 0 = plain, 1 = RoPE on the leading output columns, 2 = SwiGLU, 3 = SwiGLU backward. Separate instantiations on purpose: the
 // fused epilogues need more registers, and a plain GEMM compiled with that footprint leaves less of the register file to the
 // gradient-reduction / optimizer kernels of the comm stream that co-reside with it during the backward pass.
-template <int A_MN, int B_MN, int EPI, int IO>
+// TBN: tile width, BN or kWideBN (IO = 0 only). tmap_g: IO = 3 the local full-weight copy; IO = 0 wide SwiGLU the up rows of W13
+// (tmap_b then covers the FF gate rows only, so the TMA unit zero-fills a last tile that is half past FF).
+template <int A_MN, int B_MN, int EPI, int IO, int TBN>
 __global__ void __launch_bounds__(kThreads, 1)
     gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                      const __grid_constant__ CUtensorMap tmap_g, const __grid_constant__ CUtensorMap tmap_g2, const GemmParams p,
                      const __grid_constant__ PeerMaps pm) {
-  using G = Geo<IO>;
+  static_assert(TBN == BN || (TBN == kWideBN && IO == 0), "the wide tile exists for local GEMMs only");
+  constexpr bool wide = TBN == kWideBN;
+  using G = Geo<IO, TBN>;
   constexpr int kStages = G::kStages;
+  constexpr uint32_t kStageBytes = G::kStageBytes;
   const int sched_id = (int)blockIdx.x;
   const int sched_n = (int)gridDim.x;
   extern __shared__ uint8_t smem_raw[];
@@ -208,7 +217,9 @@ __global__ void __launch_bounds__(kThreads, 1)
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   constexpr bool swiglu = EPI == 2;
-  const int tiles_m = (p.M + BM - 1) / BM, tiles_n = swiglu ? p.swiglu_ff / 64 : (p.N + BN - 1) / BN;
+  // SwiGLU: a tile covers TBN / 2 features (the gate and the up rows of each)
+  const int tiles_m = (p.M + BM - 1) / BM;
+  const int tiles_n = swiglu ? (wide ? (p.swiglu_ff + TBN / 2 - 1) / (TBN / 2) : p.swiglu_ff / 64) : (p.N + TBN - 1) / TBN;
   const int num_kb = (p.K + BK - 1) / BK;
   // split-K: work item w = tile * split_k + slice; slice s covers k-blocks [s*kb_per, min(num_kb, (s+1)*kb_per))
   const int split_k = p.split_k;
@@ -263,9 +274,11 @@ __global__ void __launch_bounds__(kThreads, 1)
   }
   __syncthreads();
 
-  if (warp == 0) {
+  if (warp == 0 || (wide && warp < 4)) {
     // ------------------------------------------------------------------ TMA producer
-    if (lane == 0) {
+    // wide tile: the whole warpgroup hands registers to the consumers; lane 0 of warp 0 is the producer
+    if constexpr (wide) setmaxnreg_dec<40>();
+    if (lane == 0 && (!wide || warp == 0)) {
       int stage = 0;
       uint32_t phase = 0;
       // gather tiles have the lowest indices: this CTA's are tiles sched_id, sched_id + sched_n, … below G
@@ -299,8 +312,8 @@ __global__ void __launch_bounds__(kThreads, 1)
         const int kb0 = (tile % split_k) * kb_per, kb1 = min(num_kb, kb0 + kb_per);
         if (kb0 >= kb1) continue;  // empty K slice (split does not divide K): every role skips it identically
         const int m0 = tm * BM;
-        // SwiGLU: 64 gate rows and the matching 64 up rows; otherwise 128 consecutive B rows
-        const int n0 = swiglu ? tn * 64 : tn * BN;
+        // SwiGLU: TBN / 2 gate rows and the matching up rows; otherwise TBN consecutive B rows
+        const int n0 = swiglu ? tn * (TBN / 2) : tn * TBN;
         if (IO == 3 && B_MN == 0) {  // my B rows have landed locally
           if (swiglu) {
             gate_rows(n0, min(n0 + 64, rows_b) - 1);
@@ -337,14 +350,17 @@ __global__ void __launch_bounds__(kThreads, 1)
             for (int j = 0; j < BM / 64; ++j)  // box {64 m, 64 k} → 8 KB each
               load(&tmap_a, sa + j * (BK * 128), m0 + j * 64, kb * BK);
           }
-          if (swiglu) {  // boxes {64 k, 64 n}: gate rows, then the matching up rows
+          if (swiglu && wide) {  // boxes {64 k, 128 n}: gate rows, then the matching up rows, each from its own FF-row map
+            load(&tmap_b, sb, kb * BK, n0);
+            load(&tmap_g, sb + 128 * 128, kb * BK, n0);
+          } else if (swiglu) {  // boxes {64 k, 64 n}: gate rows, then the matching up rows
             load(&tmap_b, sb, kb * BK, n0);
             load(&tmap_b, sb + 64 * 128, kb * BK, p.swiglu_ff + n0);
           } else if (B_MN == 0) {
-            load(&tmap_b, sb, kb * BK, n0);  // box {64 k, 128 n}
+            load(&tmap_b, sb, kb * BK, n0);  // box {64 k, TBN n}
           } else {
 #pragma unroll
-            for (int j = 0; j < BN / 64; ++j)
+            for (int j = 0; j < TBN / 64; ++j)
               load(&tmap_b, sb + j * (BK * 128), n0 + j * 64, kb * BK);
           }
           if (++stage == kStages) stage = 0, phase ^= 1;
@@ -436,18 +452,19 @@ __global__ void __launch_bounds__(kThreads, 1)
     }
   } else if (warp >= 4) {
     // ------------------------------------------------------------------ consumers: wgmma main loop + epilogue
+    if constexpr (wide) setmaxnreg_inc<232>();
     const int wg = (warp - 4) >> 2;  // rows [wg*64, wg*64 + 64) of the tile
     const int wi = warp & 3;         // warp inside the warpgroup: accumulator rows wi*16 + lane/4 (+8)
     int stage = 0;
     uint32_t phase = 0;
-    float acc[64];
+    float acc[TBN / 2];
     for (int it = 0, tile; (tile = next_tile(it)) >= 0;) {
       int tm, tn, kind;
       coords(tile, tm, tn, kind);
       const int kb0 = (tile % split_k) * kb_per, kb1 = min(num_kb, kb0 + kb_per);
       if (kb0 >= kb1) continue;  // empty K slice
 #pragma unroll
-      for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+      for (int i = 0; i < TBN / 2; ++i) acc[i] = 0.f;
       int prev = -1;
       for (int kb = kb0; kb < kb1; ++kb) {
         mbar_wait(&full_bar[stage], phase);
@@ -459,7 +476,8 @@ __global__ void __launch_bounds__(kThreads, 1)
           // K-major: +32 B per k16 step inside the 128 B swizzle row.  MN-major: +16 k-rows * 128 B.
           const uint64_t adesc = A_MN == 0 ? make_smem_desc(sa + k * 32, 16, 1024) : make_smem_desc(sa + k * 2048, BK * 128, 1024);
           const uint64_t bdesc = B_MN == 0 ? make_smem_desc(sb + k * 32, 16, 1024) : make_smem_desc(sb + k * 2048, BK * 128, 1024);
-          wgmma_m64n128k16<A_MN, B_MN>(acc, adesc, bdesc);
+          if constexpr (wide) wgmma_m64n256k16<A_MN, B_MN>(acc, adesc, bdesc);
+          else wgmma_m64n128k16<A_MN, B_MN>(acc, adesc, bdesc);
         }
         wgmma_commit();
         wgmma_wait<1>();  // the previous k-block's wgmmas have retired: its ring slot may be refilled
@@ -477,15 +495,17 @@ __global__ void __launch_bounds__(kThreads, 1)
         const int FF = p.swiglu_ff;
         __nv_bfloat16* gu = reinterpret_cast<__nv_bfloat16*>(p.C);
         __nv_bfloat16* hp = reinterpret_cast<__nv_bfloat16*>(p.H);
+        constexpr int kFeat8 = TBN / 16;  // 8-feature column groups of the gate half; the up half follows
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const int f = tn * 64 + 8 * j + cq;
+        for (int j = 0; j < kFeat8; ++j) {
+          const int f = tn * (TBN / 2) + 8 * j + cq;
+          if (wide && f >= FF) continue;  // FF % 128 = 64: the last wide tile's gate and up halves are half zero-filled
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
             const int r = r0 + 8 * h;
             if (r >= p.M) continue;
             const uint32_t gw = bf16x2_bits(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
-            const uint32_t uw = bf16x2_bits(acc[4 * (j + 8) + 2 * h], acc[4 * (j + 8) + 2 * h + 1]);
+            const uint32_t uw = bf16x2_bits(acc[4 * (j + kFeat8) + 2 * h], acc[4 * (j + kFeat8) + 2 * h + 1]);
             // h = silu(gate)·up from the bf16-ROUNDED gate/up — bit-compatible with the stand-alone kernel that reads them back
             const float2 gf = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&gw));
             const float2 uf = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&uw));
@@ -500,8 +520,8 @@ __global__ void __launch_bounds__(kThreads, 1)
         const __nv_bfloat16* gu = reinterpret_cast<const __nv_bfloat16*>(p.aux);
         __nv_bfloat16* dgu = reinterpret_cast<__nv_bfloat16*>(p.C);
 #pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          const int f = tn * BN + 8 * j + cq;
+        for (int j = 0; j < TBN / 8; ++j) {
+          const int f = tn * TBN + 8 * j + cq;
           if (f >= FF) continue;
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
@@ -523,8 +543,8 @@ __global__ void __launch_bounds__(kThreads, 1)
         }
       } else {
 #pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          const int c = tn * BN + 8 * j + cq;
+        for (int j = 0; j < TBN / 8; ++j) {
+          const int c = tn * TBN + 8 * j + cq;
           if (c >= p.N) continue;  // N is even: c < N ⇒ c + 1 < N
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
@@ -595,62 +615,99 @@ int g_split_k_mode = -1;  // -1 auto, 0/1 off, n>1 forced
 
 const GemmEpilogue kPlain = {};
 
-template <int A_MN, int B_MN, int EPI, int IO>
+template <int A_MN, int B_MN, int EPI, int IO, int TBN>
 int launch(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, cudaStream_t stream, const PeerMaps* pmp,
            const CUtensorMap* tgp, const CUtensorMap* tg2p) {
   static const PeerMaps kNoPeers = {};
   const PeerMaps& pm = pmp ? *pmp : kNoPeers;
   const CUtensorMap& tg = tgp ? *tgp : ta;
   const CUtensorMap& tg2 = tg2p ? *tg2p : tg;
-  using G = Geo<IO>;
+  using G = Geo<IO, TBN>;
   static bool configured = false;
   if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_bf16_kernel<A_MN, B_MN, EPI, IO>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    cudaError_t e = cudaFuncSetAttribute(gemm_bf16_kernel<A_MN, B_MN, EPI, IO, TBN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          (int)G::kSmemBytes);
     if (e != cudaSuccess) return (int)e;
     configured = true;
   }
   if (g_num_sms == 0) g_num_sms = pbhost::num_sms();
   int grid = g_num_sms;
-  const int tiles_n = EPI == 2 ? p.swiglu_ff / 64 : (p.N + BN - 1) / BN;
+  const int tiles_n = EPI == 2 ? (p.swiglu_ff + TBN / 2 - 1) / (TBN / 2) : (p.N + TBN - 1) / TBN;
   const int tiles = ((p.M + BM - 1) / BM) * tiles_n * p.split_k;
   // IO = 1 / 3 need every CTA resident at once (tiles wait on flags other CTAs publish): the grid never exceeds the SM count
   if (tiles < grid) grid = tiles;
-  gemm_bf16_kernel<A_MN, B_MN, EPI, IO><<<grid, kThreads, G::kSmemBytes, stream>>>(ta, tb, tg, tg2, p, pm);
+  gemm_bf16_kernel<A_MN, B_MN, EPI, IO, TBN><<<grid, kThreads, G::kSmemBytes, stream>>>(ta, tb, tg, tg2, p, pm);
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? 0 : (int)e;
 }
 
-constexpr int variant(int io, int epi, int a_mn, int b_mn) { return io << 4 | epi << 2 | a_mn << 1 | b_mn; }
+constexpr int variant(int io, int epi, int a_mn, int b_mn, int wide) { return wide << 6 | io << 4 | epi << 2 | a_mn << 1 | b_mn; }
 
-// (I/O mode, epilogue, operand layouts) → kernel. These 16 instantiations are all the entry points accept: every layout for the
-// plain local GEMM, RoPE / SwiGLU on K-major B, SwiGLU backward on MN-major B, and K-major A for the collective modes.
+// (I/O mode, epilogue, operand layouts, tile width) → kernel. These 23 instantiations are all the entry points accept: every
+// layout for the plain local GEMM, RoPE / SwiGLU on K-major B, SwiGLU backward on MN-major B, each in both tile widths, and
+// K-major A for the collective modes (narrow tiles only).
 int dispatch(int io, int epi, const GemmParams& p, const CUtensorMap& ta, const CUtensorMap& tb, cudaStream_t stream,
-             const PeerMaps* pm = nullptr, const CUtensorMap* tg = nullptr, const CUtensorMap* tg2 = nullptr) {
-  switch (variant(io, epi, p.a_mn, p.b_mn)) {
-#define PB_GEMM_VARIANT(IO, EPI, A_MN, B_MN) \
-  case variant(IO, EPI, A_MN, B_MN):         \
-    return launch<A_MN, B_MN, EPI, IO>(ta, tb, p, stream, pm, tg, tg2);
-    PB_GEMM_VARIANT(0, 0, 0, 0)
-    PB_GEMM_VARIANT(0, 0, 0, 1)
-    PB_GEMM_VARIANT(0, 0, 1, 0)
-    PB_GEMM_VARIANT(0, 0, 1, 1)
-    PB_GEMM_VARIANT(0, 1, 0, 0)
-    PB_GEMM_VARIANT(0, 2, 0, 0)
-    PB_GEMM_VARIANT(0, 3, 0, 1)
-    PB_GEMM_VARIANT(1, 0, 0, 0)
-    PB_GEMM_VARIANT(1, 0, 0, 1)
-    PB_GEMM_VARIANT(2, 0, 0, 0)
-    PB_GEMM_VARIANT(2, 0, 0, 1)
-    PB_GEMM_VARIANT(3, 0, 0, 0)
-    PB_GEMM_VARIANT(3, 0, 0, 1)
-    PB_GEMM_VARIANT(3, 1, 0, 0)
-    PB_GEMM_VARIANT(3, 2, 0, 0)
-    PB_GEMM_VARIANT(3, 3, 0, 1)
+             const PeerMaps* pm = nullptr, const CUtensorMap* tg = nullptr, const CUtensorMap* tg2 = nullptr, bool wide = false) {
+  switch (variant(io, epi, p.a_mn, p.b_mn, wide)) {
+#define PB_GEMM_VARIANT(IO, EPI, A_MN, B_MN, TBN)         \
+  case variant(IO, EPI, A_MN, B_MN, TBN == kWideBN):      \
+    return launch<A_MN, B_MN, EPI, IO, TBN>(ta, tb, p, stream, pm, tg, tg2);
+    PB_GEMM_VARIANT(0, 0, 0, 0, BN)
+    PB_GEMM_VARIANT(0, 0, 0, 1, BN)
+    PB_GEMM_VARIANT(0, 0, 1, 0, BN)
+    PB_GEMM_VARIANT(0, 0, 1, 1, BN)
+    PB_GEMM_VARIANT(0, 1, 0, 0, BN)
+    PB_GEMM_VARIANT(0, 2, 0, 0, BN)
+    PB_GEMM_VARIANT(0, 3, 0, 1, BN)
+    PB_GEMM_VARIANT(0, 0, 0, 0, kWideBN)
+    PB_GEMM_VARIANT(0, 0, 0, 1, kWideBN)
+    PB_GEMM_VARIANT(0, 0, 1, 0, kWideBN)
+    PB_GEMM_VARIANT(0, 0, 1, 1, kWideBN)
+    PB_GEMM_VARIANT(0, 1, 0, 0, kWideBN)
+    PB_GEMM_VARIANT(0, 2, 0, 0, kWideBN)
+    PB_GEMM_VARIANT(0, 3, 0, 1, kWideBN)
+    PB_GEMM_VARIANT(1, 0, 0, 0, BN)
+    PB_GEMM_VARIANT(1, 0, 0, 1, BN)
+    PB_GEMM_VARIANT(2, 0, 0, 0, BN)
+    PB_GEMM_VARIANT(2, 0, 0, 1, BN)
+    PB_GEMM_VARIANT(3, 0, 0, 0, BN)
+    PB_GEMM_VARIANT(3, 0, 0, 1, BN)
+    PB_GEMM_VARIANT(3, 1, 0, 0, BN)
+    PB_GEMM_VARIANT(3, 2, 0, 0, BN)
+    PB_GEMM_VARIANT(3, 3, 0, 1, BN)
 #undef PB_GEMM_VARIANT
     default:
       return -7;
   }
+}
+
+int g_tile_mode = -1;  // -1 automatic (tile_policy), BN or kWideBN forced
+
+// Split-K slices of an fp32 reduce-add output under the current split mode, for a grid of `tiles` output tiles.
+int split_for(int tiles, int num_kb) {
+  if (g_split_k_mode == 0 || g_split_k_mode == 1) return 1;
+  if (g_split_k_mode > 1) return num_kb / g_split_k_mode >= 1 ? g_split_k_mode : 1;
+  if (g_num_sms == 0) g_num_sms = pbhost::num_sms();
+  return choose_split_k(tiles, g_num_sms > 0 ? g_num_sms : 1, num_kb);
+}
+
+// Tile width of a local GEMM, from the shape alone. A wide tile does the work of two narrow ones per pass over its k-blocks and
+// brings 48 KB per k-block instead of 2 x 32 KB, so it runs kWideGainPct % more FLOP per unit of time. The persistent grid runs
+// ceil(tiles / SMs) rounds of equal tiles; the wide tile is taken when its rounds, each twice as long, net of that gain, take no
+// longer than the narrow rounds. Narrow stays for M <= 128 (one row of tiles: the decode-step GEMMs), and for fp32 reduce-add
+// outputs that split K under either width (a split sums through atomics, so a different width would change the result).
+constexpr int kWideGainPct = 10;
+int tile_policy(int M, int N, int K, int epi, int c_fp32, int accumulate, int units) {
+  if (M <= BM) return BN;
+  const int tm = (M + BM - 1) / BM;
+  const int t128 = tm * (epi == 2 ? (N / 2 + 63) / 64 : (N + BN - 1) / BN);
+  const int t256 = tm * (epi == 2 ? (N / 2 + 127) / 128 : (N + kWideBN - 1) / kWideBN);
+  if (c_fp32 && accumulate) {
+    const int num_kb = (K + BK - 1) / BK;
+    if (choose_split_k(t128, units, num_kb) > 1 || choose_split_k(t256, units, num_kb) > 1) return BN;
+  }
+  const int r128 = (t128 + units - 1) / units, r256 = (t256 + units - 1) / units;
+  return 2 * r256 * 100 <= r128 * (100 + kWideGainPct) ? kWideBN : BN;
 }
 
 // Argument rules of the fused epilogues, for both entry points; N is the N of the product A·Bᵀ (2·FF for SwiGLU, FF for SwiGLU
@@ -713,6 +770,20 @@ PB_EXPORT int pb_gemm_set_split_k(int mode) {
   return old;
 }
 
+// Tile width of pb_gemm_bf16: -1 = automatic (default, tile_policy), 128 or 256 = always that width (testing). Returns the old
+// mode; -9 and no change for any other value.
+PB_EXPORT int pb_gemm_set_tile(int mode) {
+  if (mode != -1 && mode != BN && mode != kWideBN) return -9;
+  const int old = g_tile_mode;
+  g_tile_mode = mode;
+  return old;
+}
+
+// The tile width (128 | 256) the automatic policy gives pb_gemm_bf16 for this shape on a GPU with `num_sms` SMs; host only.
+PB_EXPORT int pb_gemm_tile_policy(int M, int N, int K, int epi_kind, int c_fp32, int accumulate, int num_sms) {
+  return tile_policy(M, N, K, epi_kind, c_fp32, accumulate, num_sms > 0 ? num_sms : 1);
+}
+
 // C[M, N] (bf16 | fp32, += with `accumulate`) = A·Bᵀ, optionally with a fused epilogue (null `epi` = plain).
 // lda/ldb: row stride (elements) of the matrix AS STORED (see header comment).
 //   RoPE:            y = x·Wᵀ with the Q/K head columns rotated (the fused QKV projection)
@@ -727,18 +798,22 @@ PB_EXPORT int pb_gemm_bf16(const void* A, const void* B, void* C, int M, int N, 
   if (M <= 0 || N <= 0 || K <= 0) return 0;
   if ((lda % 8) || (ldb % 8) || (ldc % (c_fp32 ? 4 : 8))) return -1;
   if ((reinterpret_cast<uintptr_t>(A) | reinterpret_cast<uintptr_t>(B) | reinterpret_cast<uintptr_t>(C)) & 15) return -2;
-  CUtensorMap ta, tb;
+  if (g_num_sms == 0) g_num_sms = pbhost::num_sms();
+  const int tbn = g_tile_mode > 0 ? g_tile_mode : tile_policy(M, N, K, e.kind, c_fp32, accumulate, g_num_sms > 0 ? g_num_sms : 1);
+  const bool wide = tbn == kWideBN;
+  CUtensorMap ta, tb, tup;
   if ((rc = operand_tmap(&ta, A, M, K, lda, a_mn_major, BM))) return rc;
-  if ((rc = operand_tmap(&tb, B, N, K, ldb, b_mn_major, e.kind == 2 ? 64 : BN))) return rc;
-  GemmParams p = make_params(C, M, N, K, ldc, a_mn_major, b_mn_major, c_fp32, accumulate, e);
-  if (c_fp32 && accumulate && g_split_k_mode != 0 && g_split_k_mode != 1) {
-    if (g_num_sms == 0) g_num_sms = pbhost::num_sms();
-    const int units = g_num_sms > 0 ? g_num_sms : 1;
-    const int tiles = ((M + BM - 1) / BM) * ((N + BN - 1) / BN);
-    const int num_kb = (K + BK - 1) / BK;
-    p.split_k = g_split_k_mode > 1 ? (num_kb / g_split_k_mode >= 1 ? g_split_k_mode : 1) : choose_split_k(tiles, units, num_kb);
+  if (wide && e.kind == 2) {  // SwiGLU: the gate rows and the up rows of W13 as two maps of FF rows each
+    const int FF = N / 2;
+    if ((rc = pbhost::cached_tmap(&tb, B, (uint64_t)FF, (uint64_t)K, (uint64_t)ldb, BK, 128))) return rc;
+    const void* up = static_cast<const __nv_bfloat16*>(B) + (int64_t)FF * ldb;
+    if ((rc = pbhost::cached_tmap(&tup, up, (uint64_t)FF, (uint64_t)K, (uint64_t)ldb, BK, 128))) return rc;
+  } else if ((rc = operand_tmap(&tb, B, N, K, ldb, b_mn_major, e.kind == 2 ? 64 : tbn))) {
+    return rc;
   }
-  return dispatch(0, e.kind, p, ta, tb, stream);
+  GemmParams p = make_params(C, M, N, K, ldc, a_mn_major, b_mn_major, c_fp32, accumulate, e);
+  if (c_fp32 && accumulate) p.split_k = split_for(((M + BM - 1) / BM) * ((N + tbn - 1) / tbn), (K + BK - 1) / BK);  // plain only
+  return dispatch(0, e.kind, p, ta, tb, stream, nullptr, wide && e.kind == 2 ? &tup : nullptr, nullptr, wide);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------------

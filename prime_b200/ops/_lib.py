@@ -154,6 +154,8 @@ def _sigs() -> dict:
         "pb_quantize_mxfp8": [vp, i64, vp, vp, i32, i32, i32, vp],
         "pb_gemm_mxfp8": [vp, vp, vp, vp, vp, i32, i32, i32, i32, vp],
         "pb_gemm_set_split_k": [i32],
+        "pb_gemm_set_tile": [i32],
+        "pb_gemm_tile_policy": [i32, i32, i32, i32, i32, i32, i32],
         "pb_flash_attn_fwd": [vp, vp, vp, vp, i32, i32, i32, i32, i32, f32, i32, vp],
         "pb_flash_attn_bwd": [vp, vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, f32, i32, vp, vp, vp],
         "pb_doc_bounds": [vp, i32, i32, i64, i32, vp, vp, vp],

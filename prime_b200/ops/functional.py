@@ -121,6 +121,22 @@ def set_gemm_split_k(mode: int) -> int:
     return int(_lib.load().pb_gemm_set_split_k(int(mode)))
 
 
+GEMM_TILE_MODES = (128, 256)  # tile widths of the local GEMM (128 x 128 and 128 x 256 tiles)
+
+
+def set_gemm_tile(mode: int) -> int:
+    """Tile width of :func:`gemm`: -1 automatic (the shape policy), 128 or 256 forced (testing). Returns the old mode."""
+    if mode != -1 and mode not in GEMM_TILE_MODES:
+        raise ValueError(f"GEMM tile mode must be -1 or one of {GEMM_TILE_MODES}, got {mode}")
+    return int(_lib.load().pb_gemm_set_tile(int(mode)))
+
+
+def gemm_tile_policy(M: int, N: int, K: int, *, epilogue: int = 0, c_fp32: bool = False, accumulate: bool = False, num_sms: int = 132) -> int:
+    """The tile width (128 | 256) the automatic policy picks for C[M, N] = A·Bᵀ with contraction K; ``epilogue`` is the
+    ``GemmEpilogue`` kind (2: SwiGLU, N = 2·FF). Host-side only: needs the library, not a GPU."""
+    return int(_lib.load().pb_gemm_tile_policy(M, N, K, epilogue, int(c_fp32), int(accumulate), num_sms))
+
+
 def _take_fresh(param: torch.Tensor) -> bool:
     """True exactly once per optimizer step and parameter (the sharded engine arms ``_mg_fresh`` in ``zero_grad``): the first
     gradient write of the step OVERWRITES main_grad, which is what lets the engine skip the 4·N-byte memset."""

@@ -24,4 +24,7 @@ run memcheck  "gpu and (kv_append or decode_advance or graph_replay or generate_
 # flash attention against fp64: every instantiation, tile-edge documents and windows, probes (S >= 4096 is left to the plain run)
 run memcheck  "gpu and not S4096 and not S8192 and not 32768" memcheck_attention_fp64 tests/test_attention_fp64_gpu.py
 run racecheck "gpu and not S4096 and not S8192 and not 32768 and not doc_bounds" racecheck_attention_fp64 tests/test_attention_fp64_gpu.py
+# bf16 GEMM in both tile widths (128 x 128 and the 128 x 256 setmaxnreg tile): every layout and epilogue at the small edge shapes
+run memcheck  "gpu and not 5632" memcheck_gemm_wide tests/test_gemm_wide_gpu.py
+run racecheck "gpu and not 5632" racecheck_gemm_wide tests/test_gemm_wide_gpu.py
 cat gpurun_out/sanitizer_summary.txt
