@@ -36,6 +36,8 @@ import numpy as np
 import torch
 import torch.distributed as dist
 
+from .parallel.layout import plan_layout, use_zero3
+
 MAGIC = b"PBCK0001"
 _NP = {torch.float32: np.float32, torch.int8: np.int8, torch.int64: np.int64, torch.uint8: np.uint8, torch.float16: np.float16,
        torch.int32: np.int32, torch.bfloat16: np.uint16}  # fmt: skip
@@ -320,7 +322,7 @@ def trainer_state(trainer) -> tuple[dict[str, torch.Tensor], dict[str, Any]]:
     tensors = {"master": eng.master, "exp_avg": eng.exp_avg, "exp_avg_sq": eng.exp_avg_sq}
     extra: dict[str, Any] = {
         "trainer_step": trainer.step_count, "engine_step": eng.step_count, "fsdp_size": eng.F, "fsdp_rank": eng.mesh.fsdp_rank,
-        "layout": [[b.name, b.start, b.size, b.shard_start, b.shard_size] for b in eng.buckets],
+        "layout": eng.layout.signature,
         "data": trainer.loader.state_dict(),
         "shard_params": bool(getattr(eng, "shard_params", False)),
     }  # fmt: skip
@@ -335,9 +337,7 @@ def trainer_state(trainer) -> tuple[dict[str, torch.Tensor], dict[str, Any]]:
 
 def restore_trainer(trainer, tensors: dict[str, torch.Tensor], extra: dict[str, Any], *, skip_dataloader: bool = False) -> None:
     eng, outer = trainer.engine, trainer.outer
-    layout = [[b.name, b.start, b.size, b.shard_start, b.shard_size] for b in eng.buckets]
-    if extra["layout"] != layout or extra["fsdp_size"] != eng.F:
-        raise ValueError("checkpoint shard layout does not match this model/mesh")
+    eng.layout.check_saved(extra["layout"], extra["fsdp_size"], extra.get("shard_params", False))
     with torch.no_grad():
         eng.master.copy_(tensors["master"])
         eng.exp_avg.copy_(tensors["exp_avg"])
@@ -367,52 +367,6 @@ def restore_trainer(trainer, tensors: dict[str, torch.Tensor], extra: dict[str, 
 SHARDED_KINDS = ("master", "exp_avg", "exp_avg_sq", "theta0", "momentum")  # per-rank 1/F slices of parameter-shaped state
 
 
-def _layout_plan(model, fsdp_size: int, shard_params: bool):
-    """The engine's own bucket planner without buffers, hooks or a process group: one source of truth for who holds what."""
-    from .parallel.fsdp import ShardedEngine
-
-    plan = ShardedEngine.__new__(ShardedEngine)
-    plan.model, plan.F, plan.shard_params = model, int(fsdp_size), bool(shard_params)
-    plan._build_buckets()
-    return plan
-
-
-def _plan_layout(plan) -> list[list]:
-    return [[b.name, b.start, b.size, b.shard_start, b.shard_size] for b in plan.buckets]
-
-
-def _gather_params(plan, shards: dict[int, torch.Tensor]) -> dict[str, torch.Tensor]:
-    """Per-rank flat shards of one kind of state → {qualified parameter name: full tensor in the parameter's shape}."""
-    F, out = plan.F, {}
-    for b in plan.buckets:
-        if b.kind == "rows":
-            for (qn, p, _), (soff, piece) in zip(b.params, b.pieces):
-                rows, cols = p.shape
-                out[qn] = torch.cat([shards[r][b.shard_start + soff : b.shard_start + soff + piece].view(rows // F, cols) for r in range(F)], dim=0)
-        else:
-            full = torch.cat([shards[r][b.shard_start : b.shard_start + b.shard_size] for r in range(F)])
-            for qn, p, off in b.params:
-                out[qn] = full[off : off + p.numel()].view(p.shape)
-    return out
-
-
-def _scatter_params(plan, full: dict[str, torch.Tensor], rank: int, dtype: torch.dtype = torch.float32) -> torch.Tensor:
-    """Inverse of :func:`_gather_params` for one rank of the target layout (padding stays zero)."""
-    F = plan.F
-    shard = torch.zeros(plan.shard_total, dtype=dtype)
-    for b in plan.buckets:
-        if b.kind == "rows":
-            for (qn, p, _), (soff, piece) in zip(b.params, b.pieces):
-                rpr = p.shape[0] // F
-                shard[b.shard_start + soff : b.shard_start + soff + piece] = full[qn][rank * rpr : (rank + 1) * rpr].reshape(-1)
-        else:
-            flat = torch.zeros(b.size, dtype=dtype)
-            for qn, p, off in b.params:
-                flat[off : off + p.numel()] = full[qn].reshape(-1)
-            shard[b.shard_start : b.shard_start + b.shard_size] = flat[rank * b.shard_size : (rank + 1) * b.shard_size]
-    return shard
-
-
 def _read_all_ranks(d: Path) -> tuple[dict, list[tuple[dict[str, torch.Tensor], dict[str, Any]]]]:
     meta = json.loads((d / "meta.json").read_text())
     return meta, [read_shard(d / f"rank_{r:05d}.pbck", "cpu") for r in range(int(meta["world_size"]))]
@@ -421,7 +375,7 @@ def _read_all_ranks(d: Path) -> tuple[dict, list[tuple[dict[str, torch.Tensor], 
 def assemble_full_model(path: str | Path, name_model: str, type_model: str = "llama2", *, dtype: torch.dtype = torch.float32, **overrides):
     """Rebuild the complete model on the CPU from a published checkpoint step directory: every ``rank_*.pbck`` holds its rank's
     1/F slice of the fp32 master weights, cut either as contiguous bucket slices (replicated-parameter mode) or as one row block
-    per weight (ZeRO-3). The layout is recomputed with the engine's own planner, so there is one source of truth.
+    per weight (ZeRO-3). The layout is recomputed with the engine's own planner (``parallel/layout.py``).
     Used by ``python -m prime_b200.models.hf export`` and ``examples/inspect_checkpoint.py``; DiLoCo workers are identical after
     an outer step, the first worker's shards are taken. The sliding window is taken from the run's recorded config (the bucket
     layout does not depend on it), so a windowed model is never rebuilt with full attention."""
@@ -445,10 +399,10 @@ def assemble_full_model(path: str | Path, name_model: str, type_model: str = "ll
     if sorted(shards) != list(range(F)):
         raise ValueError(f"checkpoint {d} is incomplete: have fsdp ranks {sorted(shards)} of {F}")
     model = build_model(name_model, type_model, dtype=dtype, seed=None, **overrides)
-    plan = _layout_plan(model, F, bool(extra0.get("shard_params", False)))
-    if _plan_layout(plan) != [list(x) for x in extra0["layout"]]:
+    layout = plan_layout(model, F, bool(extra0.get("shard_params", False)))
+    if not layout.matches(extra0["layout"]):
         raise ValueError(f"checkpoint {d} was written for a different model than {type_model}/{name_model} (bucket layout differs)")
-    full = _gather_params(plan, shards)
+    full = layout.gather(shards)
     with torch.no_grad():
         for qn, p in model.named_parameters():
             p.copy_(full[qn])
@@ -475,10 +429,10 @@ def reshard_checkpoint(src: str | Path, dst: str | Path, name_model: str, type_m
         raise ValueError(f"{src}: {world0} rank files do not divide into groups of fsdp_size={F0}")
     workers = world0 // F0
     sp0 = bool(ranks[0][1].get("shard_params", False))
-    sp1 = (sp0 if shard_params is None else bool(shard_params)) and int(fsdp_size) > 1  # a single rank holds whole parameters
-    model = build_model(name_model, type_model, dtype=torch.float32, seed=None, **overrides)
-    plan0, plan1 = _layout_plan(model, F0, sp0), _layout_plan(model, fsdp_size, sp1)
-    if _plan_layout(plan0) != [list(x) for x in ranks[0][1]["layout"]]:
+    sp1 = use_zero3(sp0 if shard_params is None else shard_params, fused=True, fsdp_size=int(fsdp_size))
+    model = build_model(name_model, type_model, device="meta", dtype=torch.float32, seed=None, **overrides)  # shapes only
+    plan0, plan1 = plan_layout(model, F0, sp0), plan_layout(model, fsdp_size, sp1)
+    if not plan0.matches(ranks[0][1]["layout"]):
         raise ValueError(f"checkpoint {src} was written for a different model than {type_model}/{name_model} (bucket layout differs)")
     tmp = dst.parent / f".tmp-{dst.name}"
     if tmp.exists():
@@ -492,11 +446,11 @@ def reshard_checkpoint(src: str | Path, dst: str | Path, name_model: str, type_m
         by_rank = {int(e["fsdp_rank"]): t for t, e in group}
         first_t, first_e = group[0]
         kinds = [k for k in SHARDED_KINDS if k in first_t]
-        whole = {k: _gather_params(plan0, {r: by_rank[r][k].float() for r in range(F0)}) for k in kinds}
+        whole = {k: plan0.gather({r: by_rank[r][k].float() for r in range(F0)}) for k in kinds}
         data_states = [e.get("data") for _, e in group]
         furthest = max((d.get("cursor", d.get("n_served", 0)) for d in data_states if isinstance(d, dict)), default=None)
         for r in range(fsdp_size):
-            tensors = {k: _scatter_params(plan1, whole[k], r) for k in kinds}
+            tensors = {k: plan1.scatter(whole[k], r) for k in kinds}
             for k, v in first_t.items():  # RNG state and anything else that is not parameter-shaped: the worker's first rank's
                 if k not in tensors:
                     tensors[k] = v
@@ -505,7 +459,7 @@ def reshard_checkpoint(src: str | Path, dst: str | Path, name_model: str, type_m
             data = data_states[r] if r < F0 else None
             if isinstance(data_states[0], dict) and "cursor" in data_states[0]:
                 data = {**data_states[0], "cursor": furthest}
-            extra = {**first_e, "fsdp_size": int(fsdp_size), "fsdp_rank": r, "layout": _plan_layout(plan1), "shard_params": sp1, "data": data,
+            extra = {**first_e, "fsdp_size": int(fsdp_size), "fsdp_rank": r, "layout": plan1.signature, "shard_params": sp1, "data": data,
                      "resharded_from": {"fsdp_size": F0, "shard_params": sp0, "path": str(src)}}  # fmt: skip
             written += write_shard(tmp / f"rank_{w * fsdp_size + r:05d}.pbck", tensors, extra)
     new_meta = {**meta, "world_size": workers * fsdp_size, "mesh": f"dl{workers}xfsdp{fsdp_size}",

@@ -25,7 +25,8 @@ import torch.distributed as dist
 
 from ..ops import _lib, reference
 from ..ops.functional import _count
-from .fsdp import SHARD_ALIGN, ShardedEngine
+from .fsdp import ShardedEngine
+from .layout import SHARD_ALIGN
 
 
 @dataclass

@@ -33,7 +33,6 @@ from __future__ import annotations
 
 import ctypes
 from dataclasses import dataclass, field
-from typing import Iterable
 
 import torch
 import torch.distributed as dist
@@ -41,26 +40,9 @@ import torch.nn as nn
 
 from ..ops import _lib, reference
 from ..ops.functional import _count
+from .layout import Bucket, plan_layout, use_zero3
 from .mesh import Mesh
 from .symm import SymmetricHeap
-
-SHARD_ALIGN = 1024  # elements; also the int8 quantisation block of the outer step
-
-
-@dataclass
-class Bucket:
-    name: str
-    params: list[tuple[str, nn.Parameter, int]]  # (qualified name, param, offset inside bucket)
-    start: int = 0  # offset in the flat buffers
-    size: int = 0  # padded element count (multiple of F * SHARD_ALIGN)
-    shard_start: int = 0  # offset in this rank's shard buffers
-    shard_size: int = 0
-    ready: bool = False
-    work: object = None  # async collective handle (collective backend)
-    kind: str = "flat"  # "flat": the shard is the r-th contiguous 1/F slice of the bucket; "rows": one row block per parameter
-    pieces: list = field(default_factory=list)  # rows kind: per parameter (offset inside the bucket's shard, elements)
-    pstart: int = 0  # flat kind: offset of the bucket in ``param_flat``
-    segs: object = None  # rows kind: cached SegTable of this rank's pieces inside ``grad_flat``
 
 
 @dataclass
@@ -132,8 +114,7 @@ class ShardedEngine:
         if backend == "fused" and (heap is None or self.device.type != "cuda"):
             raise ValueError("fused backend needs CUDA and a SymmetricHeap")
         self.backend, self.heap, self.overlap, self.reduce_ctas = backend, heap, overlap, reduce_ctas
-        # ZeRO-3 needs peers to read each other's shards from inside the GEMMs: fused backend, F > 1
-        self.shard_params = bool(shard_params) and backend == "fused" and self.F > 1
+        self.shard_params = use_zero3(bool(shard_params), fused=backend == "fused", fsdp_size=self.F)
         self.master_in_heap = bool(master_in_heap) and backend == "fused"
         # first weight-gradient write of a step overwrites (GEMM epilogue with accumulate=false) instead of adding into a buffer that
         # a 4·N-byte memset had to clear first; off while a CUDA graph is captured/replayed (the accumulate flag is baked in there)
@@ -153,94 +134,21 @@ class ShardedEngine:
         from ..ops.functional import reset_gather_cache
 
         reset_gather_cache()
-        self._build_buckets()
+        self.layout = plan_layout(model, self.F, self.shard_params)
+        self.buckets, self.total, self.shard_total = self.layout.buckets, self.layout.total, self.layout.shard_total
+        self.bucket_index = {b.name: i for i, b in enumerate(self.buckets)}
+        self._ready = [False] * len(self.buckets)
+        self._work: list = [None] * len(self.buckets)  # async collective handles (collective backend)
+        self._segs: list = [None] * len(self.buckets)  # rows kind: SegTable of this rank's pieces inside ``grad_flat``
         self._allocate()
         self._install_hooks()
 
-    # ------------------------------------------------------------------ layout
-    def _stages(self) -> list[tuple[str, list[tuple[str, nn.Parameter]]]]:
-        m = self.model
-        named = dict(m.named_parameters())
-        used: set[str] = set()
-        stages: list[tuple[str, list[tuple[str, nn.Parameter]]]] = []
-
-        def take(prefix_list: Iterable[str], name: str):
-            items = [(k, v) for k, v in named.items() if any(k == p or k.startswith(p + ".") for p in prefix_list)]
-            used.update(k for k, _ in items)
-            stages.append((name, items))
-
-        if hasattr(m, "layers") and hasattr(m, "tok_embeddings"):
-            take(["tok_embeddings"], "embed")
-            for i in range(len(m.layers)):
-                take([f"layers.{i}"], f"layer{i}")
-            take(["norm", "output"], "head")
-        rest = [(k, v) for k, v in named.items() if k not in used]
-        if rest:
-            stages.append(("rest", rest))
-        return [s for s in stages if s[1]]
-
-    def _row_shardable(self, p: nn.Parameter) -> bool:
-        return p.dim() == 2 and p.shape[0] % self.F == 0 and p.shape[1] % 64 == 0 and (p.numel() // self.F) % 8 == 0
-
-    def _build_buckets(self) -> None:
-        gran = self.F * SHARD_ALIGN
-        self.buckets: list[Bucket] = []
-        flat_off = shard_off = pflat_off = 0
-        stages = self._stages()
-        small: list[tuple[str, nn.Parameter]] = []
-        if self.shard_params:
-            # every row-shardable 2-D weight goes to a "rows" bucket of its stage; the rest (norm gains, odd shapes) is
-            # collected into ONE replicated flat bucket at the end of the shard space
-            kept = []
-            for name, items in stages:
-                rows_items = [(k, v) for k, v in items if self._row_shardable(v)]
-                small += [(k, v) for k, v in items if not self._row_shardable(v)]
-                if rows_items:
-                    kept.append((name, rows_items, "rows"))
-            if small:
-                kept.append(("small", small, "flat"))
-            plan = kept
-        else:
-            plan = [(name, items, "flat") for name, items in stages]
-        for name, items, kind in plan:
-            off = 0
-            plist = []
-            for qn, p in items:
-                off = (off + 7) // 8 * 8  # 16-byte alignment of every bf16 parameter (TMA base address)
-                plist.append((qn, p, off))
-                off += p.numel()
-            size = (off + gran - 1) // gran * gran
-            if kind == "rows":
-                soff, pieces = 0, []
-                for _, p, _ in plist:
-                    piece = p.numel() // self.F
-                    pieces.append((soff, piece))
-                    soff += (piece + 7) // 8 * 8
-                ssize = (soff + SHARD_ALIGN - 1) // SHARD_ALIGN * SHARD_ALIGN
-                b = Bucket(name, plist, flat_off, size, shard_off, ssize, kind="rows", pieces=pieces)
-            else:
-                b = Bucket(name, plist, flat_off, size, shard_off, size // self.F, kind="flat", pstart=pflat_off)
-                pflat_off += size
-            self.buckets.append(b)
-            flat_off += size
-            shard_off += b.shard_size
-        self.total, self.shard_total, self.pflat_total = flat_off, shard_off, pflat_off
-        self.bucket_index = {b.name: i for i, b in enumerate(self.buckets)}
-
-    def heap_bytes_needed(self) -> int:
-        """Upper bound of what this engine allocates from the symmetric heap (the Trainer sizes the heap from it)."""
-        n = self.pflat_total * 2 + self.total * 4 + (4 << 20)
-        if self.shard_params:
-            n += self.shard_total * 2
-        if self.master_in_heap:
-            n += self.shard_total * 4
-        return n
-
+    # ------------------------------------------------------------------ buffers
     def _allocate(self) -> None:
         dev, F, r = self.device, self.F, self.mesh.fsdp_rank
         fused = self.backend == "fused"
         if fused:
-            self.param_flat = self.heap.alloc(max(self.pflat_total, 8), self.param_dtype)
+            self.param_flat = self.heap.alloc(max(self.layout.pflat_total, 8), self.param_dtype)
             self.grad_flat = self.heap.alloc(self.total, torch.float32)
             self.pshard = self.heap.alloc(self.shard_total, self.param_dtype) if self.shard_params else None
             self.slot_grad = self.heap.alloc_flags(len(self.buckets) * F)
@@ -252,7 +160,7 @@ class ShardedEngine:
             self.sumsq_partial = torch.zeros(self.lib_grid(), dtype=torch.float32, device=dev)
             self.gnorm_buf = torch.zeros(1, dtype=torch.float32, device=dev)
         else:
-            self.param_flat = torch.zeros(max(self.pflat_total, 8), dtype=self.param_dtype, device=dev)
+            self.param_flat = torch.zeros(max(self.layout.pflat_total, 8), dtype=self.param_dtype, device=dev)
             self.grad_flat = torch.zeros(self.total, dtype=torch.float32, device=dev)
             self.pshard = None
         self.param_flat.zero_()
@@ -274,17 +182,17 @@ class ShardedEngine:
             self._scratch = {k: torch.empty(v, dtype=self.param_dtype, device=dev) for k, v in by_stage.items()}
             self._gather_flags = torch.zeros(64, dtype=torch.int32, device=dev)
         with torch.no_grad():
-            for b in self.buckets:
+            for i, b in enumerate(self.buckets):
                 if b.kind == "rows":
-                    self._attach_rows_bucket(b)
+                    self._attach_rows_bucket(i, b)
                     continue
                 for _, p, off in b.params:
                     view = self.param_flat[b.pstart + off : b.pstart + off + p.numel()].view(p.shape)
                     view.copy_(p.data)
                     p.data = view
                     p.main_grad = self.grad_flat[b.start + off : b.start + off + p.numel()].view(p.shape)
-                s = b.pstart + r * b.shard_size
-                self.master[b.shard_start : b.shard_start + b.shard_size] = self.param_flat[s : s + b.shard_size].float()
+                for src, dst, n in b.owned(r):
+                    self.master[dst : dst + n] = self.param_flat[b.pstart + src : b.pstart + src + n].float()
         self.exp_avg = torch.zeros_like(self.master) if not self.master_in_heap else torch.zeros(self.shard_total, dtype=torch.float32, device=dev)
         self.exp_avg_sq = torch.zeros_like(self.exp_avg)
         # reduced gradient shard; with F == 1 the shard *is* the bucket, so alias instead of copying
@@ -310,19 +218,18 @@ class ShardedEngine:
             a.next_fwd = b
             b.next_bwd = a
 
-    def _attach_rows_bucket(self, b: Bucket) -> None:
+    def _attach_rows_bucket(self, bucket_id: int, b: Bucket) -> None:
         """ZeRO-3: copy this rank's row block of every weight into the shard buffer, then re-point the parameter at the shared
         gather scratch (embedding: at a stride-0 placeholder — its rows are only ever read through the peers' shards)."""
         F, r, heap = self.F, self.mesh.fsdp_rank, self.heap
         ranks = self.mesh.fsdp_ranks
         key = "layer" if b.name.startswith("layer") else b.name
         segs = []
-        for (qn, p, off), (soff, piece) in zip(b.params, b.pieces):
+        for (qn, p, off), (src, lo, piece) in zip(b.params, b.owned(r)):
             rows, cols = p.shape
             rpr = rows // F
-            lo = b.shard_start + soff
             shard = self.pshard[lo : lo + piece].view(rpr, cols)
-            shard.copy_(p.data[r * rpr : (r + 1) * rpr])
+            shard.view(-1).copy_(p.data.view(-1)[src - off : src - off + piece])
             self.master[lo : lo + piece] = shard.reshape(-1).float()
             if b.name == "embed":
                 full = torch.zeros(1, dtype=self.param_dtype, device=self.device).expand(rows, cols)
@@ -335,8 +242,8 @@ class ShardedEngine:
             p.main_grad = self.grad_flat[b.start + off : b.start + off + p.numel()].view(p.shape)
             p.z3 = RowShard(rows, cols, F, r, rpr, peers, full_ptr, self._gather_flags, shard, full=full if b.name != "embed" else None,
                             ver=self._pver)
-            segs.append((b.start + off + r * piece, lo, piece))
-        b.segs = _lib.SegTable.of(segs)
+            segs.append((b.start + src, lo, piece))
+        self._segs[bucket_id] = _lib.SegTable.of(segs)
 
     def lib_grid(self) -> int:
         return _lib.load().pb_grad_reduce_grid()
@@ -398,8 +305,8 @@ class ShardedEngine:
                         p._mg_fresh = True
         else:
             self.grad_flat.zero_()
-        for b in self.buckets:
-            b.ready, b.work = False, None
+        self._ready = [False] * len(self.buckets)
+        self._work = [None] * len(self.buckets)
 
     def set_micro_step(self, last: bool) -> None:
         """Tell the engine whether the coming backward is the last of the accumulation window."""
@@ -429,9 +336,9 @@ class ShardedEngine:
 
     def _on_bucket_ready(self, bucket_id: int) -> None:
         b = self.buckets[bucket_id]
-        if self.capture_mode or not self._last_micro or b.ready:
+        if self.capture_mode or not self._last_micro or self._ready[bucket_id]:
             return
-        b.ready = True
+        self._ready[bucket_id] = True
         self._fold_autograd_grads(b)
         self._settle_fresh(b)
         self._reduce_bucket(bucket_id)
@@ -455,7 +362,7 @@ class ShardedEngine:
                     wait_flags = self.heap.flags.data_ptr()
                 ctas = self.reduce_ctas if (F > 1 and self.overlap) else 0
                 if b.kind == "rows" and self._nvls:  # ZeRO-3 + NVLS: each parameter's row block is summed inside the switch
-                    segs = b.segs
+                    segs = self._segs[bucket_id]
                     for i in range(segs.nseg):
                         _lib.check(
                             self.lib.pb_mc_grad_reduce(
@@ -470,7 +377,7 @@ class ShardedEngine:
                 if b.kind == "rows":  # ZeRO-3 bucket: one row block per parameter
                     gp = self.heap.peers(ranks, self.grad_flat)
                     _lib.check(
-                        self.lib.pb_grad_reduce_segs(ctypes.byref(gp), ctypes.byref(b.segs), 1.0 / F, self.gshard.data_ptr(),
+                        self.lib.pb_grad_reduce_segs(ctypes.byref(gp), ctypes.byref(self._segs[bucket_id]), 1.0 / F, self.gshard.data_ptr(),
                                                      self.sumsq_partial.data_ptr(), wait_flags, slot_base, self._epoch,
                                                      self.heap.err.data_ptr(), ctas, s),
                         "pb_grad_reduce_segs",
@@ -506,7 +413,7 @@ class ShardedEngine:
         dst = self.gshard[b.shard_start : b.shard_start + b.shard_size]
         g = self.mesh.fsdp_group
         if dist.get_backend(g) == "nccl":
-            b.work = dist.reduce_scatter_tensor(dst, src, op=dist.ReduceOp.AVG, group=g, async_op=True)
+            self._work[bucket_id] = dist.reduce_scatter_tensor(dst, src, op=dist.ReduceOp.AVG, group=g, async_op=True)
         else:  # gloo has no reduce_scatter: all-reduce the bucket, keep my slice
             dist.all_reduce(src, group=g)
             dst.copy_(src[r * b.shard_size : (r + 1) * b.shard_size])
@@ -517,8 +424,8 @@ class ShardedEngine:
         if self.trace is not None:
             self.trace.mark("backward_end")
         for i, b in enumerate(self.buckets):
-            if not b.ready:
-                b.ready = True
+            if not self._ready[i]:
+                self._ready[i] = True
                 self._fold_autograd_grads(b)
                 self._settle_fresh(b)
                 self._reduce_bucket(i)
@@ -539,8 +446,8 @@ class ShardedEngine:
             self._step_fused(lr, bc1, bc2)
         else:
             self._step_collective(lr, bc1, bc2)
-        for b in self.buckets:
-            b.ready, b.work = False, None
+        self._ready = [False] * len(self.buckets)
+        self._work = [None] * len(self.buckets)
         self._pver[0] += 1
 
     def _param_dst(self, b: Bucket) -> tuple[_lib.PeerPtrs, int]:
@@ -613,9 +520,9 @@ class ShardedEngine:
     def _step_collective(self, lr: float, bc1: float, bc2: float) -> None:
         h, F, r = self.hyper, self.F, self.mesh.fsdp_rank
         g = self.mesh.fsdp_group
-        for b in self.buckets:
-            if b.work is not None:
-                b.work.wait()
+        for w in self._work:
+            if w is not None:
+                w.wait()
         gsh = self.gshard  # aliases grad_flat when F == 1 (identical layout)
         sumsq = gsh.pow(2).sum()
         if F > 1:
@@ -674,24 +581,14 @@ class ShardedEngine:
             "master": self.master,
             "exp_avg": self.exp_avg,
             "exp_avg_sq": self.exp_avg_sq,
-            "layout": [(b.name, b.start, b.size, b.shard_start, b.shard_size) for b in self.buckets],
+            "layout": self.layout.signature,
             "shard_params": self.shard_params,
             "fsdp_size": self.F,
             "fsdp_rank": self.mesh.fsdp_rank,
         }
 
     def load_state_dict(self, sd: dict) -> None:
-        if sd["fsdp_size"] != self.F:
-            raise ValueError(f"checkpoint was written with fsdp_size={sd['fsdp_size']}, engine has {self.F}")
-        if bool(sd.get("shard_params", False)) != self.shard_params:
-            # the two modes cut the optimizer shards differently (contiguous 1/F slices of a bucket vs one row block per weight)
-            raise ValueError(
-                f"checkpoint was written with train.reshard_after_forward={bool(sd.get('shard_params', False))} (shard layout differs), "
-                f"engine runs with {self.shard_params}: resume with the same setting"
-            )
-        layout = [(b.name, b.start, b.size, b.shard_start, b.shard_size) for b in self.buckets]
-        if "layout" in sd and [tuple(x) for x in sd["layout"]] != layout:
-            raise ValueError("checkpoint bucket layout does not match this model / mesh (different model size or parameter set)")
+        self.layout.check_saved(sd.get("layout"), sd["fsdp_size"], sd.get("shard_params", False))
         self.step_count = int(sd["step"])
         self.master.copy_(sd["master"])
         self.exp_avg.copy_(sd["exp_avg"])

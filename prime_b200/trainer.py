@@ -20,6 +20,7 @@ from .models.llama import Transformer, build_model
 from .optim.schedule import lr_at
 from .parallel.diloco import DilocoOuter, OuterHyper
 from .parallel.fsdp import AdamHyper, ShardedEngine
+from .parallel.layout import plan_layout, use_zero3
 from .parallel.mesh import Mesh, WorldInfo, build_mesh, init_distributed
 
 
@@ -64,11 +65,8 @@ class Trainer:
         self.model.set_fp8(cfg.train.fp8)  # MXFP8 forward / dgrad GEMMs (opt-in; the headline benchmark is bf16)
         self.heap = None
         use_fused = cuda and cfg.train.fused_comm
-        n_params = sum(p.numel() for p in self.model.parameters())
-        reshard = cfg.train.reshard_after_forward
-        if reshard is None:
-            reshard = n_params >= 5e9
-        shard_params = bool(reshard) and use_fused and mesh.fsdp_size > 1
+        shard_params = use_zero3(cfg.train.reshard_after_forward, fused=use_fused, fsdp_size=mesh.fsdp_size,
+                                 n_params=sum(p.numel() for p in self.model.parameters()))
         if cfg.train.reshard_after_forward and not shard_params:
             raise ValueError("train.reshard_after_forward=true needs CUDA, train.fused_comm=true and mesh.fsdp_size > 1 "
                              "(the parameter gather runs inside the GEMM kernels over the symmetric NVLink heap)")  # fmt: skip
@@ -78,14 +76,7 @@ class Trainer:
         if use_fused:
             from .parallel.symm import SymmetricHeap, dist_exchange
 
-            F = mesh.fsdp_size
-            pad = (len(list(self.model.parameters())) + 64) * 8 + (self.model.args.n_layers + 4) * F * 1024
-            total = n_params + pad
-            per_shard = total // F + (self.model.args.n_layers + 4) * 1024
-            # fp32 main_grad (+ bf16 params when replicated, + the bf16 shard under ZeRO-3) + int8 outer payload and scales
-            nbytes = total * 4 + (per_shard * 2 if shard_params else total * 2) + per_shard * 2 + (64 << 20)
-            if fp32_outer:
-                nbytes += per_shard * 4
+            nbytes = plan_layout(self.model, mesh.fsdp_size, shard_params).heap_bytes(fp32_master=fp32_outer)
             heap_cls = SymmetricHeap
             if _want_nvls() and mesh.world.world_size > 1:
                 from .parallel.multicast import MulticastHeap, nvls_available

@@ -33,10 +33,10 @@ import sys
 from dataclasses import dataclass, field
 
 from ..models.llama import ModelArgs, get_model_args
+from ..parallel.layout import SHARD_ALIGN, use_zero3
 
 GB = 1e9
 H100_HBM_BYTES = int(80 * GB)
-SHARD_ALIGN = 1024
 CUDA_CONTEXT_BYTES = int(1.5 * GB)  # context + loaded modules + cuBLAS / NCCL workspaces of the comparison paths (measured ≈ 1.1 GB)
 
 
@@ -123,9 +123,7 @@ def plan_memory(a: ModelArgs, *, fsdp_size: int = 1, micro_bs: int = 1, seq_len:
     backend is on)."""
     c = count_params(a)
     N, F = c["total"], max(1, fsdp_size)
-    if shard_params is None:
-        shard_params = N >= 5e9
-    shard_params = bool(shard_params) and fused and F > 1
+    shard_params = use_zero3(shard_params, fused=fused, fsdp_size=F, n_params=N)
     pad = 1.001  # bucket padding to F·1024 elements and 16-byte parameter alignment
     shard = N / F * pad
     where = "heap" if fused else "torch"

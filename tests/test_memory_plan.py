@@ -8,6 +8,7 @@ import pytest
 import torch
 
 from prime_b200.models.llama import Transformer, get_model_args
+from prime_b200.parallel.layout import plan_layout
 from prime_b200.utils import memory_plan as mp
 
 
@@ -70,15 +71,12 @@ def test_torch_side_rows_match_the_measured_1b_run():
 
 
 def test_heap_rows_equal_the_trainers_heap_sizing():
-    """trainer.py sizes the symmetric heap as 4·total + 2·(total | shard) + 2·shard + 64 MiB: the plan's heap rows must add up to it."""
+    """trainer.py sizes the symmetric heap with the shard layout's ``heap_bytes``: the plan's heap rows must add up to it."""
     for name, F, z3 in (("1B", 2, False), ("7B", 8, True)):
         a = get_model_args(name)
         with torch.device("meta"):
             model = Transformer(a)
-        n_params, n_tensors = sum(p.numel() for p in model.parameters()), len(list(model.parameters()))
-        total = n_params + (n_tensors + 64) * 8 + (a.n_layers + 4) * F * 1024
-        per_shard = total // F + (a.n_layers + 4) * 1024
-        nbytes = total * 4 + (per_shard * 2 if z3 else total * 2) + per_shard * 2 + (64 << 20)
+        nbytes = plan_layout(model, F, z3).heap_bytes()
         plan = mp.plan_memory(a, fsdp_size=F, shard_params=z3)
         assert abs(plan.heap_bytes - nbytes) / nbytes < 0.005, (name, plan.heap_bytes, nbytes)
 

@@ -223,20 +223,18 @@ def test_assemble_full_model_from_fsdp2_shards(tmp_path):
     assert abs(total - rows[-1]["param_hash"]) < 1e-3 * abs(total), (total, rows[-1]["param_hash"])
 
 
-def test_assemble_full_model_from_zero3_row_shards(tmp_path):
+def test_assemble_full_model_from_zero3_row_shards_planned_by_the_layout(tmp_path):
     """ZeRO-3 checkpoints cut every 2-D weight into one row block per rank (and keep the 1-D gains in a small flat bucket).
-    The engine only runs that mode on GPUs, so the rank files are synthesised here with the engine's own planner and the
-    slicing rule of ``ShardedEngine._attach_rows_bucket``."""
+    The engine only runs that mode on GPUs, so the rank files are synthesised here with the engine's own planner and an
+    independent statement of the row cut."""
     from prime_b200.models.llama import build_model
-    from prime_b200.parallel.fsdp import ShardedEngine
+    from prime_b200.parallel.layout import plan_layout
 
     F = 2
     src = build_model("debugmodel", dtype=torch.float32, seed=21)
-    plan = ShardedEngine.__new__(ShardedEngine)
-    plan.model, plan.F, plan.shard_params = src, F, True
-    plan._build_buckets()
+    plan = plan_layout(src, F, True)
     assert {b.kind for b in plan.buckets} == {"rows", "flat"}
-    layout = [[b.name, b.start, b.size, b.shard_start, b.shard_size] for b in plan.buckets]
+    layout = plan.signature
     step = tmp_path / "step_000001"
     step.mkdir()
     for r in range(F):
