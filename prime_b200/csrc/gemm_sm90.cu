@@ -1,4 +1,5 @@
-// bf16 GEMM for sm_90a: TMA → 128B-swizzled shared memory → wgmma (accumulators in registers) → epilogue from registers.
+// bf16 GEMM for sm_90a: TMA → 128B-swizzled shared memory → wgmma (accumulators in registers) → epilogue (local GEMMs: staged
+// through shared memory and written by TMA stores; collective variants: straight from registers).
 // Persistent, warp-specialised, one CTA per SM.
 //
 //   C[M,N] (bf16 | fp32, optional +=)  =  A ⋅ Bᵀ   with fp32 accumulation
@@ -14,8 +15,8 @@
 // BN = 256 (local GEMMs only, IO = 0): 4 stages of 48 KB; the producer warpgroup drops to 40 registers and the consumer
 // warpgroups rise to 232 (setmaxnreg) to hold 128 fp32 accumulators per thread. tile_policy() picks BN from the shape.
 // Warp roles: warpgroup 0 = w0 TMA producer (1 lane), w3 gather copier (IO = 1 / 3); warpgroups 1 and 2 = consumers, each
-// issuing m64nBNk16 wgmma for 64 rows of the tile and running the epilogue of those rows straight from its registers, while
-// the producer already fills the ring for the next tile.
+// issuing m64nBNk16 wgmma for 64 rows of the tile and running the epilogue of those rows, while the producer already fills
+// the ring for the next tile (IO = 0: see kOutSlots).
 #include <cuda.h>
 
 #include "common.cuh"
@@ -48,15 +49,23 @@ constexpr uint32_t kCopyChunkBytes = 128 * BK * 2;  // IO = 3 weight-gather copi
 constexpr int kCopyBufs = 2;
 constexpr int kGatherSub = 4;  // IO = 3: readiness flags per rank block (a block is released to the MMA tiles in quarters)
 
+// IO = 0 epilogue staging: each consumer warpgroup owns kOutSlots slots of 64 rows x 64 B, the box of a 64B-swizzled output
+// tensor map (32 bf16 or 16 fp32 columns). The epilogue writes a step of slots, one elected thread TMA-stores them, and the
+// warpgroup goes on without waiting for the global writes.
+constexpr int kOutSlots = 4;
+constexpr uint32_t kSlotBytes = 64 * 64;
+
 template <int IO, int TBN>
 struct Geo {
   static constexpr int kStages = TBN == kWideBN ? 4 : IO == 3 ? 5 : 6;
   static constexpr uint32_t kBBytes = TBN * BK * 2;  // 16 | 32 KB
   static constexpr uint32_t kStageBytes = kABytes + kBBytes;
   static constexpr uint32_t kCopyBytes = IO == 3 ? kCopyBufs * kCopyChunkBytes : 0;
-  static constexpr uint32_t kSmemBytes = kStages * kStageBytes + kCopyBytes + 1024 /*align slack*/ + 512 /*barriers*/;
+  static constexpr uint32_t kOutBytes = IO == 0 ? 2 * kOutSlots * kSlotBytes : 0;
+  static constexpr uint32_t kSmemBytes = kStages * kStageBytes + kCopyBytes + kOutBytes + 1024 /*align slack*/ + 512 /*barriers*/;
 };
-static_assert(Geo<0, kWideBN>::kSmemBytes <= 227 * 1024, "wide tile ring exceeds the shared memory of an SM");
+static_assert(Geo<0, kWideBN>::kSmemBytes <= 227 * 1024, "wide tile ring + epilogue staging exceed the shared memory of an SM");
+static_assert(Geo<0, BN>::kSmemBytes <= 227 * 1024, "narrow tile ring + epilogue staging exceed the shared memory of an SM");
 
 using namespace tc;
 
@@ -117,7 +126,7 @@ struct GemmParams {
 //           contraction runs over the sharded rows): the K loop is rotated instead. The shards are read-only during
 //           forward/backward, so no inter-rank barrier is needed around the kernel.
 struct PeerMaps {
-  CUtensorMap m[8];
+  CUtensorMap m[8];   // IO = 0: the epilogue's 64B-swizzled output maps: m[0] C, m[1] h (SwiGLU), m[2] the saved gate_up (read)
   float* c[8];        // IO = 2: the ranks' fp32 output buffers as mapped in this process
   int n;              // ranks
   int rows_per_rank;  // IO 1/2: multiple of the tile height; IO 3: rows of B owned by each rank
@@ -210,10 +219,12 @@ __global__ void __launch_bounds__(kThreads, 1)
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* copy_buf = smem + kStages * kStageBytes;  // IO = 3: kCopyBufs x 16 KB bounce buffers of the weight-gather copier
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(copy_buf + G::kCopyBytes);
+  uint8_t* out_buf = copy_buf + G::kCopyBytes;  // IO = 0: 2 x kOutSlots epilogue staging slots
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(out_buf + G::kOutBytes);
   uint64_t* empty_bar = full_bar + kStages;
   uint64_t* copied_bar = empty_bar + kStages;  // IO = 1: the gather copier has finished reading a consumed ring slot
   uint64_t* cp_bar = copied_bar + kStages;     // IO = 3: a peer box has landed in bounce buffer i
+  uint64_t* aux_bar = cp_bar + kCopyBufs;      // IO = 0 SwiGLU backward: gate / up boxes landed in slot pair 2·wg + half
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   constexpr bool swiglu = EPI == 2;
@@ -262,6 +273,11 @@ __global__ void __launch_bounds__(kThreads, 1)
     }
     if (IO == 1 || IO == 3)
       for (int i = 0; i < pm.n; ++i) prefetch_tmap(&pm.m[i]);
+    if (IO == 0) {  // the epilogue's maps (see PeerMaps)
+      prefetch_tmap(&pm.m[0]);
+      if (EPI == 2) prefetch_tmap(&pm.m[1]);
+      if (EPI == 3) prefetch_tmap(&pm.m[2]);
+    }
   }
   if (warp == 1 && lane == 0) {
     for (int i = 0; i < kStages; ++i) {
@@ -270,6 +286,8 @@ __global__ void __launch_bounds__(kThreads, 1)
       mbar_init(&copied_bar[i], 1);
     }
     for (int i = 0; i < kCopyBufs; ++i) mbar_init(&cp_bar[i], 1);
+    if (IO == 0 && EPI == 3)
+      for (int i = 0; i < 4; ++i) mbar_init(&aux_bar[i], 1);
     fence_barrier_init();
   }
   __syncthreads();
@@ -458,6 +476,33 @@ __global__ void __launch_bounds__(kThreads, 1)
     int stage = 0;
     uint32_t phase = 0;
     float acc[TBN / 2];
+    // IO = 0 staged epilogue: this warpgroup's slots, its leader (the one thread that issues TMA), the swizzle key of this
+    // thread's rows (rows r and r + 8 share it), the slot offset of row r, and the count of double-buffered steps so far
+    uint8_t* slots = out_buf + wg * (kOutSlots * kSlotBytes);
+    const bool leader = IO == 0 && (threadIdx.x & 127) == 0;
+    const uint32_t skey = (lane >> 3) & 3;
+    const uint32_t roff = (wi * 16 + (lane >> 2)) * 64;
+    uint32_t ostep = 0;
+    // SwiGLU backward: the leader TMA-loads the gate / up boxes of the step two ahead of the one the warpgroup is working on, in
+    // the step order of the tile sequence, so the first two steps of a tile land during its main loop. Cursor: tile, step.
+    int l_it = 0, l_tile = sched_id, l_st = 0;
+    uint32_t l_n = 0;
+    auto aux_issue = [&] {  // leader: load the cursor's step into slot pair l_n % 2, then advance the cursor
+      int tm, tn, kind;
+      coords(l_tile, tm, tn, kind);
+      const int f0 = tn * TBN + 32 * l_st;
+      uint64_t* bar = &aux_bar[2 * wg + (l_n & 1)];
+      uint8_t* dst = slots + (l_n & 1) * (2 * kSlotBytes);
+      mbar_expect_tx(bar, 2 * kSlotBytes);
+      tma_load_2d(&pm.m[2], bar, dst, f0, tm * BM + wg * 64);
+      tma_load_2d(&pm.m[2], bar, dst + kSlotBytes, p.swiglu_ff + f0, tm * BM + wg * 64);
+      ++l_n;
+      if (++l_st == TBN / 32 || f0 + 32 >= p.swiglu_ff) l_st = 0, l_tile = sched_id + (++l_it) * sched_n;
+    };
+    if constexpr (IO == 0 && EPI == 3) {
+      if (leader)
+        for (int i = 0; i < 2 && l_tile < num_tiles; ++i) aux_issue();
+    }
     for (int it = 0, tile; (tile = next_tile(it)) >= 0;) {
       int tm, tn, kind;
       coords(tile, tm, tn, kind);
@@ -491,7 +536,176 @@ __global__ void __launch_bounds__(kThreads, 1)
       // ---- epilogue: accumulator element acc[4j + i] is row r0 (+8 for i >= 2), column 8j + 2·(lane % 4) (+1 for odd i)
       const int r0 = tm * BM + wg * 64 + wi * 16 + (lane >> 2);
       const int cq = 2 * (lane & 3);
-      if constexpr (EPI == 2) {
+      if constexpr (IO == 0) {
+        // Staged: a step writes slots, then the leader TMA-stores them (the unit clips rows >= M and columns past the map).
+        const int row0 = tm * BM + wg * 64;
+        auto step_begin = [&](bool single) {  // the slots about to be written have been read out by their previous store
+          if (leader) {
+            if (single) bulk_wait_read<0>();
+            else bulk_wait_read<1>();
+          }
+          named_bar_sync(1 + wg, 128);
+        };
+        auto step_end = [&] {  // every thread's slot writes → the leader's TMA store
+          fence_proxy_async_smem();
+          named_bar_sync(1 + wg, 128);
+        };
+        // byte offset in a slot of this thread's pair in 16-byte chunk jj (0..3), row + 8h; 64B swizzle: chunk ^= (row / 2) % 4
+        auto off16 = [&](int jj, int h) { return roff + h * 512 + ((((uint32_t)jj) ^ skey) << 4) + 4 * (lane & 3); };
+        // fp32 pair of column group jj (0..1) of a 16-column slot
+        auto off32 = [&](int jj, int h) { return roff + h * 512 + (((2u * jj + ((lane & 3) >> 1)) ^ skey) << 4) + 8 * (lane & 1); };
+        auto st32 = [&](uint8_t* s, uint32_t v) { *reinterpret_cast<uint32_t*>(s) = v; };
+        if constexpr (EPI == 2) {
+          const int FF = p.swiglu_ff;
+          constexpr int kFeat8 = TBN / 16;  // 8-feature column groups of the gate half; the up half follows
+#pragma unroll
+          for (int st = 0; st < TBN / 64; ++st) {  // 32 features per step: gate, up and h in slots 0, 1, 2 (single-buffered)
+            const int f0 = tn * (TBN / 2) + 32 * st;
+            if (f0 >= FF) break;  // FF % 128 = 64: the last wide tile's gate and up halves are half zero-filled
+            step_begin(true);
+#pragma unroll
+            for (int jj = 0; jj < 4; ++jj) {
+              const int j = 4 * st + jj;
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+                const uint32_t gw = bf16x2_bits(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+                const uint32_t uw = bf16x2_bits(acc[4 * (j + kFeat8) + 2 * h], acc[4 * (j + kFeat8) + 2 * h + 1]);
+                // h = silu(gate)·up from the bf16-ROUNDED gate/up — bit-compatible with the stand-alone kernel that reads them back
+                const float2 gf = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&gw));
+                const float2 uf = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&uw));
+                const float h0 = gf.x / (1.f + __expf(-gf.x)) * uf.x, h1 = gf.y / (1.f + __expf(-gf.y)) * uf.y;
+                const uint32_t o = off16(jj, h);
+                st32(slots + o, gw);
+                st32(slots + kSlotBytes + o, uw);
+                st32(slots + 2 * kSlotBytes + o, bf16x2_bits(h0, h1));
+              }
+            }
+            step_end();
+            if (leader) {
+              tma_store_2d(&pm.m[0], slots, f0, row0);
+              tma_store_2d(&pm.m[0], slots + kSlotBytes, FF + f0, row0);
+              tma_store_2d(&pm.m[1], slots + 2 * kSlotBytes, f0, row0);
+              bulk_commit();
+            }
+          }
+        } else if constexpr (EPI == 3) {
+          const int FF = p.swiglu_ff;
+#pragma unroll
+          for (int st = 0; st < TBN / 32; ++st) {  // 32 features per step, turned into d_gate / d_up in the slot pair loaded for it
+            const int f0 = tn * TBN + 32 * st;
+            if (f0 >= FF) break;
+            uint8_t* sg = slots + (ostep & 1) * (2 * kSlotBytes);
+            mbar_wait(&aux_bar[2 * wg + (ostep & 1)], (ostep >> 1) & 1);
+#pragma unroll
+            for (int jj = 0; jj < 4; ++jj) {
+              const int j = 4 * st + jj;
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+                const uint32_t o = off16(jj, h);
+                const uint32_t gw = *reinterpret_cast<const uint32_t*>(sg + o);
+                const uint32_t uw = *reinterpret_cast<const uint32_t*>(sg + kSlotBytes + o);
+                const float2 gf = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&gw));
+                const float2 uf = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&uw));
+                const float d0 = acc[4 * j + 2 * h], d1 = acc[4 * j + 2 * h + 1];
+                // sigmoid through ex2.approx + rcp.approx: IEEE division would make the epilogue longer than the tile's MMAs
+                const float s0 = __fdividef(1.f, 1.f + exp2f(-1.4426950408889634f * gf.x));
+                const float s1 = __fdividef(1.f, 1.f + exp2f(-1.4426950408889634f * gf.y));
+                const float dg0 = d0 * uf.x * s0 * (1.f + gf.x * (1.f - s0)), dg1 = d1 * uf.y * s1 * (1.f + gf.y * (1.f - s1));
+                const float du0 = d0 * gf.x * s0, du1 = d1 * gf.y * s1;
+                st32(sg + o, bf16x2_bits(dg0, dg1));
+                st32(sg + kSlotBytes + o, bf16x2_bits(du0, du1));
+              }
+            }
+            step_end();
+            if (leader) {
+              tma_store_2d(&pm.m[0], sg, f0, row0);
+              tma_store_2d(&pm.m[0], sg + kSlotBytes, FF + f0, row0);
+              bulk_commit();
+              if (l_tile < num_tiles) {  // the pair is read out: it takes the boxes of the step two ahead
+                bulk_wait_read<0>();
+                aux_issue();
+              }
+            }
+            ++ostep;
+          }
+        } else if (p.c_fp32) {
+#pragma unroll
+          for (int st = 0; st < TBN / 32; ++st) {  // 32 columns = 2 slots per step, double-buffered
+            const int c0 = tn * TBN + 32 * st;
+            if (c0 >= p.N) break;
+            uint8_t* sb = slots + (ostep & 1) * (2 * kSlotBytes);
+            step_begin(false);
+#pragma unroll
+            for (int jj = 0; jj < 4; ++jj) {
+              const int j = 4 * st + jj;
+#pragma unroll
+              for (int h = 0; h < 2; ++h)
+                *reinterpret_cast<float2*>(sb + (jj >> 1) * kSlotBytes + off32(jj & 1, h)) =
+                    make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+            }
+            step_end();
+            if (leader) {
+              // += (unsplit or split-K): the TMA unit adds the slot into C in the L2, one fp32 add per element
+#pragma unroll
+              for (int i = 0; i < 2; ++i) {
+                if (c0 + 16 * i >= p.N) break;
+                if (p.accumulate) tma_reduce_add_2d(&pm.m[0], sb + i * kSlotBytes, c0 + 16 * i, row0);
+                else tma_store_2d(&pm.m[0], sb + i * kSlotBytes, c0 + 16 * i, row0);
+              }
+              bulk_commit();
+            }
+            ++ostep;
+          }
+        } else {
+          // RoPE: the position of each of this thread's two rows is fixed for the tile; TBN is a multiple of rope_D
+          int rope_row[2] = {0, 0};
+          if (EPI == 1) {
+            rope_row[0] = (r0 % p.rope_S) * (p.rope_D >> 1);
+            rope_row[1] = ((r0 + 8) % p.rope_S) * (p.rope_D >> 1);
+          }
+#pragma unroll
+          for (int st = 0; st < TBN / 64; ++st) {  // 64 columns = 2 slots per step, double-buffered
+            const int c0 = tn * TBN + 64 * st;
+            if (c0 >= p.N) break;
+            uint8_t* sb = slots + (ostep & 1) * (2 * kSlotBytes);
+            const bool rot = EPI == 1 && c0 < p.rope_cols;  // rope_cols is a multiple of rope_D (64 | 128)
+            step_begin(false);
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj) {
+              const int j = 8 * st + jj;
+              const int c = tn * TBN + 8 * j + cq;
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+                float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+                if (rot) {  // Q/K head columns: rotate the interleaved pair in registers
+                  const int ti = rope_row[h] + (((8 * j + cq) & (p.rope_D - 1)) >> 1);
+                  const float cs = __ldg(p.rope_cos + ti), sn = __ldg(p.rope_sin + ti);
+                  const float a = v0, b = v1;
+                  v0 = a * cs - b * sn;
+                  v1 = a * sn + b * cs;
+                }
+                if (EPI == 0 && p.accumulate && r0 + 8 * h < p.M && c < p.N) {  // bf16 += (RoPE never): fp32 add, one rounding
+                  const float2 o =
+                      __bfloat1622float2(*(reinterpret_cast<const __nv_bfloat162*>(p.C) + ((int64_t)(r0 + 8 * h) * p.ldc + c) / 2));
+                  v0 += o.x;
+                  v1 += o.y;
+                }
+                st32(sb + (jj >> 2) * kSlotBytes + off16(jj & 3, h), bf16x2_bits(v0, v1));
+              }
+            }
+            step_end();
+            if (leader) {
+#pragma unroll
+              for (int i = 0; i < 2; ++i) {
+                if (c0 + 32 * i >= p.N) break;
+                tma_store_2d(&pm.m[0], sb + i * kSlotBytes, c0 + 32 * i, row0);
+              }
+              bulk_commit();
+            }
+            ++ostep;
+          }
+        }
+      } else if constexpr (EPI == 2) {
         const int FF = p.swiglu_ff;
         __nv_bfloat16* gu = reinterpret_cast<__nv_bfloat16*>(p.C);
         __nv_bfloat16* hp = reinterpret_cast<__nv_bfloat16*>(p.H);
@@ -592,6 +806,7 @@ __global__ void __launch_bounds__(kThreads, 1)
         }
       }
     }
+    if (IO == 0 && leader) bulk_wait_all();  // the last stores have left shared memory
     if (IO == 2) __threadfence_system();  // peer reductions are performed before this kernel retires (a barrier follows)
   }
 }
@@ -811,9 +1026,15 @@ PB_EXPORT int pb_gemm_bf16(const void* A, const void* B, void* C, int M, int N, 
   } else if ((rc = operand_tmap(&tb, B, N, K, ldb, b_mn_major, e.kind == 2 ? 64 : tbn))) {
     return rc;
   }
+  // the staged epilogue's maps (the checks above and check_epilogue give TMA its 16-byte aligned addresses and row strides):
+  // C [M, N] (SwiGLU backward: d_gate_up [M, 2·N]), h [M, FF] for SwiGLU, the saved gate_up [M, 2·N] for SwiGLU backward
+  PeerMaps om = {};
+  if ((rc = pbhost::cached_tmap_staging(&om.m[0], C, M, e.kind == 3 ? 2 * N : N, ldc, c_fp32 != 0))) return rc;
+  if (e.kind == 2 && (rc = pbhost::cached_tmap_staging(&om.m[1], e.aux, M, N / 2, e.ld_aux, false))) return rc;
+  if (e.kind == 3 && (rc = pbhost::cached_tmap_staging(&om.m[2], e.aux, M, 2 * N, e.ld_aux, false))) return rc;
   GemmParams p = make_params(C, M, N, K, ldc, a_mn_major, b_mn_major, c_fp32, accumulate, e);
   if (c_fp32 && accumulate) p.split_k = split_for(((M + BM - 1) / BM) * ((N + tbn - 1) / tbn), (K + BK - 1) / BK);  // plain only
-  return dispatch(0, e.kind, p, ta, tb, stream, nullptr, wide && e.kind == 2 ? &tup : nullptr, nullptr, wide);
+  return dispatch(0, e.kind, p, ta, tb, stream, &om, wide && e.kind == 2 ? &tup : nullptr, nullptr, wide);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------------

@@ -84,6 +84,18 @@ __device__ __forceinline__ void tma_store_3d(const CUtensorMap* map, const void*
                "r"(smem_u32(smem)), "r"(c0), "r"(c1), "r"(c2)
                : "memory");
 }
+// smem → global tensor reduce-add (fp32 += in the L2, one add per element; bulk async-group completion)
+__device__ __forceinline__ void tma_reduce_add_2d(const CUtensorMap* map, const void* smem, int c0, int c1) {
+  asm volatile("cp.reduce.async.bulk.tensor.2d.global.shared::cta.add.bulk_group [%0, {%2, %3}], [%1];" ::"l"(map),
+               "r"(smem_u32(smem)), "r"(c0), "r"(c1)
+               : "memory");
+}
+// generic-proxy shared-memory writes → visible to a following TMA store (async proxy) from the same CTA
+__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// named barrier of `count` threads (id 0 is __syncthreads)
+__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void bulk_wait_read() {

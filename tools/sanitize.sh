@@ -27,4 +27,8 @@ run racecheck "gpu and not S4096 and not S8192 and not 32768 and not doc_bounds"
 # bf16 GEMM in both tile widths (128 x 128 and the 128 x 256 setmaxnreg tile): every layout and epilogue at the small edge shapes
 run memcheck  "gpu and not 5632" memcheck_gemm_wide tests/test_gemm_wide_gpu.py
 run racecheck "gpu and not 5632" racecheck_gemm_wide tests/test_gemm_wide_gpu.py
+# staged GEMM epilogue (shared-memory slots, TMA stores, TMA loads of the saved gate_up) in both tile widths
+run memcheck  "gpu" memcheck_gemm_epilogue tests/test_gemm_epilogue_gpu.py
+run racecheck "gpu" racecheck_gemm_epilogue tests/test_gemm_epilogue_gpu.py
+run synccheck "gpu" synccheck_gemm_epilogue tests/test_gemm_epilogue_gpu.py
 cat gpurun_out/sanitizer_summary.txt
