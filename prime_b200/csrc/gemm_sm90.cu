@@ -1,5 +1,5 @@
-// bf16 GEMM for sm_90a: TMA → 128B-swizzled shared memory → wgmma (accumulators in registers) → epilogue (local GEMMs: staged
-// through shared memory and written by TMA stores; collective variants: straight from registers).
+// bf16 GEMM for sm_90a: TMA → 128B-swizzled shared memory → wgmma (accumulators in registers) → epilogue staged through shared
+// memory and written by TMA stores (GEMM ⊕ reduce-scatter: fp32 atomics from registers into the owner rank's buffer).
 // Persistent, warp-specialised, one CTA per SM.
 //
 //   C[M,N] (bf16 | fp32, optional +=)  =  A ⋅ Bᵀ   with fp32 accumulation
@@ -16,7 +16,7 @@
 // warpgroups rise to 232 (setmaxnreg) to hold 128 fp32 accumulators per thread. tile_policy() picks BN from the shape.
 // Warp roles: warpgroup 0 = w0 TMA producer (1 lane), w3 gather copier (IO = 1 / 3); warpgroups 1 and 2 = consumers, each
 // issuing m64nBNk16 wgmma for 64 rows of the tile and running the epilogue of those rows, while the producer already fills
-// the ring for the next tile (IO = 0: see kOutSlots).
+// the ring for the next tile (see kOutSlots).
 #include <cuda.h>
 
 #include "common.cuh"
@@ -44,14 +44,15 @@ constexpr int kThreads = 384;
 constexpr int kConsumerWarps = 8;
 constexpr uint32_t kABytes = BM * BK * 2;  // 16 KB
 constexpr int kGroupM = 16;  // raster: super-rows of 16 M-tiles keep the A slab L2-resident
+constexpr int kAgIdleRounds = 2;  // IO = 1: scheduling rounds a CTA sits out after a gather tile (it costs several ordinary tiles)
 
 constexpr uint32_t kCopyChunkBytes = 128 * BK * 2;  // IO = 3 weight-gather copier: one {64 col, 128 row} box = 16 KB
 constexpr int kCopyBufs = 2;
 constexpr int kGatherSub = 4;  // IO = 3: readiness flags per rank block (a block is released to the MMA tiles in quarters)
 
-// IO = 0 epilogue staging: each consumer warpgroup owns kOutSlots slots of 64 rows x 64 B, the box of a 64B-swizzled output
-// tensor map (32 bf16 or 16 fp32 columns). The epilogue writes a step of slots, one elected thread TMA-stores them, and the
-// warpgroup goes on without waiting for the global writes.
+// Epilogue staging (every IO mode but the reduce-scatter): each consumer warpgroup owns kOutSlots slots of 64 rows x 64 B, the
+// box of a 64B-swizzled output tensor map (32 bf16 or 16 fp32 columns). The epilogue writes a step of slots, one elected thread
+// TMA-stores them, and the warpgroup goes on without waiting for the global writes.
 constexpr int kOutSlots = 4;
 constexpr uint32_t kSlotBytes = 64 * 64;
 
@@ -61,19 +62,22 @@ struct Geo {
   static constexpr uint32_t kBBytes = TBN * BK * 2;  // 16 | 32 KB
   static constexpr uint32_t kStageBytes = kABytes + kBBytes;
   static constexpr uint32_t kCopyBytes = IO == 3 ? kCopyBufs * kCopyChunkBytes : 0;
-  static constexpr uint32_t kOutBytes = IO == 0 ? 2 * kOutSlots * kSlotBytes : 0;
+  static constexpr uint32_t kOutBytes = IO != 2 ? 2 * kOutSlots * kSlotBytes : 0;
   static constexpr uint32_t kSmemBytes = kStages * kStageBytes + kCopyBytes + kOutBytes + 1024 /*align slack*/ + 512 /*barriers*/;
 };
 static_assert(Geo<0, kWideBN>::kSmemBytes <= 227 * 1024, "wide tile ring + epilogue staging exceed the shared memory of an SM");
 static_assert(Geo<0, BN>::kSmemBytes <= 227 * 1024, "narrow tile ring + epilogue staging exceed the shared memory of an SM");
+static_assert(Geo<1, BN>::kSmemBytes <= 227 * 1024, "all-gather ring + epilogue staging exceed the shared memory of an SM");
+static_assert(Geo<2, BN>::kSmemBytes <= 227 * 1024, "reduce-scatter ring exceeds the shared memory of an SM");
+static_assert(Geo<3, BN>::kSmemBytes <= 227 * 1024, "weight-gather ring + copier + epilogue staging exceed the shared memory of an SM");
 
 using namespace tc;
 
-__device__ __forceinline__ void tile_coords(int tile, int tiles_m, int tiles_n, int& tm, int& tn, int group_m = kGroupM) {
-  const int per_group = group_m * tiles_n;
+__device__ __forceinline__ void tile_coords(int tile, int tiles_m, int tiles_n, int& tm, int& tn) {
+  const int per_group = kGroupM * tiles_n;
   const int g = tile / per_group;
-  const int first_m = g * group_m;
-  const int gsz = min(group_m, tiles_m - first_m);
+  const int first_m = g * kGroupM;
+  const int gsz = min(kGroupM, tiles_m - first_m);
   const int r = tile - g * per_group;
   tm = first_m + r % gsz;
   tn = r / gsz;
@@ -85,25 +89,25 @@ struct GemmParams {
   int a_mn, b_mn;
   int c_fp32, accumulate;
   int split_k;  // >1 only with c_fp32 && accumulate: every K slice atomically adds its partial tile (weight-gradient GEMMs)
-  void* C;
-  // optional RoPE epilogue (QKV projection): output columns [0, rope_cols) are heads of width rope_D whose interleaved pairs are
-  // rotated by the position (row % rope_S) while the tile is still in registers; tables fp32 [rope_S.., rope_D/2]. bf16 outputs only.
-  const float* rope_cos;
-  const float* rope_sin;
-  int rope_S, rope_cols, rope_D;
-  // optional SwiGLU epilogue (gate/up projection): B = W13 stored [2·FF, K] as [gate rows | up rows]; a tile covers 64 features:
-  // the producer stages the 64 GATE rows and the matching 64 UP rows, so every thread holds gate and up of the same (row, feature)
-  // in accumulator columns j and j + 64. The epilogue stores gate and up (bf16, for the backward) into C = gate_up [M, 2·FF] and
-  // h = silu(gate)·up into the second output H [M, FF].
+  void* C;  // read by the bf16 += only; the staged epilogue writes through EpiMaps
+  // RoPE (EPI = 1, the QKV projection): output columns [0, rope_cols) are heads of width rope_D whose interleaved pairs are rotated
+  // by the position (row % rope_S) while the tile is still in registers. The kernel reads the RoPE fields only.
+  GemmEpilogue epi;
+  // SwiGLU (EPI = 2, gate/up projection): B = W13 stored [2·FF, K] as [gate rows | up rows]; a tile covers 64 features: the
+  // producer stages the 64 GATE rows and the matching 64 UP rows, so every thread holds gate and up of the same (row, feature) in
+  // accumulator columns j and j + 64. The epilogue stores gate and up (bf16, for the backward) into C = gate_up [M, 2·FF] and
+  // h = silu(gate)·up into h [M, FF].
+  // SwiGLU backward (EPI = 3, the down-projection's input-gradient GEMM dh = dy·W2, N = FF): the epilogue reads the saved bf16
+  // gate/up of the same (row, feature) from gate_up [M, 2·FF] and stores d_gate = dh·up·silu'(gate) and d_up = dh·silu(gate) into
+  // C = d_gate_up [M, 2·FF] — dh never exists in memory.
   int swiglu_ff;
-  int group_m;  // raster super-row height in M tiles (0 = kGroupM)
-  // optional SwiGLU-BACKWARD epilogue (EPI = 3; the down-projection's input-gradient GEMM dh = dy·W2, N = FF): the epilogue reads the
-  // saved bf16 gate/up activations of the same (row, feature) from `aux` = gate_up [M, 2·FF] and stores d_gate = dh·up·silu'(gate)
-  // and d_up = dh·silu(gate) into C = d_gate_up [M, 2·FF] — dh never exists in memory.
-  const void* aux;
-  int ld_aux;
-  void* H;  // EPI = 2: h [M, FF]
-  int ldh;
+};
+
+// The staged epilogue's 64B-swizzled tensor maps (see kOutSlots), for every IO mode but the reduce-scatter.
+struct EpiMaps {
+  CUtensorMap c;   // C [M, N] (SwiGLU backward: d_gate_up [M, 2·N]), bf16 or fp32
+  CUtensorMap h;   // EPI = 2: h [M, FF]
+  CUtensorMap gu;  // EPI = 3: the saved gate_up [M, 2·FF] (read)
 };
 
 // Fused collective GEMMs over the NVLink symmetric heap (IO template parameter of the kernel):
@@ -126,14 +130,13 @@ struct GemmParams {
 //           contraction runs over the sharded rows): the K loop is rotated instead. The shards are read-only during
 //           forward/backward, so no inter-rank barrier is needed around the kernel.
 struct PeerMaps {
-  CUtensorMap m[8];   // IO = 0: the epilogue's 64B-swizzled output maps: m[0] C, m[1] h (SwiGLU), m[2] the saved gate_up (read)
+  CUtensorMap m[8];   // IO = 1: the ranks' blocks of A; IO = 3: the ranks' shards of the weight
   float* c[8];        // IO = 2: the ranks' fp32 output buffers as mapped in this process
   int n;              // ranks
   int rows_per_rank;  // IO 1/2: multiple of the tile height; IO 3: rows of B owned by each rank
   int rank;
   uint32_t* flags;    // IO = 1: one counter per 128-row block of the gathered A (zeroed by the host before the launch)
                       // IO = 3: n * kGatherSub counters (chunks landed per quarter block), zeroed before the launch
-  int idle_rounds;    // IO = 1: scheduling rounds a CTA sits out after a gather tile (it costs several ordinary tiles: NVLink latency)
   // IO = 3
   int order[8];       // rank blocks in the order the copiers fetch them (= the order the tiles consume them)
   int cpr;            // 128-row chunk rows per rank block = ceil(rows_per_rank / 128)
@@ -150,6 +153,9 @@ struct PeerMaps {
   int ncpr, ncol_chunks;
   int norder[8];
 };
+// the kernel's parameters: four operand maps, GemmParams (padded to the maps' 64-byte alignment), EpiMaps and PeerMaps
+static_assert(4 * sizeof(CUtensorMap) + (sizeof(GemmParams) + 63) / 64 * 64 + sizeof(EpiMaps) + sizeof(PeerMaps) <= 4096,
+              "gemm_bf16_kernel's parameters exceed 4 KB");
 
 // IO = 1 tile schedule: [gather tiles][local tiles][dependent tiles]; kind 1 = gather (tn = 0 of a remote block), 0 = local rows,
 // 2 = dependent (waits for the block's flag, reads the local gathered copy). Lower indices never wait on higher ones.
@@ -172,9 +178,10 @@ __device__ __forceinline__ void ag_tile(int idx, const PeerMaps& pm, int tiles_n
   }
 }
 // IO = 1 static schedule with load balancing: iteration `it` of CTA `sched_id` → tile index, -1 = idle slot, -2 = done.
-// Round 0 hands gather tile p to CTA p < G; those CTAs then sit out `idle` rounds while the others keep taking tiles.
-__device__ __forceinline__ int ag_next(int it, int sched_id, int sched_n, int G, int idle, int num_tiles) {
-  if (G == 0 || G > sched_n || idle == 0) {
+// Round 0 hands gather tile p to CTA p < G; those CTAs then sit out kAgIdleRounds rounds while the others keep taking tiles.
+__device__ __forceinline__ int ag_next(int it, int sched_id, int sched_n, int G, int num_tiles) {
+  constexpr int idle = kAgIdleRounds;
+  if (G == 0 || G > sched_n) {
     const int t = sched_id + it * sched_n;
     return t < num_tiles ? t : -2;
   }
@@ -208,8 +215,9 @@ template <int A_MN, int B_MN, int EPI, int IO, int TBN>
 __global__ void __launch_bounds__(kThreads, 1)
     gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                      const __grid_constant__ CUtensorMap tmap_g, const __grid_constant__ CUtensorMap tmap_g2, const GemmParams p,
-                     const __grid_constant__ PeerMaps pm) {
+                     const __grid_constant__ EpiMaps em, const __grid_constant__ PeerMaps pm) {
   static_assert(TBN == BN || (TBN == kWideBN && IO == 0), "the wide tile exists for local GEMMs only");
+  static_assert(IO != 1 || EPI == 0, "all-gather ⊕ GEMM has no fused epilogue (its ag_next order would break the gate_up cursor)");
   constexpr bool wide = TBN == kWideBN;
   using G = Geo<IO, TBN>;
   constexpr int kStages = G::kStages;
@@ -219,12 +227,12 @@ __global__ void __launch_bounds__(kThreads, 1)
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* copy_buf = smem + kStages * kStageBytes;  // IO = 3: kCopyBufs x 16 KB bounce buffers of the weight-gather copier
-  uint8_t* out_buf = copy_buf + G::kCopyBytes;  // IO = 0: 2 x kOutSlots epilogue staging slots
+  uint8_t* out_buf = copy_buf + G::kCopyBytes;  // IO != 2: 2 x kOutSlots epilogue staging slots
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(out_buf + G::kOutBytes);
   uint64_t* empty_bar = full_bar + kStages;
   uint64_t* copied_bar = empty_bar + kStages;  // IO = 1: the gather copier has finished reading a consumed ring slot
   uint64_t* cp_bar = copied_bar + kStages;     // IO = 3: a peer box has landed in bounce buffer i
-  uint64_t* aux_bar = cp_bar + kCopyBufs;      // IO = 0 SwiGLU backward: gate / up boxes landed in slot pair 2·wg + half
+  uint64_t* aux_bar = cp_bar + kCopyBufs;      // SwiGLU backward: gate / up boxes landed in slot pair 2·wg + half
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   constexpr bool swiglu = EPI == 2;
@@ -241,14 +249,13 @@ __global__ void __launch_bounds__(kThreads, 1)
   auto next_tile = [&](int& it) -> int {
     if (IO == 1 && pm.n > 1) {
       for (;;) {
-        const int t = ag_next(it++, sched_id, sched_n, ag_G, pm.idle_rounds, num_tiles);
+        const int t = ag_next(it++, sched_id, sched_n, ag_G, num_tiles);
         if (t != -1) return t;
       }
     }
     const int t = sched_id + (it++) * sched_n;
     return t < num_tiles ? t : -2;
   };
-  const int group_m = p.group_m > 0 ? p.group_m : kGroupM;
   // IO = 3 rotations (see PeerMaps): K-major B → output columns start at the own rank block; MN-major B → the K loop does
   const int tn_rot = (IO == 3 && B_MN == 0 && pm.gate) ? pm.start : 0;
   const int kb_rot = (IO == 3 && B_MN == 1 && pm.gate) ? pm.start : 0;
@@ -258,7 +265,7 @@ __global__ void __launch_bounds__(kThreads, 1)
     if (IO == 1 && pm.n > 1) {
       ag_tile(tile, pm, tiles_n, tpr, tm, tn, kind);
     } else {
-      tile_coords(tile / split_k, tiles_m, tiles_n, tm, tn, group_m);
+      tile_coords(tile / split_k, tiles_m, tiles_n, tm, tn);
       if (IO == 2) tm = rs_tile_row(tm, pm, tpr);
       if (IO == 3 && tn_rot) tn = (tn + tn_rot) % tiles_n;
     }
@@ -273,10 +280,10 @@ __global__ void __launch_bounds__(kThreads, 1)
     }
     if (IO == 1 || IO == 3)
       for (int i = 0; i < pm.n; ++i) prefetch_tmap(&pm.m[i]);
-    if (IO == 0) {  // the epilogue's maps (see PeerMaps)
-      prefetch_tmap(&pm.m[0]);
-      if (EPI == 2) prefetch_tmap(&pm.m[1]);
-      if (EPI == 3) prefetch_tmap(&pm.m[2]);
+    if (IO != 2) {  // the staged epilogue's maps
+      prefetch_tmap(&em.c);
+      if (EPI == 2) prefetch_tmap(&em.h);
+      if (EPI == 3) prefetch_tmap(&em.gu);
     }
   }
   if (warp == 1 && lane == 0) {
@@ -286,7 +293,7 @@ __global__ void __launch_bounds__(kThreads, 1)
       mbar_init(&copied_bar[i], 1);
     }
     for (int i = 0; i < kCopyBufs; ++i) mbar_init(&cp_bar[i], 1);
-    if (IO == 0 && EPI == 3)
+    if (EPI == 3)
       for (int i = 0; i < 4; ++i) mbar_init(&aux_bar[i], 1);
     fence_barrier_init();
   }
@@ -416,7 +423,7 @@ __global__ void __launch_bounds__(kThreads, 1)
     // consumption order: peer shard --TMA load (NVLink)--> bounce buffer --TMA store--> local full copy, then bumps the
     // readiness counter of the box's quarter block once the store has fully completed. Two boxes are in flight per CTA.
     if (lane == 0) {
-      uint32_t ph[kCopyBufs] = {0, 0};
+      uint32_t ph = 0;  // bit i: the phase of bounce buffer i (a bit mask, not an array: no stack frame)
       // one list = one weight: (peer maps, local store map, rank order, geometry); `flags` != nullptr → publish per-quarter counters
       auto gather_list = [&](const CUtensorMap* maps, const CUtensorMap* store_map, const int* order, int n, int cpr, int col_chunks,
                              int spc, uint32_t* flags) {
@@ -443,8 +450,8 @@ __global__ void __launch_bounds__(kThreads, 1)
           int owner, cr, cc;
           box(i, owner, cr, cc);
           const int buf = i % kCopyBufs;
-          mbar_wait(&cp_bar[buf], ph[buf]);
-          ph[buf] ^= 1;
+          mbar_wait(&cp_bar[buf], (ph >> buf) & 1u);
+          ph ^= 1u << buf;
           // … and clipped by the store: dimension 1 of the 3-D map is the rows of ONE rank block
           tma_store_3d(store_map, copy_buf + buf * kCopyChunkBytes, cc * BK, cr * 128, owner);
           bulk_commit();
@@ -476,15 +483,17 @@ __global__ void __launch_bounds__(kThreads, 1)
     int stage = 0;
     uint32_t phase = 0;
     float acc[TBN / 2];
-    // IO = 0 staged epilogue: this warpgroup's slots, its leader (the one thread that issues TMA), the swizzle key of this
-    // thread's rows (rows r and r + 8 share it), the slot offset of row r, and the count of double-buffered steps so far
+    // staged epilogue: this warpgroup's slots, its leader (the one thread that issues TMA), the swizzle key of this thread's rows
+    // (rows r and r + 8 share it), the slot offset of row r, and the count of double-buffered steps so far
     uint8_t* slots = out_buf + wg * (kOutSlots * kSlotBytes);
-    const bool leader = IO == 0 && (threadIdx.x & 127) == 0;
+    const bool leader = IO != 2 && (threadIdx.x & 127) == 0;
     const uint32_t skey = (lane >> 3) & 3;
     const uint32_t roff = (wi * 16 + (lane >> 2)) * 64;
     uint32_t ostep = 0;
     // SwiGLU backward: the leader TMA-loads the gate / up boxes of the step two ahead of the one the warpgroup is working on, in
     // the step order of the tile sequence, so the first two steps of a tile land during its main loop. Cursor: tile, step.
+    // The cursor steps through the tiles in plain round-robin order, which is next_tile's order for IO = 0 and IO = 3 (whose tn
+    // rotation happens inside coords()); IO = 1's ag_next order would break it, and IO = 1 has no fused epilogue.
     int l_it = 0, l_tile = sched_id, l_st = 0;
     uint32_t l_n = 0;
     auto aux_issue = [&] {  // leader: load the cursor's step into slot pair l_n % 2, then advance the cursor
@@ -494,12 +503,12 @@ __global__ void __launch_bounds__(kThreads, 1)
       uint64_t* bar = &aux_bar[2 * wg + (l_n & 1)];
       uint8_t* dst = slots + (l_n & 1) * (2 * kSlotBytes);
       mbar_expect_tx(bar, 2 * kSlotBytes);
-      tma_load_2d(&pm.m[2], bar, dst, f0, tm * BM + wg * 64);
-      tma_load_2d(&pm.m[2], bar, dst + kSlotBytes, p.swiglu_ff + f0, tm * BM + wg * 64);
+      tma_load_2d(&em.gu, bar, dst, f0, tm * BM + wg * 64);
+      tma_load_2d(&em.gu, bar, dst + kSlotBytes, p.swiglu_ff + f0, tm * BM + wg * 64);
       ++l_n;
       if (++l_st == TBN / 32 || f0 + 32 >= p.swiglu_ff) l_st = 0, l_tile = sched_id + (++l_it) * sched_n;
     };
-    if constexpr (IO == 0 && EPI == 3) {
+    if constexpr (EPI == 3) {
       if (leader)
         for (int i = 0; i < 2 && l_tile < num_tiles; ++i) aux_issue();
     }
@@ -536,7 +545,7 @@ __global__ void __launch_bounds__(kThreads, 1)
       // ---- epilogue: accumulator element acc[4j + i] is row r0 (+8 for i >= 2), column 8j + 2·(lane % 4) (+1 for odd i)
       const int r0 = tm * BM + wg * 64 + wi * 16 + (lane >> 2);
       const int cq = 2 * (lane & 3);
-      if constexpr (IO == 0) {
+      if constexpr (IO != 2) {
         // Staged: a step writes slots, then the leader TMA-stores them (the unit clips rows >= M and columns past the map).
         const int row0 = tm * BM + wg * 64;
         auto step_begin = [&](bool single) {  // the slots about to be written have been read out by their previous store
@@ -582,9 +591,9 @@ __global__ void __launch_bounds__(kThreads, 1)
             }
             step_end();
             if (leader) {
-              tma_store_2d(&pm.m[0], slots, f0, row0);
-              tma_store_2d(&pm.m[0], slots + kSlotBytes, FF + f0, row0);
-              tma_store_2d(&pm.m[1], slots + 2 * kSlotBytes, f0, row0);
+              tma_store_2d(&em.c, slots, f0, row0);
+              tma_store_2d(&em.c, slots + kSlotBytes, FF + f0, row0);
+              tma_store_2d(&em.h, slots + 2 * kSlotBytes, f0, row0);
               bulk_commit();
             }
           }
@@ -618,8 +627,8 @@ __global__ void __launch_bounds__(kThreads, 1)
             }
             step_end();
             if (leader) {
-              tma_store_2d(&pm.m[0], sg, f0, row0);
-              tma_store_2d(&pm.m[0], sg + kSlotBytes, FF + f0, row0);
+              tma_store_2d(&em.c, sg, f0, row0);
+              tma_store_2d(&em.c, sg + kSlotBytes, FF + f0, row0);
               bulk_commit();
               if (l_tile < num_tiles) {  // the pair is read out: it takes the boxes of the step two ahead
                 bulk_wait_read<0>();
@@ -628,7 +637,7 @@ __global__ void __launch_bounds__(kThreads, 1)
             }
             ++ostep;
           }
-        } else if (p.c_fp32) {
+        } else if (IO == 0 && p.c_fp32) {  // fp32 outputs and += are local-GEMM only
 #pragma unroll
           for (int st = 0; st < TBN / 32; ++st) {  // 32 columns = 2 slots per step, double-buffered
             const int c0 = tn * TBN + 32 * st;
@@ -649,8 +658,8 @@ __global__ void __launch_bounds__(kThreads, 1)
 #pragma unroll
               for (int i = 0; i < 2; ++i) {
                 if (c0 + 16 * i >= p.N) break;
-                if (p.accumulate) tma_reduce_add_2d(&pm.m[0], sb + i * kSlotBytes, c0 + 16 * i, row0);
-                else tma_store_2d(&pm.m[0], sb + i * kSlotBytes, c0 + 16 * i, row0);
+                if (p.accumulate) tma_reduce_add_2d(&em.c, sb + i * kSlotBytes, c0 + 16 * i, row0);
+                else tma_store_2d(&em.c, sb + i * kSlotBytes, c0 + 16 * i, row0);
               }
               bulk_commit();
             }
@@ -660,15 +669,15 @@ __global__ void __launch_bounds__(kThreads, 1)
           // RoPE: the position of each of this thread's two rows is fixed for the tile; TBN is a multiple of rope_D
           int rope_row[2] = {0, 0};
           if (EPI == 1) {
-            rope_row[0] = (r0 % p.rope_S) * (p.rope_D >> 1);
-            rope_row[1] = ((r0 + 8) % p.rope_S) * (p.rope_D >> 1);
+            rope_row[0] = (r0 % p.epi.rope_S) * (p.epi.rope_D >> 1);
+            rope_row[1] = ((r0 + 8) % p.epi.rope_S) * (p.epi.rope_D >> 1);
           }
 #pragma unroll
           for (int st = 0; st < TBN / 64; ++st) {  // 64 columns = 2 slots per step, double-buffered
             const int c0 = tn * TBN + 64 * st;
             if (c0 >= p.N) break;
             uint8_t* sb = slots + (ostep & 1) * (2 * kSlotBytes);
-            const bool rot = EPI == 1 && c0 < p.rope_cols;  // rope_cols is a multiple of rope_D (64 | 128)
+            const bool rot = EPI == 1 && c0 < p.epi.rope_cols;  // rope_cols is a multiple of rope_D (64 | 128)
             step_begin(false);
 #pragma unroll
             for (int jj = 0; jj < 8; ++jj) {
@@ -678,13 +687,13 @@ __global__ void __launch_bounds__(kThreads, 1)
               for (int h = 0; h < 2; ++h) {
                 float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
                 if (rot) {  // Q/K head columns: rotate the interleaved pair in registers
-                  const int ti = rope_row[h] + (((8 * j + cq) & (p.rope_D - 1)) >> 1);
-                  const float cs = __ldg(p.rope_cos + ti), sn = __ldg(p.rope_sin + ti);
+                  const int ti = rope_row[h] + (((8 * j + cq) & (p.epi.rope_D - 1)) >> 1);
+                  const float cs = __ldg(p.epi.rope_cos + ti), sn = __ldg(p.epi.rope_sin + ti);
                   const float a = v0, b = v1;
                   v0 = a * cs - b * sn;
                   v1 = a * sn + b * cs;
                 }
-                if (EPI == 0 && p.accumulate && r0 + 8 * h < p.M && c < p.N) {  // bf16 += (RoPE never): fp32 add, one rounding
+                if (IO == 0 && EPI == 0 && p.accumulate && r0 + 8 * h < p.M && c < p.N) {  // bf16 += (local, plain): one rounding
                   const float2 o =
                       __bfloat1622float2(*(reinterpret_cast<const __nv_bfloat162*>(p.C) + ((int64_t)(r0 + 8 * h) * p.ldc + c) / 2));
                   v0 += o.x;
@@ -698,64 +707,15 @@ __global__ void __launch_bounds__(kThreads, 1)
 #pragma unroll
               for (int i = 0; i < 2; ++i) {
                 if (c0 + 32 * i >= p.N) break;
-                tma_store_2d(&pm.m[0], sb + i * kSlotBytes, c0 + 32 * i, row0);
+                tma_store_2d(&em.c, sb + i * kSlotBytes, c0 + 32 * i, row0);
               }
               bulk_commit();
             }
             ++ostep;
           }
         }
-      } else if constexpr (EPI == 2) {
-        const int FF = p.swiglu_ff;
-        __nv_bfloat16* gu = reinterpret_cast<__nv_bfloat16*>(p.C);
-        __nv_bfloat16* hp = reinterpret_cast<__nv_bfloat16*>(p.H);
-        constexpr int kFeat8 = TBN / 16;  // 8-feature column groups of the gate half; the up half follows
-#pragma unroll
-        for (int j = 0; j < kFeat8; ++j) {
-          const int f = tn * (TBN / 2) + 8 * j + cq;
-          if (wide && f >= FF) continue;  // FF % 128 = 64: the last wide tile's gate and up halves are half zero-filled
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const int r = r0 + 8 * h;
-            if (r >= p.M) continue;
-            const uint32_t gw = bf16x2_bits(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
-            const uint32_t uw = bf16x2_bits(acc[4 * (j + kFeat8) + 2 * h], acc[4 * (j + kFeat8) + 2 * h + 1]);
-            // h = silu(gate)·up from the bf16-ROUNDED gate/up — bit-compatible with the stand-alone kernel that reads them back
-            const float2 gf = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&gw));
-            const float2 uf = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&uw));
-            const float h0 = gf.x / (1.f + __expf(-gf.x)) * uf.x, h1 = gf.y / (1.f + __expf(-gf.y)) * uf.y;
-            *reinterpret_cast<uint32_t*>(gu + (int64_t)r * p.ldc + f) = gw;
-            *reinterpret_cast<uint32_t*>(gu + (int64_t)r * p.ldc + FF + f) = uw;
-            *reinterpret_cast<uint32_t*>(hp + (int64_t)r * p.ldh + f) = bf16x2_bits(h0, h1);
-          }
-        }
-      } else if constexpr (EPI == 3) {
-        const int FF = p.swiglu_ff;
-        const __nv_bfloat16* gu = reinterpret_cast<const __nv_bfloat16*>(p.aux);
-        __nv_bfloat16* dgu = reinterpret_cast<__nv_bfloat16*>(p.C);
-#pragma unroll
-        for (int j = 0; j < TBN / 8; ++j) {
-          const int f = tn * TBN + 8 * j + cq;
-          if (f >= FF) continue;
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const int r = r0 + 8 * h;
-            if (r >= p.M) continue;
-            const uint32_t gw = __ldg(reinterpret_cast<const unsigned int*>(gu + (int64_t)r * p.ld_aux + f));
-            const uint32_t uw = __ldg(reinterpret_cast<const unsigned int*>(gu + (int64_t)r * p.ld_aux + FF + f));
-            const float2 gf = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&gw));
-            const float2 uf = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&uw));
-            const float d0 = acc[4 * j + 2 * h], d1 = acc[4 * j + 2 * h + 1];
-            // sigmoid through ex2.approx + rcp.approx: IEEE division would make the epilogue longer than the tile's MMAs
-            const float s0 = __fdividef(1.f, 1.f + exp2f(-1.4426950408889634f * gf.x));
-            const float s1 = __fdividef(1.f, 1.f + exp2f(-1.4426950408889634f * gf.y));
-            const float dg0 = d0 * uf.x * s0 * (1.f + gf.x * (1.f - s0)), dg1 = d1 * uf.y * s1 * (1.f + gf.y * (1.f - s1));
-            const float du0 = d0 * gf.x * s0, du1 = d1 * gf.y * s1;
-            *reinterpret_cast<uint32_t*>(dgu + (int64_t)r * p.ldc + f) = bf16x2_bits(dg0, dg1);
-            *reinterpret_cast<uint32_t*>(dgu + (int64_t)r * p.ldc + FF + f) = bf16x2_bits(du0, du1);
-          }
-        }
       } else {
+        // reduce-scatter: add each fp32 pair into the buffer of the rank that owns the row (peer-mapped)
 #pragma unroll
         for (int j = 0; j < TBN / 8; ++j) {
           const int c = tn * TBN + 8 * j + cq;
@@ -764,49 +724,15 @@ __global__ void __launch_bounds__(kThreads, 1)
           for (int h = 0; h < 2; ++h) {
             const int r = r0 + 8 * h;
             if (r >= p.M) continue;
-            float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
-            if (p.c_fp32) {
-              if (IO == 2) {  // reduce-scatter: add into the owner rank's buffer (peer-mapped)
-                const int owner = r / pm.rows_per_rank;
-                float* dst = pm.c[owner] + (int64_t)(r - owner * pm.rows_per_rank) * p.ldc + c;
-                atomicAdd(dst, v0);
-                atomicAdd(dst + 1, v1);
-              } else {
-                float* dst = reinterpret_cast<float*>(p.C) + (int64_t)r * p.ldc + c;
-                if (p.accumulate && split_k > 1) {
-                  atomicAdd(dst, v0);
-                  atomicAdd(dst + 1, v1);
-                } else {
-                  if (p.accumulate) {
-                    const float2 o = *reinterpret_cast<const float2*>(dst);
-                    v0 += o.x;
-                    v1 += o.y;
-                  }
-                  *reinterpret_cast<float2*>(dst) = make_float2(v0, v1);
-                }
-              }
-            } else {
-              if (EPI == 1 && c < p.rope_cols) {  // Q/K head columns: rotate the interleaved pair in registers
-                const int pos = r % p.rope_S, d = c % p.rope_D;
-                const int64_t ti = (int64_t)pos * (p.rope_D >> 1) + (d >> 1);
-                const float cs = __ldg(p.rope_cos + ti), sn = __ldg(p.rope_sin + ti);
-                const float a = v0, b = v1;
-                v0 = a * cs - b * sn;
-                v1 = a * sn + b * cs;
-              }
-              __nv_bfloat16* dst = reinterpret_cast<__nv_bfloat16*>(p.C) + (int64_t)r * p.ldc + c;
-              if (p.accumulate) {
-                const float2 o = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(dst));
-                v0 += o.x;
-                v1 += o.y;
-              }
-              *reinterpret_cast<uint32_t*>(dst) = bf16x2_bits(v0, v1);
-            }
+            const int owner = r / pm.rows_per_rank;
+            float* dst = pm.c[owner] + (int64_t)(r - owner * pm.rows_per_rank) * p.ldc + c;
+            atomicAdd(dst, acc[4 * j + 2 * h]);
+            atomicAdd(dst + 1, acc[4 * j + 2 * h + 1]);
           }
         }
       }
     }
-    if (IO == 0 && leader) bulk_wait_all();  // the last stores have left shared memory
+    if (IO != 2 && leader) bulk_wait_all();  // the last stores have left shared memory
     if (IO == 2) __threadfence_system();  // peer reductions are performed before this kernel retires (a barrier follows)
   }
 }
@@ -831,9 +757,11 @@ int g_split_k_mode = -1;  // -1 auto, 0/1 off, n>1 forced
 const GemmEpilogue kPlain = {};
 
 template <int A_MN, int B_MN, int EPI, int IO, int TBN>
-int launch(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, cudaStream_t stream, const PeerMaps* pmp,
-           const CUtensorMap* tgp, const CUtensorMap* tg2p) {
+int launch(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, cudaStream_t stream, const EpiMaps* emp,
+           const PeerMaps* pmp, const CUtensorMap* tgp, const CUtensorMap* tg2p) {
+  static const EpiMaps kNoEpi = {};
   static const PeerMaps kNoPeers = {};
+  const EpiMaps& em = emp ? *emp : kNoEpi;
   const PeerMaps& pm = pmp ? *pmp : kNoPeers;
   const CUtensorMap& tg = tgp ? *tgp : ta;
   const CUtensorMap& tg2 = tg2p ? *tg2p : tg;
@@ -851,7 +779,7 @@ int launch(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p, cu
   const int tiles = ((p.M + BM - 1) / BM) * tiles_n * p.split_k;
   // IO = 1 / 3 need every CTA resident at once (tiles wait on flags other CTAs publish): the grid never exceeds the SM count
   if (tiles < grid) grid = tiles;
-  gemm_bf16_kernel<A_MN, B_MN, EPI, IO, TBN><<<grid, kThreads, G::kSmemBytes, stream>>>(ta, tb, tg, tg2, p, pm);
+  gemm_bf16_kernel<A_MN, B_MN, EPI, IO, TBN><<<grid, kThreads, G::kSmemBytes, stream>>>(ta, tb, tg, tg2, p, em, pm);
   cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? 0 : (int)e;
 }
@@ -862,11 +790,12 @@ constexpr int variant(int io, int epi, int a_mn, int b_mn, int wide) { return wi
 // layout for the plain local GEMM, RoPE / SwiGLU on K-major B, SwiGLU backward on MN-major B, each in both tile widths, and
 // K-major A for the collective modes (narrow tiles only).
 int dispatch(int io, int epi, const GemmParams& p, const CUtensorMap& ta, const CUtensorMap& tb, cudaStream_t stream,
-             const PeerMaps* pm = nullptr, const CUtensorMap* tg = nullptr, const CUtensorMap* tg2 = nullptr, bool wide = false) {
+             const EpiMaps* em, const PeerMaps* pm = nullptr, const CUtensorMap* tg = nullptr, const CUtensorMap* tg2 = nullptr,
+             bool wide = false) {
   switch (variant(io, epi, p.a_mn, p.b_mn, wide)) {
 #define PB_GEMM_VARIANT(IO, EPI, A_MN, B_MN, TBN)         \
   case variant(IO, EPI, A_MN, B_MN, TBN == kWideBN):      \
-    return launch<A_MN, B_MN, EPI, IO, TBN>(ta, tb, p, stream, pm, tg, tg2);
+    return launch<A_MN, B_MN, EPI, IO, TBN>(ta, tb, p, stream, em, pm, tg, tg2);
     PB_GEMM_VARIANT(0, 0, 0, 0, BN)
     PB_GEMM_VARIANT(0, 0, 0, 1, BN)
     PB_GEMM_VARIANT(0, 0, 1, 0, BN)
@@ -935,7 +864,7 @@ int check_epilogue(const GemmEpilogue& e, int M, int N, int a_mn, int b_mn, int 
     if ((e.rope_D != 64 && e.rope_D != 128) || e.rope_cols % e.rope_D != 0 || e.rope_cols > N) return -4;
     return 0;
   }
-  // a tile covers 64 features; aux rows are read / written as 16-byte aligned bf16 pairs
+  // a tile covers 64 features; aux is the base of a TMA map (epilogue_maps): 16-byte aligned address and row stride
   if (N % (e.kind == 2 ? 128 : 64) != 0 || e.aux == nullptr || (e.ld_aux % 8) || (reinterpret_cast<uintptr_t>(e.aux) & 15)) return -5;
   if (e.kind == 3 && M <= BM) return -5;
   return 0;
@@ -953,20 +882,8 @@ GemmParams make_params(void* C, int M, int N, int K, int ldc, int a_mn, int b_mn
   p.accumulate = accumulate;
   p.split_k = 1;
   p.C = C;
-  p.rope_cos = e.rope_cos;
-  p.rope_sin = e.rope_sin;
-  p.rope_S = e.rope_S;
-  p.rope_cols = e.rope_cols;
-  p.rope_D = e.rope_D;
-  if (e.kind == 2) {
-    p.swiglu_ff = N / 2;
-    p.H = e.aux;
-    p.ldh = e.ld_aux;
-  } else if (e.kind == 3) {
-    p.swiglu_ff = N;
-    p.aux = e.aux;
-    p.ld_aux = e.ld_aux;
-  }
+  p.epi = e;
+  p.swiglu_ff = e.kind == 2 ? N / 2 : e.kind == 3 ? N : 0;
   return p;
 }
 
@@ -974,6 +891,16 @@ GemmParams make_params(void* C, int M, int N, int K, int ldc, int a_mn, int b_mn
 int operand_tmap(CUtensorMap* m, const void* ptr, int mn, int K, int ld, int mn_major, int box_rows) {
   return mn_major ? pbhost::cached_tmap(m, ptr, (uint64_t)K, (uint64_t)mn, (uint64_t)ld, 64, BK)
                   : pbhost::cached_tmap(m, ptr, (uint64_t)mn, (uint64_t)K, (uint64_t)ld, BK, box_rows);
+}
+
+// The staged epilogue's maps (the entry points' checks and check_epilogue give TMA its 16-byte aligned addresses and row
+// strides): C [M, N] (SwiGLU backward: d_gate_up [M, 2·N]), h [M, FF] for SwiGLU, the saved gate_up [M, 2·N] for SwiGLU backward.
+int epilogue_maps(EpiMaps* em, void* C, int M, int N, int ldc, int c_fp32, const GemmEpilogue& e) {
+  int rc;
+  if ((rc = pbhost::cached_tmap_staging(&em->c, C, M, e.kind == 3 ? 2 * N : N, ldc, c_fp32 != 0))) return rc;
+  if (e.kind == 2 && (rc = pbhost::cached_tmap_staging(&em->h, e.aux, M, N / 2, e.ld_aux, false))) return rc;
+  if (e.kind == 3 && (rc = pbhost::cached_tmap_staging(&em->gu, e.aux, M, 2 * N, e.ld_aux, false))) return rc;
+  return 0;
 }
 
 }  // namespace
@@ -1026,15 +953,11 @@ PB_EXPORT int pb_gemm_bf16(const void* A, const void* B, void* C, int M, int N, 
   } else if ((rc = operand_tmap(&tb, B, N, K, ldb, b_mn_major, e.kind == 2 ? 64 : tbn))) {
     return rc;
   }
-  // the staged epilogue's maps (the checks above and check_epilogue give TMA its 16-byte aligned addresses and row strides):
-  // C [M, N] (SwiGLU backward: d_gate_up [M, 2·N]), h [M, FF] for SwiGLU, the saved gate_up [M, 2·N] for SwiGLU backward
-  PeerMaps om = {};
-  if ((rc = pbhost::cached_tmap_staging(&om.m[0], C, M, e.kind == 3 ? 2 * N : N, ldc, c_fp32 != 0))) return rc;
-  if (e.kind == 2 && (rc = pbhost::cached_tmap_staging(&om.m[1], e.aux, M, N / 2, e.ld_aux, false))) return rc;
-  if (e.kind == 3 && (rc = pbhost::cached_tmap_staging(&om.m[2], e.aux, M, 2 * N, e.ld_aux, false))) return rc;
+  EpiMaps em = {};
+  if ((rc = epilogue_maps(&em, C, M, N, ldc, c_fp32, e))) return rc;
   GemmParams p = make_params(C, M, N, K, ldc, a_mn_major, b_mn_major, c_fp32, accumulate, e);
   if (c_fp32 && accumulate) p.split_k = split_for(((M + BM - 1) / BM) * ((N + tbn - 1) / tbn), (K + BK - 1) / BK);  // plain only
-  return dispatch(0, e.kind, p, ta, tb, stream, &om, wide && e.kind == 2 ? &tup : nullptr, nullptr, wide);
+  return dispatch(0, e.kind, p, ta, tb, stream, &em, nullptr, wide && e.kind == 2 ? &tup : nullptr, nullptr, wide);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------------
@@ -1048,19 +971,12 @@ PB_EXPORT int pb_gemm_allgather(const void* const* a_peers, int n, int rank, con
                                 int M_local, int N, int K, int lda, int ldb, int ldc, int b_mn_major, cudaStream_t stream) {
   if (n < 1 || n > 8 || rank < 0 || rank >= n || M_local % BM != 0) return -6;
   if ((lda % 8) || (ldb % 8) || (ldc % 8) || (K % 8)) return -1;
+  if (reinterpret_cast<uintptr_t>(C) & 15) return -2;
   PeerMaps pm = {};
   pm.n = n;
   pm.rows_per_rank = M_local;
   pm.rank = rank;
   pm.flags = flags;
-  {
-    static int idle = -1;
-    if (idle < 0) {
-      const char* e = getenv("PB_AG_IDLE_ROUNDS");
-      idle = e ? atoi(e) : 2;
-    }
-    pm.idle_rounds = idle;
-  }
   int rc;
   if (n > 1) {
     cudaError_t e = cudaMemsetAsync(flags, 0, sizeof(uint32_t) * (size_t)(n * (M_local / BM)), stream);
@@ -1072,7 +988,9 @@ PB_EXPORT int pb_gemm_allgather(const void* const* a_peers, int n, int rank, con
   CUtensorMap tfull, tb;
   if ((rc = pbhost::cached_tmap(&tfull, a_full, (uint64_t)M, (uint64_t)K, (uint64_t)K, BK, BM))) return rc;
   if ((rc = operand_tmap(&tb, B, N, K, ldb, b_mn_major, BN))) return rc;
-  return dispatch(1, 0, make_params(C, M, N, K, ldc, 0, b_mn_major, 0, 0, kPlain), tfull, tb, stream, &pm);
+  EpiMaps em = {};
+  if ((rc = epilogue_maps(&em, C, M, N, ldc, 0, kPlain))) return rc;
+  return dispatch(1, 0, make_params(C, M, N, K, ldc, 0, b_mn_major, 0, 0, kPlain), tfull, tb, stream, &em, &pm);
 }
 
 // GEMM ⊕ reduce-scatter:  every rank holds a K-shard (A [M, K_local], B [N, K_local]); rank r ends up with rows
@@ -1090,7 +1008,7 @@ PB_EXPORT int pb_gemm_reduce_scatter(const void* A, const void* B, float* const*
   CUtensorMap ta, tb;
   if ((rc = operand_tmap(&ta, A, M, K, lda, 0, BM))) return rc;
   if ((rc = operand_tmap(&tb, B, N, K, ldb, b_mn_major, BN))) return rc;
-  return dispatch(2, 0, make_params(c_peers[rank], M, N, K, ldc, 0, b_mn_major, 1, 1, kPlain), ta, tb, stream, &pm);
+  return dispatch(2, 0, make_params(c_peers[rank], M, N, K, ldc, 0, b_mn_major, 1, 1, kPlain), ta, tb, stream, nullptr, &pm);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------------
@@ -1109,6 +1027,7 @@ PB_EXPORT int pb_gemm_wgather(const void* A, const void* const* w_peers, int n, 
   const GemmEpilogue& e = epi ? *epi : kPlain;
   if (n < 1 || n > 8 || rank < 0 || rank >= n || rowsW % n != 0 || colsW % 64 != 0) return -6;
   if ((lda % 8) || (ldc % 8)) return -1;
+  if (reinterpret_cast<uintptr_t>(C) & 15) return -2;
   const int N = b_mn_major ? colsW : rowsW, K = b_mn_major ? rowsW : colsW;
   int rc;
   if ((rc = check_epilogue(e, M, N, 0, b_mn_major, 0, 0))) return rc;
@@ -1161,12 +1080,8 @@ PB_EXPORT int pb_gemm_wgather(const void* A, const void* const* w_peers, int n, 
   if ((rc = pbhost::cached_tmap_blocks(&tg, w_full, (uint64_t)rpr, (uint64_t)colsW, (uint64_t)n, BK, 128))) return rc;
   if ((rc = operand_tmap(&ta, A, M, K, lda, 0, BM))) return rc;
   if ((rc = operand_tmap(&tb, w_full, N, K, colsW, b_mn_major, e.kind == 2 ? 64 : BN))) return rc;
-  static int group_m = -1;
-  if (group_m < 0) {
-    const char* ev = getenv("PB_WG_GROUP_M");
-    group_m = ev ? atoi(ev) : 0;
-  }
-  GemmParams p = make_params(C, M, N, K, ldc, 0, b_mn_major, 0, 0, e);
-  p.group_m = group_m;
-  return dispatch(3, e.kind, p, ta, tb, stream, &pm, &tg, have_next ? &tg2 : nullptr);
+  EpiMaps em = {};
+  if ((rc = epilogue_maps(&em, C, M, N, ldc, 0, e))) return rc;
+  return dispatch(3, e.kind, make_params(C, M, N, K, ldc, 0, b_mn_major, 0, 0, e), ta, tb, stream, &em, &pm, &tg,
+                  have_next ? &tg2 : nullptr);
 }

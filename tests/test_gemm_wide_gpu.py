@@ -8,7 +8,7 @@ SwiGLU with FF % 128 = 64 (the last wide tile's gate and up halves each half pas
 ending inside a wide tile at D = 64 and D = 128; outputs padded inside a wider buffer, whose padding must stay untouched; fp32 +=
 with a forced split-K.
 
-The CPU tests check the automatic tile policy at the Llama-1B training shapes and at its boundaries, and that no local GEMM
+The CPU tests check the automatic tile policy at the Llama-1B training shapes and at its boundaries, and that no GEMM
 instantiation of the built library has a stack frame or spills (``cuobjdump --dump-resource-usage``)."""
 
 import re
@@ -86,9 +86,9 @@ def test_set_gemm_tile_rejects_unknown_width():
 
 
 @pytest.mark.skipif(shutil.which("cuobjdump") is None or shutil.which("nvcc") is None, reason="CUDA toolkit not installed")
-def test_local_gemm_instantiations_have_no_stack_frame():
-    """Every local (IO = 0) GEMM instantiation, narrow and wide: no stack frame, no local memory. The wide tile's 128 accumulators
-    per consumer thread fit only because the consumers take the producer warpgroup's registers (setmaxnreg)."""
+def test_gemm_instantiations_have_no_stack_frame():
+    """Every GEMM instantiation, local (narrow and wide) and collective: no stack frame, no local memory. The wide tile's 128
+    accumulators per consumer thread fit only because the consumers take the producer warpgroup's registers (setmaxnreg)."""
     from prime_b200.ops import _lib
 
     lib = _lib.build()
@@ -97,12 +97,12 @@ def test_local_gemm_instantiations_have_no_stack_frame():
     lines = out.splitlines()
     for i, line in enumerate(lines):
         m = re.search(r"gemm_bf16_kernelILi(\d)ELi(\d)ELi(\d)ELi(\d)ELi(\d+)E", line)
-        if m and m.group(4) == "0":
+        if m:
             usage = lines[i + 1]
             seen[m.groups()] = usage
             assert "STACK:0 " in usage and "LOCAL:0 " in usage, f"gemm_bf16_kernel<{', '.join(m.groups())}>: {usage.strip()}"
-    assert len(seen) == 14, sorted(seen)  # 7 (layout, epilogue) variants × 2 widths
-    assert {k[4] for k in seen} == {"128", "256"}
+    assert len(seen) == 23, sorted(seen)  # local: 7 (layout, epilogue) variants × 2 widths; collective: 2 + 2 + 5 narrow
+    assert {k[4] for k in seen} == {"128", "256"} and {k[3] for k in seen} == {"0", "1", "2", "3"}
 
 
 # -------------------------------------------------------------------------------------------------- GPU

@@ -31,4 +31,8 @@ run racecheck "gpu and not 5632" racecheck_gemm_wide tests/test_gemm_wide_gpu.py
 run memcheck  "gpu" memcheck_gemm_epilogue tests/test_gemm_epilogue_gpu.py
 run racecheck "gpu" racecheck_gemm_epilogue tests/test_gemm_epilogue_gpu.py
 run synccheck "gpu" synccheck_gemm_epilogue tests/test_gemm_epilogue_gpu.py
+# the collective GEMMs (all-gather, reduce-scatter, weight-gather) on a one-rank group against the local GEMM, bit for bit
+run memcheck  "gpu" memcheck_gemm_collective tests/test_gemm_collective_epilogue_gpu.py
+run racecheck "gpu" racecheck_gemm_collective tests/test_gemm_collective_epilogue_gpu.py
+run synccheck "gpu" synccheck_gemm_collective tests/test_gemm_collective_epilogue_gpu.py
 cat gpurun_out/sanitizer_summary.txt
