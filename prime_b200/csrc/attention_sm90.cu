@@ -19,49 +19,19 @@
 // end = doc_end is its matching upper bound (end[k] = one past the last query that sees key k). pb_doc_bounds builds them for
 // documents of packed rows, a sliding window of W keys (lo[q] = q - W + 1), or both. Key tiles below a query block's first
 // visible key are skipped, not masked.
+#include <type_traits>
+
 #include "common.cuh"
+#include "tc_common.cuh"
 
 namespace {
+
+using namespace tc;
 
 constexpr int kThreads = 128;
 constexpr int BQ = 64;    // forward / dQ query block
 constexpr int BKV = 64;   // key block
 constexpr int BQB = 32;   // query tile of the dK/dV kernel
-
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ float fast_exp2(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() {
-  asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
-}
-__device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t (&r)[4]) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
-               : "r"(addr));
-}
-__device__ __forceinline__ void ldsm_x4_t(uint32_t addr, uint32_t (&r)[4]) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
-               : "r"(addr));
-}
-// D[16x8] += A[16x16] · B[16x8], bf16 in, fp32 accumulate
-__device__ __forceinline__ void mma16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
-               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-__device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
-  const __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
-  return *reinterpret_cast<const uint32_t*>(&v);
-}
 
 // Shared-memory tile of `rows` x D bf16 with a 16-byte pad per row (conflict-free ldmatrix).
 template <int D>
@@ -86,17 +56,32 @@ __device__ __forceinline__ void ld_a(uint32_t base, int row0, int k0, uint32_t (
   const int l = threadIdx.x & 31;
   ldsm_x4(base + (uint32_t)((row0 + (l & 15)) * Tile<D>::kLd + k0 + (l >> 4) * 8) * 2, a);
 }
-// B operands of two n8 blocks (n0, n0 + 8) for k16 at k0, from a tile stored [n][k] (k contiguous): b[0], b[1] | b[2], b[3]
-template <int D>
-__device__ __forceinline__ void ld_b_nk(uint32_t base, int n0, int k0, uint32_t (&b)[4]) {
+
+// Tile products, one k16 step each: acc[n] += A · B[k0 .. k0 + 16, 8n .. 8n + 8] for every n8 block of acc, where A is a 16 x 16
+// fragment (ld_a). Callers step k0 upwards, so every accumulator adds its products in increasing k.
+// B stored [n][k] (k contiguous): the K tile of Q·Kᵀ, the Q tile of K·Qᵀ.
+template <int D, int N8>
+__device__ __forceinline__ void mma_b_nk(float (&acc)[N8][4], const uint32_t (&a)[4], uint32_t b, int k0) {
   const int l = threadIdx.x & 31;
-  ldsm_x4(base + (uint32_t)((n0 + (l & 7) + (l >> 4) * 8) * Tile<D>::kLd + k0 + ((l >> 3) & 1) * 8) * 2, b);
+#pragma unroll
+  for (int n = 0; n < N8; n += 2) {
+    uint32_t bf[4];
+    ldsm_x4(b + (uint32_t)((n * 8 + (l & 7) + (l >> 4) * 8) * Tile<D>::kLd + k0 + ((l >> 3) & 1) * 8) * 2, bf);
+    mma16816(acc[n], a, bf[0], bf[1]);
+    mma16816(acc[n + 1], a, bf[2], bf[3]);
+  }
 }
-// B operands of two n8 blocks (n0, n0 + 8) for k16 at k0, from a tile stored [k][n] (n contiguous)
-template <int D>
-__device__ __forceinline__ void ld_b_kn(uint32_t base, int n0, int k0, uint32_t (&b)[4]) {
+// B stored [k][n] (n contiguous): the V tile of P·V, the K tile of dS·K.
+template <int D, int N8>
+__device__ __forceinline__ void mma_b_kn(float (&acc)[N8][4], const uint32_t (&a)[4], uint32_t b, int k0) {
   const int l = threadIdx.x & 31;
-  ldsm_x4_t(base + (uint32_t)((k0 + (l & 7) + ((l >> 3) & 1) * 8) * Tile<D>::kLd + n0 + (l >> 4) * 8) * 2, b);
+#pragma unroll
+  for (int n = 0; n < N8; n += 2) {
+    uint32_t bf[4];
+    ldsm_x4_t(b + (uint32_t)((k0 + (l & 7) + ((l >> 3) & 1) * 8) * Tile<D>::kLd + n * 8 + (l >> 4) * 8) * 2, bf);
+    mma16816(acc[n], a, bf[0], bf[1]);
+    mma16816(acc[n + 1], a, bf[2], bf[3]);
+  }
 }
 
 struct AttnParams {
@@ -116,89 +101,116 @@ struct AttnParams {
   const int* doc_end;    //                     int32 [B, S] end[s], one past the last query that sees key s
 };
 
+// One batch row of the fused [B, S, (H + 2·Hkv)·D] activation (qkv, or its gradient dqkv): the Q head h, K head hk and V head hk
+// of token s.
+template <int D, typename T>
+struct FusedRow {
+  T* row;  // token 0
+  int W;   // elements per token
+  int H, Hkv;
+  __device__ FusedRow(T* x, const AttnParams& p, int b)
+      : row(x + (int64_t)b * p.S * ((p.H + 2 * p.Hkv) * D)), W((p.H + 2 * p.Hkv) * D), H(p.H), Hkv(p.Hkv) {}
+  __device__ T* q(int s, int h) const { return row + (int64_t)s * W + h * D; }
+  __device__ T* k(int s, int hk) const { return q(s, H + hk); }
+  __device__ T* v(int s, int hk) const { return q(s, H + Hkv + hk); }
+};
+
+// Which keys the queries of one batch row see: all of them when not causal, k <= q when causal, and lo[q] <= k <= q under kDoc
+// (which implies causal). lo never decreases along a row and end is its matching upper bound, so the keys a block of queries sees
+// and the queries that see a block of keys are contiguous tile ranges: the kernels skip the tiles outside them, and only edge
+// tiles pay for the per-element predicate. Built once per block; kDoc = false never reads the bounds.
+template <bool kDoc>
+struct Visibility {
+  const int* lo;  // kDoc: doc_start of the row
+  bool causal;
+  int first, end;  // the tiles the block visits: key tiles of a query block, query tiles of a key block
+  int qb;          // query block: its index, whose key tile holds the diagonal
+  int lo_last;     // query block, kDoc: lo of its last query; key tiles below it hold keys some query of the block does not see
+
+  // 64-key tiles [first, end) that 64-query block qb sees something of
+  __device__ static Visibility query_block(const AttnParams& p, int b, int qb) {
+    Visibility v{kDoc ? p.doc_start + (int64_t)b * p.S : nullptr, p.causal != 0};
+    v.qb = qb;
+    v.first = kDoc ? v.lo[qb * BQ] / BKV : 0;
+    v.end = p.causal ? qb + 1 : p.S / BKV;
+    v.lo_last = kDoc ? v.lo[qb * BQ + BQ - 1] : 0;
+    return v;
+  }
+  // 32-query tiles [first, end) that see something of 64-key block kb (end stops at the tile holding end[last key of the block])
+  __device__ static Visibility key_block(const AttnParams& p, int b, int kb) {
+    Visibility v{kDoc ? p.doc_start + (int64_t)b * p.S : nullptr, p.causal != 0};
+    v.first = p.causal ? kb * BKV / BQB : 0;
+    v.end = kDoc ? (p.doc_end[(int64_t)b * p.S + kb * BKV + BKV - 1] + BQB - 1) / BQB : p.S / BQB;
+    return v;
+  }
+  __device__ int lo_of(int q) const { return kDoc ? lo[q] : 0; }
+  // query block: key tile j is the diagonal tile or lies below lo_last
+  __device__ bool masked(int j) const { return causal && (j == qb || (kDoc && j * BKV < lo_last)); }
+  // query q sees key k; lo_q = lo_of(q), which the kernels keep in registers or shared memory
+  __device__ bool sees(int q, int k, int lo_q) const { return kDoc ? lo_q <= k && k <= q : !causal || k <= q; }
+};
+
 // ------------------------------------------------------------------------------------------------------------------ forward
-// kDoc: lower-bounded causal masking. Query q sees key k iff lo[q] <= k <= q (lo = doc_start). lo never decreases along a row,
-// so the key loop starts at the tile of lo[q0]; only tiles below lo[q0 + BQ - 1] and the diagonal tile need a mask, the others
-// take the plain path.
+// The key loop starts at Visibility::first, whose tile the first cp.async prefetch loads.
 template <int D, bool kDoc>
 __global__ void __launch_bounds__(kThreads) flash_fwd_kernel(const AttnParams p) {
   extern __shared__ __align__(128) uint8_t smem[];
   const int qb = (int)blockIdx.x, bh = (int)blockIdx.y;
   const int b = bh / p.H, h = bh - b * p.H, hk = h / (p.H / p.Hkv);
-  const int W = (p.H + 2 * p.Hkv) * D;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
-  const __nv_bfloat16* base = p.qkv + (int64_t)b * p.S * W;
+  const FusedRow<D, const __nv_bfloat16> x(p.qkv, p, b);
   const uint32_t sq = smem_u32(smem);
   const uint32_t skv = sq + Tile<D>::bytes(BQ);  // [stage][K | V]
   constexpr uint32_t kKV = Tile<D>::bytes(BKV);
 
   const int q0 = qb * BQ;
-  const int n_kv = p.causal ? qb + 1 : p.S / BKV;
-  // kDoc: first key tile, document start of the block's last row, document starts of this thread's two rows
-  const int* ds = kDoc ? p.doc_start + (int64_t)b * p.S : nullptr;
-  const int j0 = kDoc ? ds[q0] / BKV : 0;
-  const int ds_max = kDoc ? ds[q0 + BQ - 1] : 0;
-  const int rds[2] = {kDoc ? ds[q0 + warp * 16 + g] : 0, kDoc ? ds[q0 + warp * 16 + g + 8] : 0};
-  load_tile<D>(sq, base + (int64_t)q0 * W + h * D, W, BQ);
-  load_tile<D>(skv, base + (int64_t)j0 * BKV * W + p.H * D + hk * D, W, BKV);
-  load_tile<D>(skv + kKV, base + (int64_t)j0 * BKV * W + (p.H + p.Hkv) * D + hk * D, W, BKV);
+  const auto vis = Visibility<kDoc>::query_block(p, b, qb);
+  const int rlo[2] = {vis.lo_of(q0 + warp * 16 + g), vis.lo_of(q0 + warp * 16 + g + 8)};  // this thread's two rows
+  load_tile<D>(sq, x.q(q0, h), x.W, BQ);
+  load_tile<D>(skv, x.k(vis.first * BKV, hk), x.W, BKV);
+  load_tile<D>(skv + kKV, x.v(vis.first * BKV, hk), x.W, BKV);
   cp_async_commit();
 
   uint32_t qf[D / 16][4];
-  float o[D / 8][4];
-#pragma unroll
-  for (int i = 0; i < D / 8; ++i) o[i][0] = o[i][1] = o[i][2] = o[i][3] = 0.f;
+  float o[D / 8][4] = {};
   float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
 
-  for (int j = j0; j < n_kv; ++j) {
-    const int st = (j - j0) & 1;
-    if (j + 1 < n_kv) {  // prefetch the next key/value tile into the other stage
+  for (int j = vis.first; j < vis.end; ++j) {
+    const int st = (j - vis.first) & 1;
+    if (j + 1 < vis.end) {  // prefetch the next key/value tile into the other stage
       const int k1 = (j + 1) * BKV;
       const uint32_t nxt = skv + (st ^ 1) * 2 * kKV;
-      load_tile<D>(nxt, base + (int64_t)k1 * W + p.H * D + hk * D, W, BKV);
-      load_tile<D>(nxt + kKV, base + (int64_t)k1 * W + (p.H + p.Hkv) * D + hk * D, W, BKV);
+      load_tile<D>(nxt, x.k(k1, hk), x.W, BKV);
+      load_tile<D>(nxt + kKV, x.v(k1, hk), x.W, BKV);
     }
     cp_async_commit();
     cp_async_wait<1>();
     __syncthreads();
-    if (j == j0) {
+    if (j == vis.first) {
 #pragma unroll
       for (int kk = 0; kk < D / 16; ++kk) ld_a<D>(sq, warp * 16, kk * 16, qf[kk]);
     }
     const uint32_t sk = skv + st * 2 * kKV, sv = sk + kKV;
-    float s[BKV / 8][4];
+    float s[BKV / 8][4] = {};
 #pragma unroll
-    for (int n = 0; n < BKV / 8; ++n) s[n][0] = s[n][1] = s[n][2] = s[n][3] = 0.f;
-#pragma unroll
-    for (int kk = 0; kk < D / 16; ++kk) {
-#pragma unroll
-      for (int n = 0; n < BKV / 8; n += 2) {
-        uint32_t bf[4];
-        ld_b_nk<D>(sk, n * 8, kk * 16, bf);
-        mma16816(s[n], qf[kk], bf[0], bf[1]);
-        mma16816(s[n + 1], qf[kk], bf[2], bf[3]);
-      }
-    }
+    for (int kk = 0; kk < D / 16; ++kk) mma_b_nk<D>(s, qf[kk], sk, kk * 16);
     // online softmax (log2 domain); rows g and g + 8 of this warp's 16
-    const bool diag = p.causal && j == qb;
-    const bool edge = kDoc && (diag || j * BKV < ds_max);
+    const bool masked = vis.masked(j);
     float mx[2] = {m[0], m[1]};
 #pragma unroll
     for (int n = 0; n < BKV / 8; ++n)
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
+        const int r = e >> 1;
         float v = s[n][e] * p.scale_log2;
-        if constexpr (kDoc) {
-          if (edge) {
-            const int qi = q0 + warp * 16 + g + (e >> 1) * 8, ki = j * BKV + n * 8 + 2 * t + (e & 1);
-            if (ki > qi || ki < rds[e >> 1]) v = -INFINITY;
-          }
-        } else if (diag) {
-          const int qi = warp * 16 + g + (e >> 1) * 8, ki = n * 8 + 2 * t + (e & 1);
-          if (ki > qi) v = -INFINITY;
+        if (masked) {
+          const int qi = warp * 16 + g + r * 8, ki = n * 8 + 2 * t + (e & 1);
+          // plain causal masks the diagonal tile only, where positions within the tile compare as token positions do. They do not
+          // change with j; from token positions, the plain D = 128 forward compiles to 50 fewer registers and runs ~15 % slower.
+          if (!(kDoc ? vis.sees(q0 + qi, j * BKV + ki, rlo[r]) : vis.sees(qi, ki, 0))) v = -INFINITY;
         }
         s[n][e] = v;
-        mx[e >> 1] = fmaxf(mx[e >> 1], v);
+        mx[r] = fmaxf(mx[r], v);
       }
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
@@ -243,15 +255,7 @@ __global__ void __launch_bounds__(kThreads) flash_fwd_kernel(const AttnParams p)
       o[i][3] *= corr[1];
     }
 #pragma unroll
-    for (int kk = 0; kk < BKV / 16; ++kk) {
-#pragma unroll
-      for (int n = 0; n < D / 8; n += 2) {
-        uint32_t bf[4];
-        ld_b_kn<D>(sv, n * 8, kk * 16, bf);
-        mma16816(o[n], pf[kk], bf[0], bf[1]);
-        mma16816(o[n + 1], pf[kk], bf[2], bf[3]);
-      }
-    }
+    for (int kk = 0; kk < BKV / 16; ++kk) mma_b_kn<D>(o, pf[kk], sv, kk * 16);
     __syncthreads();  // this stage is refilled by the prefetch of iteration j + 1
   }
 #pragma unroll
@@ -303,15 +307,14 @@ __global__ void __launch_bounds__(256) bwd_delta_kernel(const pb::bf16x8* __rest
   }
 }
 
-// store a 16-row x D fp32 accumulator (mma C layout) as bf16 into rows [row0, row0 + 16) of a [.., ld] buffer at column col0,
-// optionally un-rotating the interleaved RoPE pairs (position = sequence index of the row)
+// store a 16-row x D fp32 accumulator (mma C layout) as bf16 into the 16 rows from dst on (row stride ld; token s0 first),
+// optionally un-rotating the interleaved RoPE pairs (position = token)
 template <int D>
-__device__ __forceinline__ void store_rows(__nv_bfloat16* dst, int64_t ld, int row0, int s0, float (&acc)[D / 8][4], const AttnParams& p,
-                                           bool rope) {
+__device__ __forceinline__ void store_rows(__nv_bfloat16* dst, int64_t ld, int s0, float (&acc)[D / 8][4], const AttnParams& p, bool rope) {
   const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
 #pragma unroll
   for (int r = 0; r < 2; ++r) {
-    const int row = row0 + g + r * 8, pos = s0 + g + r * 8;
+    const int row = g + r * 8, pos = s0 + row;
 #pragma unroll
     for (int n = 0; n < D / 8; ++n) {
       float a = acc[n][2 * r], c = acc[n][2 * r + 1];
@@ -327,72 +330,52 @@ __device__ __forceinline__ void store_rows(__nv_bfloat16* dst, int64_t ld, int r
   }
 }
 
-// kDoc: the query-tile loop stops at the tile holding end[b, k0 + BKV - 1] (end never decreases, so no later query sees a key of
-// this block) and Pᵀ is zero unless lo[q] <= key <= q; the tile's lo values are staged in shared memory after lse2 and delta.
+// The query-tile loop covers Visibility::key_block; the tile's lo values are staged in shared memory after lse2 and delta.
 template <int D, bool kDoc>
 __global__ void __launch_bounds__(kThreads) bwd_dkdv_kernel(const AttnParams p) {
   extern __shared__ __align__(128) uint8_t smem[];
   const int kb = (int)blockIdx.x, bhk = (int)blockIdx.y;
   const int b = bhk / p.Hkv, hk = bhk - b * p.Hkv, grp = p.H / p.Hkv;
-  const int W = (p.H + 2 * p.Hkv) * D;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
-  const __nv_bfloat16* base = p.qkv + (int64_t)b * p.S * W;
+  const FusedRow<D, const __nv_bfloat16> x(p.qkv, p, b);
   const __nv_bfloat16* dbase = p.dout + (int64_t)b * p.S * (p.H * D);
   const uint32_t sk = smem_u32(smem), sv = sk + Tile<D>::bytes(BKV);
   const uint32_t sq = sv + Tile<D>::bytes(BKV), sdo = sq + Tile<D>::bytes(BQB);
   float* s_ld = reinterpret_cast<float*>(smem + 2 * Tile<D>::bytes(BKV) + 2 * Tile<D>::bytes(BQB));  // [lse2 BQB | delta BQB]
-  int* s_ds = reinterpret_cast<int*>(s_ld + 2 * BQB);  // kDoc: [doc_start BQB]
+  int* s_lo = reinterpret_cast<int*>(s_ld + 2 * BQB);  // kDoc: [lo BQB]
   const int k0 = kb * BKV;
-  load_tile<D>(sk, base + (int64_t)k0 * W + (p.H + hk) * D, W, BKV);
-  load_tile<D>(sv, base + (int64_t)k0 * W + (p.H + p.Hkv + hk) * D, W, BKV);
+  load_tile<D>(sk, x.k(k0, hk), x.W, BKV);
+  load_tile<D>(sv, x.v(k0, hk), x.W, BKV);
   cp_async_commit();
 
-  float dk[D / 8][4], dv[D / 8][4];
-#pragma unroll
-  for (int i = 0; i < D / 8; ++i)
-#pragma unroll
-    for (int e = 0; e < 4; ++e) dk[i][e] = dv[i][e] = 0.f;
-
-  const int qt0 = p.causal ? k0 / BQB : 0;
-  const int qt_doc = kDoc ? (p.doc_end[(int64_t)b * p.S + k0 + BKV - 1] + BQB - 1) / BQB : 0;
+  float dk[D / 8][4] = {}, dv[D / 8][4] = {};
+  const auto vis = Visibility<kDoc>::key_block(p, b, kb);
   for (int hh = 0; hh < grp; ++hh) {
     const int h = hk * grp + hh;
-    for (int qt = qt0; qt < (kDoc ? qt_doc : p.S / BQB); ++qt) {
+    for (int qt = vis.first; qt < vis.end; ++qt) {
       const int q0 = qt * BQB;
       __syncthreads();  // the previous tile has been consumed
-      load_tile<D>(sq, base + (int64_t)q0 * W + h * D, W, BQB);
+      load_tile<D>(sq, x.q(q0, h), x.W, BQB);
       load_tile<D>(sdo, dbase + (int64_t)q0 * (p.H * D) + h * D, p.H * D, BQB);
       cp_async_commit();
       if (threadIdx.x < BQB) s_ld[threadIdx.x] = p.lse2[((int64_t)b * p.H + h) * p.S + q0 + threadIdx.x];
       else if (threadIdx.x < 2 * BQB) s_ld[threadIdx.x] = p.delta[((int64_t)b * p.H + h) * p.S + q0 + threadIdx.x - BQB];
       if constexpr (kDoc) {
-        if (threadIdx.x >= 2 * BQB && threadIdx.x < 3 * BQB) s_ds[threadIdx.x - 2 * BQB] = p.doc_start[(int64_t)b * p.S + q0 + threadIdx.x - 2 * BQB];
+        if (threadIdx.x >= 2 * BQB && threadIdx.x < 3 * BQB) s_lo[threadIdx.x - 2 * BQB] = vis.lo_of(q0 + threadIdx.x - 2 * BQB);
       }
       cp_async_wait<0>();
       __syncthreads();
       // Sᵀ = K Qᵀ and dPᵀ = V dOᵀ: 16 keys (this warp) x BQB queries
-      float st[BQB / 8][4], dpt[BQB / 8][4];
-#pragma unroll
-      for (int n = 0; n < BQB / 8; ++n)
-#pragma unroll
-        for (int e = 0; e < 4; ++e) st[n][e] = dpt[n][e] = 0.f;
+      float st[BQB / 8][4] = {}, dpt[BQB / 8][4] = {};
 #pragma unroll
       for (int kk = 0; kk < D / 16; ++kk) {
         uint32_t ka[4], va[4];
         ld_a<D>(sk, warp * 16, kk * 16, ka);
         ld_a<D>(sv, warp * 16, kk * 16, va);
-#pragma unroll
-        for (int n = 0; n < BQB / 8; n += 2) {
-          uint32_t bq[4], bo[4];
-          ld_b_nk<D>(sq, n * 8, kk * 16, bq);
-          ld_b_nk<D>(sdo, n * 8, kk * 16, bo);
-          mma16816(st[n], ka, bq[0], bq[1]);
-          mma16816(st[n + 1], ka, bq[2], bq[3]);
-          mma16816(dpt[n], va, bo[0], bo[1]);
-          mma16816(dpt[n + 1], va, bo[2], bo[3]);
-        }
+        mma_b_nk<D>(st, ka, sq, kk * 16);
+        mma_b_nk<D>(dpt, va, sdo, kk * 16);
       }
-      // Pᵀ = exp2(s·scale·log2e − lse2[q]) (0 where q < key), dSᵀ = Pᵀ ∘ (dPᵀ·scale − delta·scale)
+      // Pᵀ = exp2(s·scale·log2e − lse2[q]) (0 where q does not see the key), dSᵀ = Pᵀ ∘ (dPᵀ·scale − delta·scale)
       uint32_t pa[BQB / 16][4], da[BQB / 16][4];
 #pragma unroll
       for (int n = 0; n < BQB / 8; ++n) {
@@ -401,11 +384,7 @@ __global__ void __launch_bounds__(kThreads) bwd_dkdv_kernel(const AttnParams p) 
         for (int e = 0; e < 4; ++e) {
           const int qi = n * 8 + 2 * t + (e & 1), ki = k0 + warp * 16 + g + (e >> 1) * 8;
           float pe = fast_exp2(st[n][e] * p.scale_log2 - s_ld[qi]);
-          if constexpr (kDoc) {
-            if (q0 + qi < ki || s_ds[qi] > ki) pe = 0.f;
-          } else if (p.causal && q0 + qi < ki) {
-            pe = 0.f;
-          }
+          if (!vis.sees(q0 + qi, ki, kDoc ? s_lo[qi] : 0)) pe = 0.f;
           pv[e] = pe;
           dsv[e] = pe * (dpt[n][e] * p.scale - s_ld[BQB + qi]);
         }
@@ -417,37 +396,29 @@ __global__ void __launch_bounds__(kThreads) bwd_dkdv_kernel(const AttnParams p) 
       // dV += Pᵀ dO, dK += dSᵀ Q  (k = queries)
 #pragma unroll
       for (int kk = 0; kk < BQB / 16; ++kk) {
-#pragma unroll
-        for (int n = 0; n < D / 8; n += 2) {
-          uint32_t bo[4], bq[4];
-          ld_b_kn<D>(sdo, n * 8, kk * 16, bo);
-          ld_b_kn<D>(sq, n * 8, kk * 16, bq);
-          mma16816(dv[n], pa[kk], bo[0], bo[1]);
-          mma16816(dv[n + 1], pa[kk], bo[2], bo[3]);
-          mma16816(dk[n], da[kk], bq[0], bq[1]);
-          mma16816(dk[n + 1], da[kk], bq[2], bq[3]);
-        }
+        mma_b_kn<D>(dv, pa[kk], sdo, kk * 16);
+        mma_b_kn<D>(dk, da[kk], sq, kk * 16);
       }
     }
   }
-  __nv_bfloat16* dst = p.dqkv + (int64_t)b * p.S * W;
-  store_rows<D>(dst + (p.H + hk) * D, W, k0 + warp * 16, k0 + warp * 16, dk, p, p.rope_cos != nullptr);
-  store_rows<D>(dst + (p.H + p.Hkv + hk) * D, W, k0 + warp * 16, k0 + warp * 16, dv, p, false);
+  const FusedRow<D, __nv_bfloat16> dx(p.dqkv, p, b);
+  const int s0 = k0 + warp * 16;
+  store_rows<D>(dx.k(s0, hk), dx.W, s0, dk, p, p.rope_cos != nullptr);
+  store_rows<D>(dx.v(s0, hk), dx.W, s0, dv, p, false);
 }
 
-// kDoc: key tiles from lo[b, q0] / BKV to the diagonal, masks as in the forward
+// The key loop covers Visibility::query_block, masked as in the forward.
 template <int D, bool kDoc>
 __global__ void __launch_bounds__(kThreads) bwd_dq_kernel(const AttnParams p) {
   extern __shared__ __align__(128) uint8_t smem[];
   const int qb = (int)blockIdx.x, bh = (int)blockIdx.y;
   const int b = bh / p.H, h = bh - b * p.H, hk = h / (p.H / p.Hkv);
-  const int W = (p.H + 2 * p.Hkv) * D;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
-  const __nv_bfloat16* base = p.qkv + (int64_t)b * p.S * W;
+  const FusedRow<D, const __nv_bfloat16> x(p.qkv, p, b);
   const uint32_t sq = smem_u32(smem), sdo = sq + Tile<D>::bytes(BQ);
   const uint32_t sk = sdo + Tile<D>::bytes(BQ), sv = sk + Tile<D>::bytes(BKV);
   const int q0 = qb * BQ;
-  load_tile<D>(sq, base + (int64_t)q0 * W + h * D, W, BQ);
+  load_tile<D>(sq, x.q(q0, h), x.W, BQ);
   load_tile<D>(sdo, p.dout + ((int64_t)b * p.S + q0) * (p.H * D) + h * D, p.H * D, BQ);
   cp_async_commit();
   float lse[2], del[2];
@@ -457,43 +428,26 @@ __global__ void __launch_bounds__(kThreads) bwd_dq_kernel(const AttnParams p) {
     lse[r] = p.lse2[i];
     del[r] = p.delta[i];
   }
-  float dq[D / 8][4];
-#pragma unroll
-  for (int i = 0; i < D / 8; ++i) dq[i][0] = dq[i][1] = dq[i][2] = dq[i][3] = 0.f;
-  const int n_kv = p.causal ? qb + 1 : p.S / BKV;
-  const int* ds = kDoc ? p.doc_start + (int64_t)b * p.S : nullptr;
-  const int j0 = kDoc ? ds[q0] / BKV : 0;
-  const int ds_max = kDoc ? ds[q0 + BQ - 1] : 0;
-  const int rds[2] = {kDoc ? ds[q0 + warp * 16 + g] : 0, kDoc ? ds[q0 + warp * 16 + g + 8] : 0};
-  for (int j = j0; j < n_kv; ++j) {
+  float dq[D / 8][4] = {};
+  const auto vis = Visibility<kDoc>::query_block(p, b, qb);
+  const int rlo[2] = {vis.lo_of(q0 + warp * 16 + g), vis.lo_of(q0 + warp * 16 + g + 8)};
+  for (int j = vis.first; j < vis.end; ++j) {
     const int k0 = j * BKV;
-    const bool edge = kDoc && (j == qb || k0 < ds_max);
+    const bool masked = vis.masked(j);
     __syncthreads();
-    load_tile<D>(sk, base + (int64_t)k0 * W + (p.H + hk) * D, W, BKV);
-    load_tile<D>(sv, base + (int64_t)k0 * W + (p.H + p.Hkv + hk) * D, W, BKV);
+    load_tile<D>(sk, x.k(k0, hk), x.W, BKV);
+    load_tile<D>(sv, x.v(k0, hk), x.W, BKV);
     cp_async_commit();
     cp_async_wait<0>();
     __syncthreads();
-    float s[BKV / 8][4], dp[BKV / 8][4];
-#pragma unroll
-    for (int n = 0; n < BKV / 8; ++n)
-#pragma unroll
-      for (int e = 0; e < 4; ++e) s[n][e] = dp[n][e] = 0.f;
+    float s[BKV / 8][4] = {}, dp[BKV / 8][4] = {};
 #pragma unroll
     for (int kk = 0; kk < D / 16; ++kk) {
       uint32_t qa[4], oa[4];
       ld_a<D>(sq, warp * 16, kk * 16, qa);
       ld_a<D>(sdo, warp * 16, kk * 16, oa);
-#pragma unroll
-      for (int n = 0; n < BKV / 8; n += 2) {
-        uint32_t bk[4], bv[4];
-        ld_b_nk<D>(sk, n * 8, kk * 16, bk);
-        ld_b_nk<D>(sv, n * 8, kk * 16, bv);
-        mma16816(s[n], qa, bk[0], bk[1]);
-        mma16816(s[n + 1], qa, bk[2], bk[3]);
-        mma16816(dp[n], oa, bv[0], bv[1]);
-        mma16816(dp[n + 1], oa, bv[2], bv[3]);
-      }
+      mma_b_nk<D>(s, qa, sk, kk * 16);
+      mma_b_nk<D>(dp, oa, sv, kk * 16);
     }
     uint32_t da[BKV / 16][4];
 #pragma unroll
@@ -503,11 +457,7 @@ __global__ void __launch_bounds__(kThreads) bwd_dq_kernel(const AttnParams p) {
       for (int e = 0; e < 4; ++e) {
         const int r = e >> 1, qi = q0 + warp * 16 + g + r * 8, ki = k0 + n * 8 + 2 * t + (e & 1);
         float pe = fast_exp2(s[n][e] * p.scale_log2 - lse[r]);
-        if constexpr (kDoc) {
-          if (edge && (ki > qi || ki < rds[r])) pe = 0.f;
-        } else if (p.causal && ki > qi) {
-          pe = 0.f;
-        }
+        if (masked && !vis.sees(qi, ki, rlo[r])) pe = 0.f;
         dsv[e] = pe * (dp[n][e] * p.scale - del[r]);
       }
       da[n >> 1][(n & 1) * 2] = pack_bf16(dsv[0], dsv[1]);
@@ -515,17 +465,10 @@ __global__ void __launch_bounds__(kThreads) bwd_dq_kernel(const AttnParams p) {
     }
     // dQ += dS K  (k = keys)
 #pragma unroll
-    for (int kk = 0; kk < BKV / 16; ++kk) {
-#pragma unroll
-      for (int n = 0; n < D / 8; n += 2) {
-        uint32_t bk[4];
-        ld_b_kn<D>(sk, n * 8, kk * 16, bk);
-        mma16816(dq[n], da[kk], bk[0], bk[1]);
-        mma16816(dq[n + 1], da[kk], bk[2], bk[3]);
-      }
-    }
+    for (int kk = 0; kk < BKV / 16; ++kk) mma_b_kn<D>(dq, da[kk], sk, kk * 16);
   }
-  store_rows<D>(p.dqkv + (int64_t)b * p.S * W + h * D, W, q0 + warp * 16, q0 + warp * 16, dq, p, p.rope_cos != nullptr);
+  const FusedRow<D, __nv_bfloat16> dx(p.dqkv, p, b);
+  store_rows<D>(dx.q(q0 + warp * 16, h), dx.W, q0 + warp * 16, dq, p, p.rope_cos != nullptr);
 }
 
 template <typename K>
@@ -559,6 +502,27 @@ int launch_bwd(const AttnParams& p, cudaStream_t stream) {
   bwd_dq_kernel<D, kDoc><<<dim3(p.S / BQ, p.B * p.H), kThreads, kDq, stream>>>(p);
   PB_CHECK_LAUNCH();
   return 0;
+}
+
+// launch(D, kDoc), both as std::integral_constant, for D ∈ {64, 128}; -2 for any other D
+template <typename Launch>
+int dispatch(int D, bool doc, Launch launch) {
+  using D64 = std::integral_constant<int, 64>;
+  using D128 = std::integral_constant<int, 128>;
+  if (D == 128) return doc ? launch(D128(), std::true_type()) : launch(D128(), std::false_type());
+  if (D == 64) return doc ? launch(D64(), std::true_type()) : launch(D64(), std::false_type());
+  return -2;
+}
+
+// the fields both entry points set; the others stay null
+AttnParams shared_params(const void* qkv, const int* doc_start, int B, int S, int H, int Hkv, float scale, int causal) {
+  AttnParams p{};
+  p.qkv = (const __nv_bfloat16*)qkv;
+  p.doc_start = doc_start;
+  p.B = B, p.S = S, p.H = H, p.Hkv = Hkv;
+  p.scale = scale, p.scale_log2 = scale * 1.4426950408889634f;
+  p.causal = causal;
+  return p;
 }
 
 // Document bounds of packed rows: one CTA per row. Every thread owns a contiguous run of positions; a block-wide exclusive
@@ -611,16 +575,11 @@ __global__ void __launch_bounds__(kBoundsThreads) doc_bounds_kernel(const int64_
 PB_EXPORT int pb_flash_attn_fwd(const void* qkv, void* out, float* lse2, const int* doc_start, int B, int S, int H, int Hkv, int D,
                                 float scale, int causal, cudaStream_t stream) {
   if (S % 128 != 0 || H % Hkv != 0 || (doc_start != nullptr && !causal)) return -1;
-  AttnParams p{(const __nv_bfloat16*)qkv, (__nv_bfloat16*)out, nullptr, nullptr, nullptr, nullptr, lse2,
-               B, S, H, Hkv, scale, scale * 1.4426950408889634f, causal, nullptr, nullptr, doc_start, nullptr};
-  if (doc_start != nullptr) {
-    if (D == 128) return launch_fwd<128, true>(p, stream);
-    if (D == 64) return launch_fwd<64, true>(p, stream);
-    return -2;
-  }
-  if (D == 128) return launch_fwd<128, false>(p, stream);
-  if (D == 64) return launch_fwd<64, false>(p, stream);
-  return -2;
+  AttnParams p = shared_params(qkv, doc_start, B, S, H, Hkv, scale, causal);
+  p.out = (__nv_bfloat16*)out;
+  p.lse2_out = lse2;
+  return dispatch(D, doc_start != nullptr,
+                  [&](auto d, auto doc) { return launch_fwd<decltype(d)::value, decltype(doc)::value>(p, stream); });
 }
 
 // delta: [B, H, S] fp32 scratch.  dqkv: [B, S, (H+2Hkv)·D] bf16, fully overwritten.
@@ -630,16 +589,16 @@ PB_EXPORT int pb_flash_attn_bwd(const void* qkv, const void* out, const void* do
                                 const int* doc_start, const int* doc_end, int B, int S, int H, int Hkv, int D, float scale, int causal,
                                 const float* rope_cos, const float* rope_sin, cudaStream_t stream) {
   if (S % 128 != 0 || H % Hkv != 0 || (doc_start == nullptr) != (doc_end == nullptr) || (doc_start != nullptr && !causal)) return -1;
-  AttnParams p{(const __nv_bfloat16*)qkv, (__nv_bfloat16*)out, (const __nv_bfloat16*)dout, (__nv_bfloat16*)dqkv, lse2, delta, nullptr,
-               B, S, H, Hkv, scale, scale * 1.4426950408889634f, causal, rope_cos, rope_sin, doc_start, doc_end};
-  if (doc_start != nullptr) {
-    if (D == 128) return launch_bwd<128, true>(p, stream);
-    if (D == 64) return launch_bwd<64, true>(p, stream);
-    return -2;
-  }
-  if (D == 128) return launch_bwd<128, false>(p, stream);
-  if (D == 64) return launch_bwd<64, false>(p, stream);
-  return -2;
+  AttnParams p = shared_params(qkv, doc_start, B, S, H, Hkv, scale, causal);
+  p.out = (__nv_bfloat16*)out;
+  p.dout = (const __nv_bfloat16*)dout;
+  p.dqkv = (__nv_bfloat16*)dqkv;
+  p.lse2 = lse2;
+  p.delta = delta;
+  p.rope_cos = rope_cos, p.rope_sin = rope_sin;
+  p.doc_end = doc_end;
+  return dispatch(D, doc_start != nullptr,
+                  [&](auto d, auto doc) { return launch_bwd<decltype(d)::value, decltype(doc)::value>(p, stream); });
 }
 
 // tokens int64 [B, S] → doc_start, doc_end int32 [B, S], the lo / end bounds of pb_flash_attn_fwd / _bwd. Position s starts a

@@ -16,8 +16,11 @@
 #include <algorithm>
 
 #include "common.cuh"
+#include "tc_common.cuh"
 
 namespace {
+
+using namespace tc;
 
 constexpr int BM = 128, BN = 64, BKB = 128;  // BKB: K elements (= bytes) per stage
 constexpr int kThreads = 128;
@@ -35,11 +38,6 @@ __device__ __forceinline__ size_t sf_offset(int r, int kblk, int atoms_r) {
   return ((size_t)(kblk >> 2) * atoms_r + (r >> 7)) * 512 + (size_t)((r & 31) * 16 + ((r & 127) >> 5) * 4 + (kblk & 3));
 }
 
-__device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t (&r)[4]) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
-               : "r"(addr));
-}
 __device__ __forceinline__ void mma_e4m3(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
   asm volatile("mma.sync.aligned.m16n8k32.row.col.f32.e4m3.e4m3.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
                : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
@@ -56,13 +54,13 @@ __global__ void __launch_bounds__(kThreads) gemm_mxfp8_kernel(const uint8_t* __r
   // rows past M / N are clamped to the last row: they only feed accumulator rows / columns that are never stored
   auto load = [&](int kt, int st) {
     uint8_t* base = smem + st * kStageBytes;
-    const uint32_t sbase = (uint32_t)__cvta_generic_to_shared(base);
+    const uint32_t sbase = smem_u32(base);
     for (int i = threadIdx.x; i < (BM + BN) * (BKB / 16); i += kThreads) {
       const int r = i / (BKB / 16), c = i % (BKB / 16);
       const uint8_t* src = r < BM ? A + (int64_t)min(m0 + r, p.M - 1) * p.K : B + (int64_t)min(n0 + r - BM, p.N - 1) * p.K;
-      asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(sbase + r * kLd + c * 16), "l"(src + kt * BKB + c * 16) : "memory");
+      cp_async16(sbase + r * kLd + c * 16, src + kt * BKB + c * 16);
     }
-    asm volatile("cp.async.commit_group;" ::: "memory");
+    cp_async_commit();
     float* sc = reinterpret_cast<float*>(base + (BM + BN) * kLd);
     for (int i = threadIdx.x; i < (BM + BN) * 4; i += kThreads) {
       const int r = i >> 2, kb = kt * 4 + (i & 3);
@@ -80,13 +78,13 @@ __global__ void __launch_bounds__(kThreads) gemm_mxfp8_kernel(const uint8_t* __r
     const int st = kt & 1;
     if (kt + 1 < ktiles) {
       load(kt + 1, st ^ 1);
-      asm volatile("cp.async.wait_group 1;" ::: "memory");
+      cp_async_wait<1>();
     } else {
-      asm volatile("cp.async.wait_group 0;" ::: "memory");
+      cp_async_wait<0>();
     }
     __syncthreads();
     const uint8_t* base = smem + st * kStageBytes;
-    const uint32_t sa = (uint32_t)__cvta_generic_to_shared(base), sb = sa + BM * kLd;
+    const uint32_t sa = smem_u32(base), sb = sa + BM * kLd;
     const float* sc = reinterpret_cast<const float*>(base + (BM + BN) * kLd);
 #pragma unroll
     for (int kb = 0; kb < 4; ++kb) {  // one UE8M0 block per k32 step

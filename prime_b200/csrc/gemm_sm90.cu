@@ -201,11 +201,6 @@ __device__ __forceinline__ int ag_next(int it, int sched_id, int sched_n, int G,
 // IO = 2 row-block order: raster index t → owner-interleaved tile row
 __device__ __forceinline__ int rs_tile_row(int t, const PeerMaps& pm, int tpr) { return ((pm.rank + 1 + t % pm.n) % pm.n) * tpr + t / pm.n; }
 
-__device__ __forceinline__ uint32_t bf16x2_bits(float lo, float hi) {
-  const __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
-  return *reinterpret_cast<const uint32_t*>(&v);
-}
-
 // EPI: 0 = plain, 1 = RoPE on the leading output columns, 2 = SwiGLU, 3 = SwiGLU backward. Separate instantiations on purpose: the
 // fused epilogues need more registers, and a plain GEMM compiled with that footprint leaves less of the register file to the
 // gradient-reduction / optimizer kernels of the comm stream that co-reside with it during the backward pass.
@@ -577,8 +572,8 @@ __global__ void __launch_bounds__(kThreads, 1)
               const int j = 4 * st + jj;
 #pragma unroll
               for (int h = 0; h < 2; ++h) {
-                const uint32_t gw = bf16x2_bits(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
-                const uint32_t uw = bf16x2_bits(acc[4 * (j + kFeat8) + 2 * h], acc[4 * (j + kFeat8) + 2 * h + 1]);
+                const uint32_t gw = pack_bf16(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+                const uint32_t uw = pack_bf16(acc[4 * (j + kFeat8) + 2 * h], acc[4 * (j + kFeat8) + 2 * h + 1]);
                 // h = silu(gate)·up from the bf16-ROUNDED gate/up — bit-compatible with the stand-alone kernel that reads them back
                 const float2 gf = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&gw));
                 const float2 uf = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&uw));
@@ -586,7 +581,7 @@ __global__ void __launch_bounds__(kThreads, 1)
                 const uint32_t o = off16(jj, h);
                 st32(slots + o, gw);
                 st32(slots + kSlotBytes + o, uw);
-                st32(slots + 2 * kSlotBytes + o, bf16x2_bits(h0, h1));
+                st32(slots + 2 * kSlotBytes + o, pack_bf16(h0, h1));
               }
             }
             step_end();
@@ -621,8 +616,8 @@ __global__ void __launch_bounds__(kThreads, 1)
                 const float s1 = __fdividef(1.f, 1.f + exp2f(-1.4426950408889634f * gf.y));
                 const float dg0 = d0 * uf.x * s0 * (1.f + gf.x * (1.f - s0)), dg1 = d1 * uf.y * s1 * (1.f + gf.y * (1.f - s1));
                 const float du0 = d0 * gf.x * s0, du1 = d1 * gf.y * s1;
-                st32(sg + o, bf16x2_bits(dg0, dg1));
-                st32(sg + kSlotBytes + o, bf16x2_bits(du0, du1));
+                st32(sg + o, pack_bf16(dg0, dg1));
+                st32(sg + kSlotBytes + o, pack_bf16(du0, du1));
               }
             }
             step_end();
@@ -699,7 +694,7 @@ __global__ void __launch_bounds__(kThreads, 1)
                   v0 += o.x;
                   v1 += o.y;
                 }
-                st32(sb + (jj >> 2) * kSlotBytes + off16(jj & 3, h), bf16x2_bits(v0, v1));
+                st32(sb + (jj >> 2) * kSlotBytes + off16(jj & 3, h), pack_bf16(v0, v1));
               }
             }
             step_end();

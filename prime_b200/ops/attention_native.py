@@ -3,8 +3,8 @@
 Forward : ``csrc/attention_sm90.cu``      qkv [B,S,(H+2Hkv)·D] → out [B,S,H·D], lse2 [B,H,S]
 Backward: ``csrc/attention_sm90.cu``    → dqkv [B,S,(H+2Hkv)·D]  (dK/dV kernel + dQ kernel + delta preprocess)
 
-No transposes, slices or concatenations ever touch HBM: the kernels address Q/K/V heads inside the fused buffer
-through one TMA tensor map and write gradients straight back in the same layout.
+No transposes, slices or concatenations ever touch HBM: the kernels load Q/K/V head tiles straight from the fused buffer
+with cp.async and write gradients from registers straight back in the same layout.
 """
 
 from __future__ import annotations
@@ -72,7 +72,7 @@ class _FlashAttnFn(torch.autograd.Function):
         delta = torch.empty_like(lse2)
         if cos is not None:
             # rotation is orthogonal: its backward is the inverse rotation, applied to dQ / dK inside the attention-backward epilogues
-            # (registers → smem → TMA store), so dQKV is written exactly once
+            # (in registers, before the 4-byte stores), so dQKV is written exactly once
             assert cos.dtype == torch.float32 and cos.is_contiguous() and sin.is_contiguous() and cos.shape[1] == D // 2 and cos.shape[0] >= S
         _launch("pb_flash_attn_bwd", _ptr(qkv), _ptr(out), _ptr(dout), _ptr(lse2), _ptr(delta), _ptr(dqkv), _ptr(doc_start), _ptr(doc_end),
                 B, S, n_heads, n_kv_heads, D, scale, int(causal), _ptr(cos), _ptr(sin), _stream(), n=3)  # fmt: skip

@@ -41,7 +41,7 @@ def timeit(fn, iters=10, warm=3, flush=None):
 
 def tile_counts(lo: torch.Tensor, end: torch.Tensor) -> tuple[int, int]:
     """Tiles the kernels visit for int32 [B, S] bounds, summed over rows: (64-key tiles of the forward / dQ kernels, 32-query tiles
-    of the dK/dV kernel). Per (b, head); the same loop bounds as csrc/attention_sm90.cu."""
+    of the dK/dV kernel). Per (b, head); the same loop bounds as Visibility::query_block / key_block in csrc/attention_sm90.cu."""
     blk = torch.arange(lo.shape[1] // 64, device=lo.device)
     fwd = (blk - lo[:, ::64].long() // 64 + 1).sum()
     dkdv = ((end[:, 63::64].long() + 31) // 32 - 2 * blk).sum()
