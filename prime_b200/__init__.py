@@ -12,4 +12,4 @@ Layout
 ``prime_b200.platform``  CLI + SDKs (pods, sandboxes, evals, tunnel, MCP …)
 """
 
-__version__ = "0.1.0"
+__version__ = "0.1.1"

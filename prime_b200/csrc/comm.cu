@@ -439,6 +439,8 @@ __global__ void __launch_bounds__(256) pseudograd_quant_kernel(const float* __re
     if (!on) continue;
     const float scale = am / 127.f;
     const float inv = scale > 0.f ? 1.f / scale : 0.f;
+    // a subnormal scale (absmax < 127·2^-126) divides instead: its reciprocal can overflow to inf, and 0·inf = NaN would clamp to +127
+    const bool divide = scale > 0.f && scale < 0x1p-126f;
     if (t64 == 0) scales[blk] = scale;
     uint32_t w[4];
 #pragma unroll
@@ -446,7 +448,8 @@ __global__ void __launch_bounds__(256) pseudograd_quant_kernel(const float* __re
       uint32_t pk = 0;
 #pragma unroll
       for (int k = 0; k < 4; ++k) {
-        const int v = (int)fmaxf(-127.f, fminf(127.f, rintf(d[4 * j + k] * inv)));
+        const float x = d[4 * j + k];
+        const int v = (int)fmaxf(-127.f, fminf(127.f, rintf(divide ? x / scale : x * inv)));
         pk |= ((uint32_t)v & 0xffu) << (8 * k);
       }
       w[j] = pk;

@@ -176,10 +176,13 @@ def quantize_int8_blockwise(x: torch.Tensor, block: int = 1024) -> tuple[torch.T
     amax = xb.abs().amax(dim=1)
     # tensor ÷ tensor: ``amax / 127.0`` (tensor ÷ Python scalar) is evaluated by torch as amax · (1/127), which differs from the
     # IEEE quotient the kernel computes by one ulp for some blocks — enough to round a tie the other way in a few elements per
-    # million and make the fused-vs-reference comparison data dependent
+    # million and make the fused-vs-reference comparison data dependent.
+    # A subnormal scale divides instead of multiplying, as the kernel does: 1/scale overflows to inf below 2^-128 (0·inf = NaN).
     scale = torch.div(amax, torch.full_like(amax, 127.0))
     inv = torch.where(scale > 0, torch.ones_like(scale) / scale, torch.zeros_like(scale))
-    q = torch.clamp(torch.round(xb * inv[:, None]), -127, 127).to(torch.int8)
+    divide = ((scale > 0) & (scale < torch.finfo(torch.float32).tiny))[:, None]
+    y = torch.where(divide, xb / torch.where(divide, scale[:, None], torch.ones_like(scale[:, None])), xb * inv[:, None])
+    q = torch.clamp(torch.round(y), -127, 127).to(torch.int8)
     return q.view(-1)[:n].contiguous(), scale
 
 

@@ -35,4 +35,9 @@ run synccheck "gpu" synccheck_gemm_epilogue tests/test_gemm_epilogue_gpu.py
 run memcheck  "gpu" memcheck_gemm_collective tests/test_gemm_collective_epilogue_gpu.py
 run racecheck "gpu" racecheck_gemm_collective tests/test_gemm_collective_epilogue_gpu.py
 run synccheck "gpu" synccheck_gemm_collective tests/test_gemm_collective_epilogue_gpu.py
+# optimizer, outer-step and peer-gather kernels with local buffers as peers, at the small shapes (block_sum / s_max shared memory;
+# pseudograd_quant's __syncthreads inside the grid-stride loop needs the 4229-block case)
+run memcheck  "gpu and not pass1 and not 4225 and not 1081352 and not 1600048 and not engine" memcheck_optimizer tests/test_optimizer_kernels_gpu.py
+run racecheck "gpu and (grad_reduce or norm_publish or pseudograd) and not pass1" racecheck_optimizer tests/test_optimizer_kernels_gpu.py
+run synccheck "gpu and pseudograd" synccheck_optimizer tests/test_optimizer_kernels_gpu.py
 cat gpurun_out/sanitizer_summary.txt
