@@ -5,10 +5,13 @@
 //  * device-side flags (st.release.sys / ld.acquire.sys) for stream-ordered signalling — no host
 //    sync, no NCCL launch on the hot path; every spin has a wall-clock bound and reports a timeout
 //    through a device error word instead of hanging the GPU;
-//  * FSDP inner step:   grad reduce-scatter (peer loads, fixed rank order)  ⊕ scale ⊕ sum-of-squares,
-//                       then clip ⊕ partitioned AdamW ⊕ bf16 cast ⊕ parameter all-gather (peer stores);
+//  * FSDP inner step:   grad reduce-scatter (peer loads in fixed rank order, or one NVSwitch multicast load) ⊕ scale ⊕
+//                       sum-of-squares, then clip ⊕ partitioned AdamW ⊕ bf16 cast ⊕ parameter all-gather (peer stores);
 //  * DiLoCo outer step: pseudo-gradient ⊕ int8 block quantise, then peer int8 all-gather ⊕ dequant-sum
-//                       ⊕ Nesterov ⊕ parameter write-back/all-gather — one kernel pair.
+//                       ⊕ Nesterov ⊕ parameter write-back/all-gather — one kernel pair;
+//  * NVLS (multimem) kernels over the multicast heap of csrc/multicast.cu: flag barrier and in-place all-reduce. They live here
+//    because every device-side wait goes through spin_wait_ge, and g_spin_timeout_ns is visible in this translation unit only
+//    (the library is built without relocatable device code).
 #include "common.cuh"
 
 using namespace pb;
@@ -51,6 +54,36 @@ __device__ __forceinline__ bool spin_wait_ge(const uint32_t* flag, uint32_t expe
 PB_EXPORT int pb_set_spin_timeout_ms(unsigned long long ms) {
   const unsigned long long ns = ms * 1000000ull;
   return (int)cudaMemcpyToSymbol(g_spin_timeout_ns, &ns, sizeof(ns));
+}
+
+// multimem PTX on NVSwitch multicast addresses: a load returns the sum over every GPU's copy, a store lands in every copy.
+__device__ __forceinline__ float4 mc_ld_reduce_f32x4(const float* mc) {
+  float4 v;
+  asm volatile("multimem.ld_reduce.relaxed.sys.global.add.v4.f32 {%0,%1,%2,%3}, [%4];"
+               : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w)
+               : "l"(mc)
+               : "memory");
+  return v;
+}
+__device__ __forceinline__ void mc_st_f32x4(float* mc, const float4& v) {
+  asm volatile("multimem.st.relaxed.sys.global.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(mc), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w)
+               : "memory");
+}
+// 8 bf16 per access; the switch accumulates in fp32 (.acc::f32) and rounds once.
+__device__ __forceinline__ uint4 mc_ld_reduce_bf16x8(const void* mc) {
+  uint4 v;
+  asm volatile("multimem.ld_reduce.relaxed.sys.global.add.acc::f32.v4.bf16x2 {%0,%1,%2,%3}, [%4];"
+               : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w)
+               : "l"(mc)
+               : "memory");
+  return v;
+}
+__device__ __forceinline__ void mc_st_bf16x8(void* mc, const uint4& v) {
+  asm volatile("multimem.st.relaxed.sys.global.v4.bf16x2 [%0], {%1,%2,%3,%4};" ::"l"(mc), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w)
+               : "memory");
+}
+__device__ __forceinline__ void mc_red_release_add_u32(uint32_t* mc, uint32_t v) {
+  asm volatile("multimem.red.release.sys.global.add.u32 [%0], %1;" ::"l"(mc), "r"(v) : "memory");
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -120,18 +153,26 @@ PB_EXPORT int pb_barrier(const PeerPtrs* flags, int base_slot, int my_idx, uint3
 }
 
 // ------------------------------------------------------------------------------------------------
-// FSDP phase 1: reduce-scatter of one gradient bucket by peer loads.
-//   out[i] = scale * sum_p grads[p][off + i]   (p in fixed rank order → bitwise identical across runs)
-//   sumsq_partial[blockIdx] += sum_i out[i]^2  (accumulated over buckets; folded by phase 2)
-// If wait_flags != nullptr the kernel first waits for flag[slot_base + p] >= expect for every peer p.
+// FSDP phase 1: reduce-scatter of one gradient bucket, over the segments of a SegTable.
+//   out[dst_off[s] + i] = scale * sum_p grads[p][src_off[s] + i]   (p in fixed rank order → bitwise identical across runs)
+//   sumsq_partial[blockIdx] += sum_i out[i]^2                      (accumulated over buckets; folded by phase 2)
+// A flat bucket's shard is one segment; a row-sharded (ZeRO-3) bucket's is one row block per parameter.
+// If wait_flags != nullptr the kernel first waits for flag[slot_base + p] >= expect for every peer p (p < grads.n).
+// MC: the gradients come as ONE multicast address and the switch sums the copies (one multimem.ld_reduce per 16 bytes instead of
+// P peer loads); its summation order is fixed by the hardware, so the result is deterministic but not bitwise equal to rank order.
 // ------------------------------------------------------------------------------------------------
+constexpr int kMaxSegs = 16;
+struct SegTable {
+  int64_t src_off[kMaxSegs], dst_off[kMaxSegs], n[kMaxSegs];
+  int nseg;
+};
+
 // U = independent 16-byte vectors per thread and iteration: with few peers a thread otherwise has one or two loads in flight and
 // the kernel runs at half the memory roof (ncu r2: F = 1 → dram 50 %, warps 49 %); U·F loads are issued before any is consumed.
-template <int U, int P>
-__global__ void __launch_bounds__(512) grad_reduce_kernel(PeerPtrs grads, int64_t off, int64_t n, float scale,
+template <int U, int P, bool MC>
+__global__ void __launch_bounds__(512) grad_reduce_kernel(PeerPtrs grads, const float* __restrict__ mc_grads, SegTable segs, float scale,
                                                           float* __restrict__ out, float* __restrict__ sumsq_partial,
-                                                          const uint32_t* wait_flags, int slot_base, uint32_t expect,
-                                                          uint32_t* err) {
+                                                          const uint32_t* wait_flags, int slot_base, uint32_t expect, uint32_t* err) {
   __shared__ float red[32];
   if (wait_flags != nullptr) {
     __shared__ int s_fail;
@@ -141,30 +182,39 @@ __global__ void __launch_bounds__(512) grad_reduce_kernel(PeerPtrs grads, int64_
     __syncthreads();
     if (s_fail) return;  // a peer never signalled: leave the shard untouched, the host raises on the error word
   }
-  const int64_t nvec = n >> 2;
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
   float ss = 0.f;
-  for (int64_t i0 = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i0 < nvec; i0 += stride * U) {
-    float4 v[U][P];  // P = compile-time bound on the number of peers (registers are allocated for P, not for kMaxPeers)
+  for (int s = 0; s < segs.nseg; ++s) {
+    const int64_t nvec = segs.n[s] >> 2, src = segs.src_off[s];
+    float4* o4 = reinterpret_cast<float4*>(out + segs.dst_off[s]);
+    for (int64_t i0 = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i0 < nvec; i0 += stride * U) {
+      float4 v[U][P];  // P = compile-time bound on the number of peers (registers are allocated for P, not for kMaxPeers)
 #pragma unroll
-    for (int u = 0; u < U; ++u) {
-      const int64_t i = i0 + u * stride;
+      for (int u = 0; u < U; ++u) {
+        const int64_t i = i0 + u * stride;
+        if constexpr (MC) {
+          if (i < nvec) v[u][0] = mc_ld_reduce_f32x4(mc_grads + src + 4 * i);
+        } else {
 #pragma unroll
-      for (int p = 0; p < P; ++p)
-        if (p < grads.n && i < nvec)
-          v[u][p] = ld_relaxed_sys_f4(reinterpret_cast<const float4*>(reinterpret_cast<const float*>(grads.p[p]) + off) + i);
-    }
+          for (int p = 0; p < P; ++p)
+            if (p < grads.n && i < nvec)
+              v[u][p] = ld_relaxed_sys_f4(reinterpret_cast<const float4*>(reinterpret_cast<const float*>(grads.p[p]) + src) + i);
+        }
+      }
 #pragma unroll
-    for (int u = 0; u < U; ++u) {
-      const int64_t i = i0 + u * stride;
-      if (i < nvec) {
-        float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+      for (int u = 0; u < U; ++u) {
+        const int64_t i = i0 + u * stride;
+        if (i < nvec) {
+          float4 acc = MC ? v[u][0] : make_float4(0.f, 0.f, 0.f, 0.f);
+          if constexpr (!MC) {
 #pragma unroll
-        for (int p = 0; p < P; ++p)
-          if (p < grads.n) acc.x += v[u][p].x, acc.y += v[u][p].y, acc.z += v[u][p].z, acc.w += v[u][p].w;  // fixed rank order
-        acc.x *= scale, acc.y *= scale, acc.z *= scale, acc.w *= scale;
-        reinterpret_cast<float4*>(out)[i] = acc;
-        ss += acc.x * acc.x + acc.y * acc.y + acc.z * acc.z + acc.w * acc.w;
+            for (int p = 0; p < P; ++p)
+              if (p < grads.n) acc.x += v[u][p].x, acc.y += v[u][p].y, acc.z += v[u][p].z, acc.w += v[u][p].w;  // fixed rank order
+          }
+          acc.x *= scale, acc.y *= scale, acc.z *= scale, acc.w *= scale;
+          o4[i] = acc;
+          ss += acc.x * acc.x + acc.y * acc.y + acc.z * acc.z + acc.w * acc.w;
+        }
       }
     }
   }
@@ -174,73 +224,24 @@ __global__ void __launch_bounds__(512) grad_reduce_kernel(PeerPtrs grads, int64_
 
 PB_EXPORT int pb_grad_reduce_grid() { return 132 * 2; }
 
-PB_EXPORT int pb_grad_reduce(const PeerPtrs* grads, int64_t off, int64_t n, float scale, float* out, float* sumsq_partial,
-                             const uint32_t* wait_flags, int slot_base, uint32_t expect, uint32_t* err, int max_ctas,
+// grads->n = peers (and flags waited on); mc_grads != nullptr selects the switch-side sum at that multicast address, to which
+// src_off is relative as it is to every grads->p[p].
+PB_EXPORT int pb_grad_reduce(const PeerPtrs* grads, const float* mc_grads, const SegTable* segs, float scale, float* out,
+                             float* sumsq_partial, const uint32_t* wait_flags, int slot_base, uint32_t expect, uint32_t* err, int max_ctas,
                              cudaStream_t stream) {
-  if (n % 4 != 0 || off % 4 != 0) return -1;
-  int grid = pb_grad_reduce_grid();
-  if (max_ctas > 0 && max_ctas < grid) grid = max_ctas;
-  if (grads->n == 1)
-    grad_reduce_kernel<4, 1><<<grid, 512, 0, stream>>>(*grads, off, n, scale, out, sumsq_partial, wait_flags, slot_base, expect, err);
-  else if (grads->n == 2)
-    grad_reduce_kernel<4, 2><<<grid, 512, 0, stream>>>(*grads, off, n, scale, out, sumsq_partial, wait_flags, slot_base, expect, err);
-  else if (grads->n <= 4)
-    grad_reduce_kernel<2, 4><<<grid, 512, 0, stream>>>(*grads, off, n, scale, out, sumsq_partial, wait_flags, slot_base, expect, err);
-  else
-    grad_reduce_kernel<1, 8><<<grid, 512, 0, stream>>>(*grads, off, n, scale, out, sumsq_partial, wait_flags, slot_base, expect, err);
-  PB_CHECK_LAUNCH();
-  return 0;
-}
-
-// Segmented variant for row-sharded (ZeRO-3) buckets: the rank's shard of a bucket is one row block PER PARAMETER, i.e. up to
-// kMaxSegs strided pieces of the full-size gradient buffer. out[dst_off[s] + i] = scale * Σ_p grads[p][src_off[s] + i].
-constexpr int kMaxSegs = 16;
-struct SegTable {
-  int64_t src_off[kMaxSegs], dst_off[kMaxSegs], n[kMaxSegs];
-  int nseg;
-};
-__global__ void __launch_bounds__(512) grad_reduce_segs_kernel(PeerPtrs grads, SegTable segs, float scale, float* __restrict__ out,
-                                                               float* __restrict__ sumsq_partial, const uint32_t* wait_flags,
-                                                               int slot_base, uint32_t expect, uint32_t* err) {
-  __shared__ float red[32];
-  if (wait_flags != nullptr) {
-    __shared__ int s_fail;
-    if (threadIdx.x == 0) s_fail = 0;
-    __syncthreads();
-    if ((int)threadIdx.x < grads.n && !spin_wait_ge(wait_flags + slot_base + threadIdx.x, expect, err)) s_fail = 1;
-    __syncthreads();
-    if (s_fail) return;
-  }
-  float ss = 0.f;
-  for (int sidx = 0; sidx < segs.nseg; ++sidx) {
-    const int64_t nvec = segs.n[sidx] >> 2, so = segs.src_off[sidx];
-    float4* o4 = reinterpret_cast<float4*>(out + segs.dst_off[sidx]);
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < nvec; i += (int64_t)gridDim.x * blockDim.x) {
-      float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-      for (int p = 0; p < kMaxPeers; ++p) {
-        if (p < grads.n) {
-          const float4 v = ld_relaxed_sys_f4(reinterpret_cast<const float4*>(reinterpret_cast<const float*>(grads.p[p]) + so) + i);
-          acc.x += v.x, acc.y += v.y, acc.z += v.z, acc.w += v.w;
-        }
-      }
-      acc.x *= scale, acc.y *= scale, acc.z *= scale, acc.w *= scale;
-      o4[i] = acc;
-      ss += acc.x * acc.x + acc.y * acc.y + acc.z * acc.z + acc.w * acc.w;
-    }
-  }
-  ss = block_sum(ss, red);
-  if (threadIdx.x == 0) sumsq_partial[blockIdx.x] += ss;
-}
-PB_EXPORT int pb_grad_reduce_segs(const PeerPtrs* grads, const SegTable* segs, float scale, float* out, float* sumsq_partial,
-                                  const uint32_t* wait_flags, int slot_base, uint32_t expect, uint32_t* err, int max_ctas,
-                                  cudaStream_t stream) {
   if (segs->nseg < 0 || segs->nseg > kMaxSegs) return -1;
   for (int i = 0; i < segs->nseg; ++i)
     if ((segs->n[i] | segs->src_off[i] | segs->dst_off[i]) & 3) return -1;
   int grid = pb_grad_reduce_grid();
-  if (max_ctas > 0 && max_ctas < grid) grid = max_ctas;
-  grad_reduce_segs_kernel<<<grid, 512, 0, stream>>>(*grads, *segs, scale, out, sumsq_partial, wait_flags, slot_base, expect, err);
+  if (max_ctas > 0 && max_ctas < grid) grid = max_ctas;  // leave SMs to the backward pass this runs under
+  const auto launch = [&](auto kernel) {
+    kernel<<<grid, 512, 0, stream>>>(*grads, mc_grads, *segs, scale, out, sumsq_partial, wait_flags, slot_base, expect, err);
+  };
+  if (mc_grads != nullptr) launch(grad_reduce_kernel<1, 1, true>);
+  else if (grads->n == 1) launch(grad_reduce_kernel<4, 1, false>);
+  else if (grads->n == 2) launch(grad_reduce_kernel<4, 2, false>);
+  else if (grads->n <= 4) launch(grad_reduce_kernel<2, 4, false>);
+  else launch(grad_reduce_kernel<1, 8, false>);
   PB_CHECK_LAUNCH();
   return 0;
 }
@@ -637,6 +638,67 @@ __global__ void __launch_bounds__(512) cast_push_kernel(const float* __restrict_
 PB_EXPORT int pb_cast_push(const float* src, int64_t n, const PeerPtrs* dst, int64_t dst_off, cudaStream_t stream) {
   if (n % 8 != 0 || dst_off % 8 != 0) return -1;
   cast_push_kernel<<<132 * 2, 512, 0, stream>>>(src, n, *dst, dst_off);
+  PB_CHECK_LAUNCH();
+  return 0;
+}
+
+// ------------------------------------------------------------------------------------------------
+// NVLS in-place all-reduce over the multicast mapping (parallel/multicast.py: MulticastHeap.all_reduce_).
+// ------------------------------------------------------------------------------------------------
+// All-ranks barrier for ONE block index: every rank's block `b` adds 1 to flag[b] on every GPU with a single multimem.red,
+// then waits on its own copy until `world` arrivals of this phase are in. Counters only grow: phase k of launch `epoch`
+// (k = 0 arrive, 1 depart) completes at world·(2·(epoch-1) + k + 1), so no reset and no ABA across launches.
+// Returns false in every thread of the block when the wait failed (timeout or host abort, recorded in the error word).
+__device__ __forceinline__ bool mc_barrier(uint32_t* mc_flags, const uint32_t* local_flags, uint32_t target, uint32_t* err) {
+  __shared__ int s_ok;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    __threadfence_system();
+    mc_red_release_add_u32(mc_flags + blockIdx.x, 1u);
+    s_ok = spin_wait_ge(local_flags + blockIdx.x, target, err);
+  }
+  __syncthreads();
+  return s_ok;
+}
+
+// n16 = number of 16-byte units; each rank owns a contiguous 1/world of them: it reduces that slice through the switch and
+// multicasts it back, so the all-reduce is two-shot in one kernel.
+template <bool BF16>
+__global__ void __launch_bounds__(512) mc_all_reduce_kernel(void* mc, int64_t n16, uint32_t* mc_flags, const uint32_t* local_flags,
+                                                             int rank, int world, uint32_t epoch, uint32_t* err) {
+  const uint32_t base = (uint32_t)world * 2u * (epoch - 1u);
+  if (!mc_barrier(mc_flags, local_flags, base + (uint32_t)world, err)) return;  // a rank's input never arrived: reduce nothing
+  const int64_t per = (n16 + world - 1) / world;
+  const int64_t lo = per * rank, hi = lo + per < n16 ? lo + per : n16;
+  uint4* p = reinterpret_cast<uint4*>(mc);
+  for (int64_t i = lo + (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < hi; i += (int64_t)gridDim.x * blockDim.x) {
+    if constexpr (BF16) {
+      const uint4 v = mc_ld_reduce_bf16x8(p + i);
+      mc_st_bf16x8(p + i, v);
+    } else {
+      const float4 v = mc_ld_reduce_f32x4(reinterpret_cast<const float*>(p + i));
+      mc_st_f32x4(reinterpret_cast<float*>(p + i), v);
+    }
+  }
+  mc_barrier(mc_flags, local_flags, base + 2u * (uint32_t)world, err);  // every slice has been written everywhere
+}
+
+// Number of flag words an all-reduce needs (one per block) — the grid is fixed so that every rank launches the same one
+// and all blocks are co-resident (a spinning block must never wait for a partner that is queued behind it).
+PB_EXPORT int pb_mc_all_reduce_grid() { return 132; }
+
+// dtype: 0 = f32, 1 = bf16. `mc_data` and `mc_flags` are addresses in the MULTICAST mapping, `local_flags` the same words
+// in this rank's unicast mapping. nbytes must be a multiple of 16. `epoch` starts at 1 and grows by 1 per call on every rank.
+PB_EXPORT int pb_mc_all_reduce(void* mc_data, int64_t nbytes, int dtype, uint32_t* mc_flags, const uint32_t* local_flags, int rank,
+                               int world, uint32_t epoch, uint32_t* err, cudaStream_t stream) {
+  if (nbytes % 16 != 0 || epoch == 0 || world < 1) return -1;
+  const int grid = pb_mc_all_reduce_grid();
+  if (dtype == 1)
+    mc_all_reduce_kernel<true><<<grid, 512, 0, stream>>>(mc_data, nbytes / 16, mc_flags, local_flags, rank, world, epoch, err);
+  else if (dtype == 0)
+    mc_all_reduce_kernel<false><<<grid, 512, 0, stream>>>(mc_data, nbytes / 16, mc_flags, local_flags, rank, world, epoch, err);
+  else
+    return -1;
   PB_CHECK_LAUNCH();
   return 0;
 }

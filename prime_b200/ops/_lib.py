@@ -109,7 +109,8 @@ class AdamArgs(ctypes.Structure):
 
 
 class SegTable(ctypes.Structure):
-    """Up to 16 (src offset, dst offset, length) pieces of a row-sharded bucket (csrc/comm.cu: grad_reduce_segs)."""
+    """Up to 16 (src offset, dst offset, length) pieces that ``pb_grad_reduce`` (csrc/comm.cu) reduces: one for a flat bucket, one
+    row block per parameter for a row-sharded one."""
 
     _fields_ = [("src_off", ctypes.c_int64 * 16), ("dst_off", ctypes.c_int64 * 16), ("n", ctypes.c_int64 * 16), ("nseg", ctypes.c_int)]
 
@@ -174,14 +175,13 @@ def _sigs() -> dict:
         "pb_signal": [PP, i32, u32, vp],
         "pb_barrier": [PP, i32, i32, u32, vp, vp],
         "pb_grad_reduce_grid": [],
-        "pb_grad_reduce": [PP, i64, i64, f32, vp, vp, vp, i32, u32, vp, i32, vp],
+        "pb_grad_reduce": [PP, vp, ctypes.POINTER(SegTable), f32, vp, vp, vp, i32, u32, vp, i32, vp],
         "pb_norm_publish": [vp, i32, PP, PP, i32, i32, u32, vp],
         "pb_adamw_push": [vp, vp, vp, vp, i64, ctypes.POINTER(AdamArgs), vp, i32, vp, i32, u32, PP, i64, vp, vp, vp, vp],
         "pb_pseudograd_quant": [vp, vp, vp, vp, i64, vp],
         "pb_outer_nesterov": [PP, PP, vp, vp, vp, i64, ctypes.POINTER(OuterArgs), PP, vp, vp, i32, vp, vp],
         "pb_outer_nesterov_f32": [PP, vp, vp, vp, i64, ctypes.POINTER(OuterArgs), PP, vp, vp, i32, vp, vp],
         "pb_set_spin_timeout_ms": [ctypes.c_ulonglong],
-        "pb_grad_reduce_segs": [PP, ctypes.POINTER(SegTable), f32, vp, vp, vp, i32, u32, vp, i32, vp],
         "pb_embedding_fwd": [vp, i64, PP, i32, i32, vp, vp],
         "pb_embedding_sort": [vp, i64, vp, vp],
         "pb_embedding_scatter": [vp, i64, vp, vp, i32, vp],
@@ -189,7 +189,7 @@ def _sigs() -> dict:
         "pb_gemm_wgather": [vp, ctypes.POINTER(vp), i32, i32, vp, vp, vp, i32, i32, i32, i32, i32, i32, ctypes.POINTER(GemmEpilogue), i32,
                             ctypes.POINTER(vp), vp, i32, i32, vp],
         "pb_cast_push": [vp, i64, PP, i64, vp],
-        # NVLS: VMM allocations shared by fd, multicast objects, multimem kernels (csrc/multicast.cu)
+        # NVLS: VMM allocations shared by fd and multicast objects (csrc/multicast.cu), the multimem all-reduce (csrc/comm.cu)
         "pb_mc_supported": [i32],
         "pb_vmm_granularity": [i32, i32, ctypes.c_size_t, ctypes.POINTER(ctypes.c_size_t)],
         "pb_vmm_create": [i32, ctypes.c_size_t, ctypes.POINTER(ctypes.c_uint64), ctypes.POINTER(i32)],
@@ -203,7 +203,6 @@ def _sigs() -> dict:
         "pb_mc_unbind": [ctypes.c_uint64, i32, ctypes.c_size_t],
         "pb_mc_all_reduce_grid": [],
         "pb_mc_all_reduce": [vp, i64, i32, vp, vp, i32, i32, u32, vp, vp],
-        "pb_mc_grad_reduce": [vp, i64, i64, f32, vp, vp, vp, i32, u32, i32, vp, i32, vp],
     }
 
 

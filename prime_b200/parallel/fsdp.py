@@ -40,7 +40,7 @@ import torch.nn as nn
 
 from ..ops import _lib, reference
 from ..ops.functional import _count
-from .layout import Bucket, plan_layout, use_zero3
+from .layout import Bucket, ShardLayout, plan_layout, use_zero3
 from .mesh import Mesh
 from .symm import SymmetricHeap
 
@@ -64,6 +64,13 @@ class RowShard:
     next_fwd: "RowShard | None" = None
     next_bwd: "RowShard | None" = None
     ver: list = field(default_factory=lambda: [0])  # shared with the engine: bumped whenever the shards change (optimizer / outer step)
+
+
+def reduce_segments(layout: ShardLayout, rank: int) -> list[_lib.SegTable]:
+    """Per bucket, what rank ``rank``'s gradient reduce-scatter reads and writes: (offset in ``grad_flat``, offset in the reduced
+    gradient shard, elements). A flat bucket is one piece, a row-sharded one a row block per parameter. At F = 1 the shard starts
+    where the bucket does, so the reduction is in place in ``grad_flat``, which the shard aliases there."""
+    return [_lib.SegTable.of((b.start + src, dst, n) for src, dst, n in b.owned(rank)) for b in layout.buckets]
 
 
 class _Boundary(torch.autograd.Function):
@@ -139,7 +146,7 @@ class ShardedEngine:
         self.bucket_index = {b.name: i for i, b in enumerate(self.buckets)}
         self._ready = [False] * len(self.buckets)
         self._work: list = [None] * len(self.buckets)  # async collective handles (collective backend)
-        self._segs: list = [None] * len(self.buckets)  # rows kind: SegTable of this rank's pieces inside ``grad_flat``
+        self._segs = reduce_segments(self.layout, mesh.fsdp_rank)
         self._allocate()
         self._install_hooks()
 
@@ -182,9 +189,9 @@ class ShardedEngine:
             self._scratch = {k: torch.empty(v, dtype=self.param_dtype, device=dev) for k, v in by_stage.items()}
             self._gather_flags = torch.zeros(64, dtype=torch.int32, device=dev)
         with torch.no_grad():
-            for i, b in enumerate(self.buckets):
+            for b in self.buckets:
                 if b.kind == "rows":
-                    self._attach_rows_bucket(i, b)
+                    self._attach_rows_bucket(b)
                     continue
                 for _, p, off in b.params:
                     view = self.param_flat[b.pstart + off : b.pstart + off + p.numel()].view(p.shape)
@@ -218,13 +225,12 @@ class ShardedEngine:
             a.next_fwd = b
             b.next_bwd = a
 
-    def _attach_rows_bucket(self, bucket_id: int, b: Bucket) -> None:
+    def _attach_rows_bucket(self, b: Bucket) -> None:
         """ZeRO-3: copy this rank's row block of every weight into the shard buffer, then re-point the parameter at the shared
         gather scratch (embedding: at a stride-0 placeholder — its rows are only ever read through the peers' shards)."""
         F, r, heap = self.F, self.mesh.fsdp_rank, self.heap
         ranks = self.mesh.fsdp_ranks
         key = "layer" if b.name.startswith("layer") else b.name
-        segs = []
         for (qn, p, off), (src, lo, piece) in zip(b.params, b.owned(r)):
             rows, cols = p.shape
             rpr = rows // F
@@ -242,8 +248,6 @@ class ShardedEngine:
             p.main_grad = self.grad_flat[b.start + off : b.start + off + p.numel()].view(p.shape)
             p.z3 = RowShard(rows, cols, F, r, rpr, peers, full_ptr, self._gather_flags, shard, full=full if b.name != "embed" else None,
                             ver=self._pver)
-            segs.append((b.start + src, lo, piece))
-        self._segs[bucket_id] = _lib.SegTable.of(segs)
 
     def lib_grid(self) -> int:
         return _lib.load().pb_grad_reduce_grid()
@@ -361,45 +365,12 @@ class ShardedEngine:
                     _count()
                     wait_flags = self.heap.flags.data_ptr()
                 ctas = self.reduce_ctas if (F > 1 and self.overlap) else 0
-                if b.kind == "rows" and self._nvls:  # ZeRO-3 + NVLS: each parameter's row block is summed inside the switch
-                    segs = self._segs[bucket_id]
-                    for i in range(segs.nseg):
-                        _lib.check(
-                            self.lib.pb_mc_grad_reduce(
-                                self.heap.mc_ptr(self.grad_flat), segs.src_off[i], segs.n[i], 1.0 / F, self.gshard[segs.dst_off[i] :].data_ptr(),
-                                self.sumsq_partial.data_ptr(), wait_flags if i == 0 else None, slot_base, self._epoch, F,
-                                self.heap.err.data_ptr(), self.reduce_ctas if self.overlap else 0, s,
-                            ),
-                            "pb_mc_grad_reduce",
-                        )  # fmt: skip
-                    _count(segs.nseg)
-                    return
-                if b.kind == "rows":  # ZeRO-3 bucket: one row block per parameter
-                    gp = self.heap.peers(ranks, self.grad_flat)
-                    _lib.check(
-                        self.lib.pb_grad_reduce_segs(ctypes.byref(gp), ctypes.byref(self._segs[bucket_id]), 1.0 / F, self.gshard.data_ptr(),
-                                                     self.sumsq_partial.data_ptr(), wait_flags, slot_base, self._epoch,
-                                                     self.heap.err.data_ptr(), ctas, s),
-                        "pb_grad_reduce_segs",
-                    )  # fmt: skip
-                    _count()
-                    return
-                out = self.gshard[b.shard_start :] if F > 1 else self.grad_flat[b.start :]
-                if self._nvls:  # the switch sums the F copies: one multimem.ld_reduce per 16 bytes instead of F peer loads
-                    _lib.check(
-                        self.lib.pb_mc_grad_reduce(
-                            self.heap.mc_ptr(self.grad_flat), b.start + r * b.shard_size, b.shard_size, 1.0 / F, out.data_ptr(),
-                            self.sumsq_partial.data_ptr(), wait_flags, slot_base, self._epoch, F, self.heap.err.data_ptr(),
-                            self.reduce_ctas if self.overlap else 0, s,
-                        ),
-                        "pb_mc_grad_reduce",
-                    )  # fmt: skip
-                    _count()
-                    return
                 gp = self.heap.peers(ranks, self.grad_flat)
+                # NVLS: the switch sums the F copies, one multimem.ld_reduce per 16 bytes instead of F peer loads
+                mc = self.heap.mc_ptr(self.grad_flat) if self._nvls else None
                 _lib.check(
                     self.lib.pb_grad_reduce(
-                        ctypes.byref(gp), b.start + r * b.shard_size, b.shard_size, 1.0 / F, out.data_ptr(),
+                        ctypes.byref(gp), mc, ctypes.byref(self._segs[bucket_id]), 1.0 / F, self.gshard.data_ptr(),
                         self.sumsq_partial.data_ptr(), wait_flags, slot_base, self._epoch, self.heap.err.data_ptr(), ctas, s,
                     ),
                     "pb_grad_reduce",

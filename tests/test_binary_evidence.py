@@ -47,7 +47,7 @@ def test_gemm_kernels_use_wgmma(sass):
 
 
 @needs_toolchain
-def test_hopper_paths_are_present(sass):
+def test_hopper_instruction_paths_are_present(sass):
     k = _kernels(sass)
 
     def body(*needles):
@@ -64,8 +64,10 @@ def test_hopper_paths_are_present(sass):
     comm = body("adamw_push_kernel")
     assert "STG.E.128" in comm  # 128-bit peer stores
     assert "LD.E.STRONG.SYS" in body("outer_nesterov") or "STRONG.SYS" in body("outer_nesterov")
-    # NVLS: the reduction is a multimem load (LDGMC), in f32 and in bf16 with fp32 accumulation in the switch
-    assert "LDGMC.E.ADD.F32x4" in body("mc_grad_reduce_kernel")
+    # NVLS: the reduction is a multimem load (LDGMC), in f32 and in bf16 with fp32 accumulation in the switch; only the multicast
+    # instantiation of the gradient reduce-scatter (MC = true) has it
+    assert "LDGMC.E.ADD.F32x4" in body("grad_reduce_kernel", "Lb1E")
+    assert "LDGMC" not in body("grad_reduce_kernel", "Lb0E") and "STRONG.SYS" in body("grad_reduce_kernel", "Lb0E")
     allred = body("mc_all_reduce_kernel")
     assert "LDGMC.E.ADD.F32x4" in allred and "BF16x8" in allred and "REDG.E.ADD.STRONG.SYS" in allred
 

@@ -287,11 +287,11 @@ NVLS_WORKER = textwrap.dedent(
     o_mc, o_p2p = torch.zeros(shard, device=dev), torch.zeros(shard, device=dev)
     ss_mc, ss_p2p = torch.zeros(grid, device=dev), torch.zeros(grid, device=dev)
     s = torch.cuda.current_stream().cuda_stream
-    _lib.check(lib.pb_mc_grad_reduce(heap.mc_ptr(grads), off, shard, 0.5, o_mc.data_ptr(), ss_mc.data_ptr(), None, 0, 0, world,
-                                     heap.err.data_ptr(), 0, s), "pb_mc_grad_reduce")
     pp = heap.peers(range(world), grads)
-    _lib.check(lib.pb_grad_reduce(ctypes.byref(pp), off, shard, 0.5, o_p2p.data_ptr(), ss_p2p.data_ptr(), None, 0, 0,
-                                  heap.err.data_ptr(), 0, s), "pb_grad_reduce")
+    table = _lib.SegTable.of([(off, 0, shard)])
+    for mc, o, ss in ((heap.mc_ptr(grads), o_mc, ss_mc), (None, o_p2p, ss_p2p)):  # the one launcher, with and without mc_grads
+        _lib.check(lib.pb_grad_reduce(ctypes.byref(pp), mc, ctypes.byref(table), 0.5, o.data_ptr(), ss.data_ptr(), None, 0, 0,
+                                      heap.err.data_ptr(), 0, s), "pb_grad_reduce")
     torch.cuda.synchronize()
     out["rs"] = float((o_mc - o_p2p).abs().max() / o_p2p.abs().max())
     out["rs_sumsq"] = abs(float(ss_mc.sum()) / float(ss_p2p.sum()) - 1.0)

@@ -16,9 +16,11 @@ rules, at the GPU tests' own shapes and step numbers, reject each plausible bug,
 arguments before touching the device.
 
 Coverage (test names below):
-- ``grad_reduce_kernel<4,1>``, ``<4,2>``, ``<2,4>`` (P = 3, 4) and ``<1,8>`` (P = 5, 8), one vector and one vector past whole
-  grid-stride passes, every rank of the bucket, ``max_ctas`` 0 / 7, sum of squares over two buckets: test_grad_reduce
-- ``grad_reduce_segs_kernel`` with 1 and 16 irregular segments and gaps, and with none: test_grad_reduce_segs
+- ``grad_reduce_kernel<4,1>``, ``<4,2>``, ``<2,4>`` (P = 3, 4) and ``<1,8>`` (P = 5, 8) through ``pb_grad_reduce``: one segment of one
+  vector and one vector past whole grid-stride passes, every rank of the bucket, ``max_ctas`` 0 / 7, sum of squares over two
+  buckets: test_grad_reduce_one_segment; 1 and 16 irregular segments and gaps, and none: test_grad_reduce_segments; the host-abort
+  error word with the flags not yet signalled (the prologue the multicast instantiation shares; a multicast address needs two GPUs
+  on an NVSwitch, tests/test_multigpu.py): test_grad_reduce_abort
 - ``norm_publish_kernel``: test_norm_publish; ``adamw_push_kernel``: test_adamw_push; both through the engine at F = 1:
   test_engine_step_matches_fp64_adamw
 - ``pseudograd_quant_kernel`` edge blocks (zero, ties, ±absmax at both ends, subnormal scale, scale 0, idle groups, grid-stride
@@ -55,7 +57,6 @@ def _gr_pass(P: int) -> int:
     return GR_GRID * 512 * 4 * U
 
 
-SEG_PASS = GR_GRID * 512 * 4
 ADAM_PASS = 264 * 512 * 8  # also cast_push
 F32_PASS = 528 * 256 * 8  # outer_nesterov_f32
 QBLK_PASS = 1056 * 4  # 1024-element blocks per pass of pseudograd_quant / outer_nesterov
@@ -383,7 +384,7 @@ def int8_sum64(qs, ss):
 
 
 # ================================================================================================== CPU: launcher contracts
-def test_launchers_reject_impossible_arguments_before_touching_the_device():
+def test_launchers_refuse_impossible_arguments_before_touching_the_device():
     try:
         lib = _lib.load()
     except Exception as e:  # noqa: BLE001
@@ -395,19 +396,15 @@ def test_launchers_reject_impossible_arguments_before_touching_the_device():
     for i in range(8):
         nine.p[i] = a
 
-    def reduce(off=0, n=1024):
-        return lib.pb_grad_reduce(ctypes.byref(pp), off, n, 1.0, a, a, None, 0, 0, a, 0, None)
-
-    assert reduce(n=1022) == -1 and reduce(off=2) == -1  # float4 vectors
-
-    def segs(table):
-        return lib.pb_grad_reduce_segs(ctypes.byref(pp), ctypes.byref(table), 1.0, a, a, None, 0, 0, a, 0, None)
-
     many = _lib.SegTable()
     many.nseg = 17  # the table holds 16
-    assert segs(many) == -1
-    for bad in ((2, 0, 8), (0, 6, 8), (0, 0, 6)):
-        assert segs(_lib.SegTable.of([(0, 0, 8), bad])) == -1  # every segment 4-aligned
+    for mc in (None, a):  # peer loads and the multicast instantiation check the same arguments
+        def reduce(table):
+            return lib.pb_grad_reduce(ctypes.byref(pp), mc, ctypes.byref(table), 1.0, a, a, None, 0, 0, a, 0, None)
+
+        assert reduce(many) == -1
+        for bad in ((2, 0, 8), (0, 6, 8), (0, 0, 6), (0, 0, 1022)):
+            assert reduce(_lib.SegTable.of([(0, 0, 8), bad])) == -1  # every segment 4-aligned: float4 vectors
 
     args = _lib.AdamArgs(1e-3, 0.9, 0.95, 1e-8, 0.1, 0.1, 0.05, 1.0)
 
@@ -514,7 +511,7 @@ def test_outer_rules_reject_wrong_sign_and_table_off_by_one(case):
 @pytest.mark.gpu
 @pytest.mark.parametrize("size", ["vector", "pass1"])
 @pytest.mark.parametrize("P", PEERS)
-def test_grad_reduce(P, size):
+def test_grad_reduce_one_segment(P, size):
     dev = _dev()
     start, shard, grads, scale = _reduce_case(P, size)
     grads = [g.to(dev) for g in grads]
@@ -530,8 +527,9 @@ def test_grad_reduce(P, size):
     nvec = shard // 4
 
     def run(off, out, part, max_ctas, wait=None):
-        _launch("pb_grad_reduce", _pref(gp), off, shard, scale, out.ptr(), part.ptr(), wait, slot_base, EPOCH, err.data_ptr(),
-                max_ctas, _stream())  # fmt: skip
+        table = _lib.SegTable.of([(off, 0, shard)])
+        _launch("pb_grad_reduce", _pref(gp), None, ctypes.byref(table), scale, out.ptr(), part.ptr(), wait, slot_base, EPOCH,
+                err.data_ptr(), max_ctas, _stream())  # fmt: skip
         _check_err(err, f"grad_reduce P={P}")
 
     for r in range(P):
@@ -564,12 +562,13 @@ def test_grad_reduce(P, size):
         assert bitwise_equal(g, s), "grad_reduce wrote its input"
 
 
-def _segments(nseg, seed):
-    """(src_off, dst_off, n) with irregular 4-aligned offsets, gaps between destinations; one segment past a grid-stride pass."""
+def _segments(nseg, seed, P):
+    """(src_off, dst_off, n) with irregular 4-aligned offsets, gaps between destinations; one segment one vector past a whole
+    grid-stride pass of the instantiation that P peers select."""
     gen = torch.Generator().manual_seed(seed)
-    lens = [SEG_PASS + 4] if nseg == 1 else [4 * int(x) for x in torch.randint(1, 3000, (nseg,), generator=gen)]
+    lens = [_gr_pass(P) + 4] if nseg == 1 else [4 * int(x) for x in torch.randint(1, 3000, (nseg,), generator=gen)]
     if nseg > 1:
-        lens[5] = SEG_PASS + 4
+        lens[5] = _gr_pass(P) + 4
         lens[0], lens[9] = 4, 8
     segs, src, dst = [], 8, 4
     for n in lens:
@@ -580,12 +579,19 @@ def _segments(nseg, seed):
     return segs, src + 12, dst + 12
 
 
+def _segs_body(grads, segs, scale, dst_len):
+    body = torch.full((dst_len,), SENT[torch.float32], device=grads[0].device)
+    for s, d, n in segs:
+        body[d : d + n] = reduce_emulated(grads, s, n, scale)
+    return body
+
+
 @pytest.mark.gpu
 @pytest.mark.parametrize("nseg", [0, 1, 16])
 @pytest.mark.parametrize("P", PEERS)
-def test_grad_reduce_segs(P, nseg):
+def test_grad_reduce_segments(P, nseg):
     dev = _dev()
-    segs, src_len, dst_len = _segments(max(nseg, 1), seed=P * 17 + nseg)
+    segs, src_len, dst_len = _segments(max(nseg, 1), seed=P * 17 + nseg, P=P)
     segs = segs[:nseg]
     grads = [_wide(src_len, -20, 4, seed=300 + 10 * P + p, zeros=0.05).to(dev) for p in range(P)]
     scale = _f32(1.0 / P)
@@ -594,21 +600,58 @@ def test_grad_reduce_segs(P, nseg):
     part = Out(GR_GRID, torch.float32, torch.rand(GR_GRID))  # accumulates onto what earlier buckets left
     part0 = part.t.clone()
     table = _lib.SegTable.of(segs)
-    _launch("pb_grad_reduce_segs", _pref(_pp(grads)), ctypes.byref(table), scale, out.ptr(), part.ptr(), None, 0, 0, err.data_ptr(), 0,
+    _launch("pb_grad_reduce", _pref(_pp(grads)), None, ctypes.byref(table), scale, out.ptr(), part.ptr(), None, 0, 0, err.data_ptr(), 0,
             _stream())  # fmt: skip
-    _check_err(err, "grad_reduce_segs")
-    body = torch.full((dst_len,), SENT[torch.float32], device=dev)
-    for s, d, n in segs:
-        body[d : d + n] = reduce_emulated(grads, s, n, scale)
-    assert_bitwise(out.buf, out.image(body), f"grad_reduce_segs P={P} nseg={nseg} (gaps untouched)")
+    _check_err(err, f"grad_reduce P={P} nseg={nseg}")
+    assert_bitwise(out.buf, out.image(_segs_body(grads, segs, scale, dst_len)), f"grad_reduce P={P} nseg={nseg} (gaps untouched)")
     part.check_guards("sumsq_partial")
     if nseg == 0:
-        assert_bitwise(part.t, part0, "grad_reduce_segs nseg=0 partials")
+        assert_bitwise(part.t, part0, "grad_reduce nseg=0 partials")
         return
     ss64 = sum(out.t[d : d + n].double().square().sum() for _, d, n in segs)
     # a thread's serial terms run through every segment; the partials it adds onto are >= 0 and part of the sum
     bound = (sum(4 * -(-n // 4 // (GR_GRID * 512)) for _, _, n in segs) + 16) * U32
-    assert_elementwise(part.t.double().sum(), ss64 + part0.double().sum(), bound, 0.0, f"grad_reduce_segs P={P} nseg={nseg} sumsq")
+    assert_elementwise(part.t.double().sum(), ss64 + part0.double().sum(), bound, 0.0, f"grad_reduce P={P} nseg={nseg} sumsq")
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("P", PEERS)
+def test_grad_reduce_abort(P):
+    """With the host watchdog's abort value in the error word and the peers' flags not yet at the epoch, the flag wait gives up and
+    the kernel returns before it reads or writes anything; once the flags are signalled and the word is cleared, the same call
+    reduces."""
+    dev = _dev()
+    segs, src_len, dst_len = _segments(16, seed=P * 29, P=P)
+    grads = [_wide(src_len, -20, 4, seed=700 + 10 * P + p, zeros=0.05).to(dev) for p in range(P)]
+    scale = _f32(1.0 / P)
+    slot_base = 2
+    flags = Out(16, torch.int32)  # 0: below EPOCH
+    out = Out(dst_len, torch.float32)
+    part = Out(GR_GRID, torch.float32, torch.rand(GR_GRID))
+    table = _lib.SegTable.of(segs)
+    err = _err()
+
+    def run():
+        _launch("pb_grad_reduce", _pref(_pp(grads)), None, ctypes.byref(table), scale, out.ptr(), part.ptr(), flags.ptr(), slot_base,
+                EPOCH, err.data_ptr(), 0, _stream())  # fmt: skip
+
+    everything = [out.buf, part.buf, flags.buf, *grads]
+    snap = [x.clone() for x in everything]
+    err[0] = 2  # the host watchdog's abort value (a software flag), as SymmetricHeap.abort() writes it
+    run()
+    torch.cuda.synchronize()
+    assert err.tolist() == [2, 0], f"grad_reduce P={P}: error word {err.tolist()}"
+    for x, s in zip(everything, snap):
+        assert bitwise_equal(x, s), f"grad_reduce P={P} wrote with the abort flag set"
+    print(f"[bitwise] grad_reduce P={P} with err = 2: every buffer untouched")
+    err.zero_()
+    for r in range(P):
+        _launch("pb_signal", _pref(_pp([flags.t])), slot_base + r, EPOCH, _stream())
+    run()
+    _check_err(err, f"grad_reduce P={P} after the abort")
+    assert_bitwise(out.buf, out.image(_segs_body(grads, segs, scale, dst_len)), f"grad_reduce P={P} after the abort")
+    for g, s in zip(grads, snap[3:]):
+        assert bitwise_equal(g, s), "grad_reduce wrote its input"
 
 
 # ================================================================================================== GPU: norm, AdamW

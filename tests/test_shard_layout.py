@@ -8,6 +8,7 @@ import pytest
 import torch
 
 from prime_b200.models.llama import Transformer, get_model_args
+from prime_b200.parallel.fsdp import reduce_segments
 from prime_b200.parallel.layout import SHARD_ALIGN, plan_layout
 
 GOLDEN = json.loads(gzip.decompress((Path(__file__).parent / "golden" / "shard_layouts.json.gz").read_bytes()))
@@ -67,3 +68,26 @@ def test_heap_bytes_cover_every_allocation(type_model, name):
         for fp32_master in (False, True):
             spare = lay.heap_bytes(fp32_master=fp32_master) - _heap_used(g, fp32_master)
             assert spare >= 64e6, (type_model, name, g["fsdp_size"], g["shard_params"], fp32_master, spare)
+
+
+@pytest.mark.parametrize("type_model,name", MODELS)
+def test_reduce_segments_follow_the_layout(type_model, name):
+    """The engine's gradient reduce-scatter tables, (offset in main_grad, offset in the shard, elements) per bucket: a flat bucket is
+    rank r's contiguous 1/F slice (at F = 1 the whole bucket, reduced in place: its shard starts where it does), a row-sharded
+    bucket is rank r's row block of every weight, in parameter order."""
+    model = _meta_model(type_model, name)
+    for g in _configs(type_model, name):
+        F = g["fsdp_size"]
+        lay = plan_layout(model, F, g["shard_params"])
+        for r in sorted({0, F // 2, F - 1}):
+            tables = reduce_segments(lay, r)
+            assert len(tables) == len(lay.buckets)
+            for b, t in zip(lay.buckets, tables):
+                got = [(t.src_off[i], t.dst_off[i], t.n[i]) for i in range(t.nseg)]
+                if b.kind == "flat":
+                    want = [(b.start + r * b.shard_size, b.shard_start, b.shard_size)]
+                    assert F > 1 or b.shard_start == b.start
+                else:
+                    want = [(b.start + off + r * (p.numel() // F), b.shard_start + soff, p.numel() // F)
+                            for (_, p, off), (soff, _) in zip(b.params, b.pieces)]  # fmt: skip
+                assert got == want, (type_model, name, F, g["shard_params"], r, b.name)

@@ -88,12 +88,11 @@ def main():
         out = torch.empty(shard, device=dev)
         ss = torch.zeros(grid, device=dev)
         pp = heap.peers(range(n), x32)
-        t = timeit(lambda: _lib.check(lib.pb_grad_reduce(ctypes.byref(pp), r * shard, shard, 1.0 / n, out.data_ptr(), ss.data_ptr(), None, 0, 0,
-                                                         heap.err.data_ptr(), 0, stream), "pb_grad_reduce"), flush)  # fmt: skip
-        row["p2p_reduce_scatter_ms"], row["p2p_rs_busbw_GBs"] = round(t, 4), round((n - 1) / n * nbytes / t / 1e6, 1)
-        t = timeit(lambda: _lib.check(lib.pb_mc_grad_reduce(heap.mc_ptr(x32), r * shard, shard, 1.0 / n, out.data_ptr(), ss.data_ptr(), None, 0, 0, n,
-                                                            heap.err.data_ptr(), 0, stream), "pb_mc_grad_reduce"), flush)  # fmt: skip
-        row["nvls_reduce_scatter_ms"], row["nvls_rs_busbw_GBs"] = round(t, 4), round((n - 1) / n * nbytes / t / 1e6, 1)
+        table = _lib.SegTable.of([(r * shard, 0, shard)])
+        for name, mc in (("p2p", None), ("nvls", heap.mc_ptr(x32))):
+            t = timeit(lambda: _lib.check(lib.pb_grad_reduce(ctypes.byref(pp), mc, ctypes.byref(table), 1.0 / n, out.data_ptr(), ss.data_ptr(),
+                                                             None, 0, 0, heap.err.data_ptr(), 0, stream), "pb_grad_reduce"), flush)  # fmt: skip
+            row[f"{name}_reduce_scatter_ms"], row[f"{name}_rs_busbw_GBs"] = round(t, 4), round((n - 1) / n * nbytes / t / 1e6, 1)
         heap.check_errors()
         rows.append(row)
         if r == 0:

@@ -52,15 +52,13 @@ PICK = [
     (r"embedding_fwd_kernel", "embedding_fwd_peer_gather"),
     (r"embedding_sort_kernel", "embedding_bwd_sort"),
     (r"embedding_bwd_kernel", "embedding_bwd_segmented"),
-    (r"^grad_reduce_kernel", "grad_reduce_p2p"),
-    (r"grad_reduce_segs_kernel", "grad_reduce_p2p_rows"),
+    (r"^grad_reduce_kernel", "grad_reduce"),
     (r"adamw_push_kernel", "adamw_push"),
     (r"norm_publish_kernel", "norm_publish"),
     (r"pseudograd_quant_kernel", "outer_pseudograd_quant"),
     (r"^outer_nesterov_kernel", "outer_nesterov_int8"),
     (r"outer_nesterov_f32_kernel", "outer_nesterov_f32"),
     (r"barrier_kernel", "flag_barrier"),
-    (r"mc_grad_reduce", "nvls_grad_reduce"),
     (r"mc_all_reduce", "nvls_all_reduce"),
 ]
 
