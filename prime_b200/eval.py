@@ -4,6 +4,7 @@
     python -m prime_b200.eval ppl --hf path/to/llama --data data/c4_val
     python -m prime_b200.eval ppl --ckpt … --model 1B --data data/c4_val --document-mask   # attention within documents only
     python -m prime_b200.eval generate --ckpt … --model 1B --prompt-ids 1,306,626 --max-new 32
+    python -m prime_b200.eval generate --ckpt … --model 1B --prompt-ids 1,306,626 --temperature 0.8 --top-p 0.9 --sampler device
 
 The model is rebuilt on one device from the per-rank optimizer shards (``checkpoint.assemble_full_model``) or from a Hugging
 Face directory (``models.hf.load_hf_dir``); the forward runs through the same ops as training (native kernels on an H100, the
@@ -22,6 +23,7 @@ import math
 import torch
 import torch.nn.functional as F
 
+from . import ops
 from .data import MemmapTokenDataset
 from .inference import generate_batch, sample
 from .models.llama import Transformer
@@ -43,29 +45,39 @@ def perplexity(model: Transformer, dataset, *, batches: int, batch_size: int, de
     return {"loss": loss, "perplexity": math.exp(min(loss, 50.0)), "tokens": n}
 
 
-def generate(model: Transformer, prompt: list[int], *, max_new: int, temperature: float = 0.0, top_k: int = 0, seed: int = 0,
-             eos_id: int | None = None) -> list[int]:  # fmt: skip
-    """Greedy (temperature 0) or top-k / temperature sampling; returns prompt + continuation."""
-    return generate_batch(model, [prompt], max_new=max_new, temperature=temperature, top_k=top_k, seed=seed, eos_id=eos_id)[0]
+def generate(model: Transformer, prompt: list[int], *, max_new: int, temperature: float = 0.0, top_k: int = 0, top_p: float = 1.0,
+             min_p: float = 0.0, seed: int = 0, eos_id: int | None = None, sampler: str = "host") -> list[int]:  # fmt: skip
+    """Greedy (temperature 0) or temperature / top-k / top-p / min-p sampling; returns prompt + continuation. ``sampler``: "host"
+    (the random stream of earlier versions) or "device" (``ops.sample_tokens``'s Philox stream), see ``generate_batch``."""
+    return generate_batch(model, [prompt], max_new=max_new, temperature=temperature, top_k=top_k, top_p=top_p, min_p=min_p, seed=seed,
+                          eos_id=eos_id, sampler=sampler)[0]  # fmt: skip
 
 
 @torch.no_grad()
-def _generate_recompute(model: Transformer, prompt: list[int], *, max_new: int, temperature: float = 0.0, top_k: int = 0, seed: int = 0,
-                        eos_id: int | None = None) -> list[int]:  # fmt: skip
+def _generate_recompute(model: Transformer, prompt: list[int], *, max_new: int, temperature: float = 0.0, top_k: int = 0,
+                        top_p: float = 1.0, min_p: float = 0.0, seed: int = 0, eos_id: int | None = None,
+                        sampler: str = "host") -> list[int]:  # fmt: skip
     """:func:`generate` without a cache: the whole prefix is run again for every token (padded to a multiple of 128 on CUDA). The
-    oracle of the cached path and the baseline of its speed-up."""
+    oracle of the cached path and the baseline of its speed-up. ``sampler="device"`` draws each token with ``ops.sample_tokens`` on
+    the model's device, keyed by ``seed`` at the token's position: row b of ``generate_batch(seed=s)`` is this with seed s + b."""
     model.eval()
     dev = next(model.parameters()).device
     ids = list(prompt)
     gen = torch.Generator(device="cpu").manual_seed(seed)
+    seeds = torch.tensor([seed], dtype=torch.int64, device=dev)
     pad_to = 128 if dev.type == "cuda" else 1
     for _ in range(max_new):
         n = len(ids)
         if n >= model.args.max_seq_len:
             break
         padded = ids + [0] * ((-n) % pad_to)
-        logits = model(torch.tensor([padded], dtype=torch.int64, device=dev))[0, n - 1].float().cpu()
-        nxt = sample(logits, temperature, top_k, gen)
+        logits = model(torch.tensor([padded], dtype=torch.int64, device=dev))[0, n - 1]
+        if sampler == "device":
+            pos = torch.tensor([n], dtype=torch.int32, device=dev)
+            nxt = int(ops.sample_tokens(logits.view(1, -1), temperature=temperature, top_k=top_k, top_p=top_p, min_p=min_p, seeds=seeds,
+                                        positions=pos)[0])  # fmt: skip
+        else:
+            nxt = sample(logits.float().cpu(), temperature, top_k, gen, top_p, min_p)
         ids.append(nxt)
         if eos_id is not None and nxt == eos_id:
             break
@@ -108,6 +120,10 @@ def main(argv: list[str] | None = None) -> dict:
     g.add_argument("--max-new", type=int, default=32)
     g.add_argument("--temperature", type=float, default=0.0)
     g.add_argument("--top-k", type=int, default=0)
+    g.add_argument("--top-p", type=float, default=1.0, help="nucleus sampling: keep the smallest top set holding this share of the mass")
+    g.add_argument("--min-p", type=float, default=0.0, help="keep tokens with at least this share of the top token's probability")
+    g.add_argument("--sampler", default="host", choices=["host", "device"],
+                   help="host: CPU generator, as earlier versions; device: sample inside the captured decode step (Philox stream)")
     g.add_argument("--seed", type=int, default=0)
     a = ap.parse_args(argv)
     model = load_model(a, a.device)
@@ -122,7 +138,8 @@ def main(argv: list[str] | None = None) -> dict:
         ds = MemmapTokenDataset(a.data, a.seq, vocab_size=model.args.vocab_size, shuffle=False)
         out = perplexity(model, ds, batches=min(a.batches, max(1, ds.windows // a.batch_size)), batch_size=a.batch_size, device=a.device)
     else:
-        ids = generate(model, [int(x) for x in a.prompt_ids.split(",")], max_new=a.max_new, temperature=a.temperature, top_k=a.top_k, seed=a.seed)
+        ids = generate(model, [int(x) for x in a.prompt_ids.split(",")], max_new=a.max_new, temperature=a.temperature, top_k=a.top_k,
+                       top_p=a.top_p, min_p=a.min_p, seed=a.seed, sampler=a.sampler)  # fmt: skip
         out = {"ids": ids}
     print(json.dumps(out))
     return out

@@ -5,6 +5,10 @@ The cache keeps, per layer, exactly the K|V columns of the fused QKV activation 
 strided copy per layer and a decode step appends one row per sequence (``ops.kv_append``) and runs split-KV attention over it
 (``ops.decode_attention``). The per-row state (``len``, ``lo``: the first key the current query may see, ``last_tok``) lives on the
 device, so a decode step depends on no host value that changes between tokens.
+
+Sampling runs on the host (one CPU generator, the stream of earlier versions) or, with ``sampler="device"``, inside the step:
+``ops.sample_tokens`` draws each row's next token from a Philox stream keyed by (seed, position), writes it into the step's static
+input buffer and applies the stop rules on the device, so the captured graph runs step after step without the host.
 """
 
 from __future__ import annotations
@@ -107,10 +111,14 @@ def prefill(model: Transformer, prompts: list[list[int]], capacity: int) -> tupl
 
 class GraphDecoder:
     """``model.decode_step`` captured once per (batch, capacity) in a CUDA graph over static token / logit buffers. A replay runs the
-    same kernels on the same buffers as the eager step, so its logits are bitwise equal."""
+    same kernels on the same buffers as the eager step, so its logits are bitwise equal.
 
-    def __init__(self, model: Transformer, cache: KVCache):
-        self.tokens = torch.zeros(cache.len.shape[0], dtype=torch.int64, device=cache.kv.device)
+    ``tokens``: use this int64 [B] buffer as the static input instead of a new one. ``then``: a function of the logits captured after
+    the step, e.g. a sampler that writes the next step's tokens into ``tokens``, so :meth:`replay` runs step after step with no host
+    work in between."""
+
+    def __init__(self, model: Transformer, cache: KVCache, tokens: torch.Tensor | None = None, then=None):
+        self.tokens = tokens if tokens is not None else torch.zeros(cache.len.shape[0], dtype=torch.int64, device=cache.kv.device)
         state = [t.clone() for t in (cache.len, cache.lo, cache.last_tok)]
         # warm-up outside the capture (library load, kernel attributes); it advances the state and writes the next cache row, so the
         # state is restored afterwards, and that row is written again by the first real step
@@ -122,6 +130,8 @@ class GraphDecoder:
         self.graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(self.graph):
             self.logits = model.decode_step(self.tokens, cache)
+            if then is not None:
+                then(self.logits)
         for t, s in zip((cache.len, cache.lo, cache.last_tok), state):
             t.copy_(s)
 
@@ -130,11 +140,21 @@ class GraphDecoder:
         self.graph.replay()
         return self.logits
 
+    def replay(self) -> None:
+        """One step on whatever the token buffer holds."""
+        self.graph.replay()
 
-def sample(logits: torch.Tensor, temperature: float, top_k: int, gen: torch.Generator) -> int:
-    """Greedy (temperature 0) or top-k / temperature sampling of one fp32 CPU logit row."""
+
+def sample(logits: torch.Tensor, temperature: float, top_k: int, gen: torch.Generator, top_p: float = 1.0, min_p: float = 0.0) -> int:
+    """Greedy (temperature 0) or temperature / top-k / top-p / min-p sampling of one fp32 CPU logit row, drawn by
+    ``torch.multinomial`` from ``gen``. With top-p or min-p on, the keep-set is ``ops.reference.sample_keep``'s, the one the device
+    sampler uses; with both off the draw is the one earlier versions made."""
     if temperature <= 0:
         return int(logits.argmax())
+    if top_p < 1.0 or min_p > 0.0:
+        keep = ops.reference.sample_keep(logits.view(1, -1), temperature, top_k, top_p, min_p)[0]
+        logits = (logits / temperature).masked_fill(~keep, float("-inf"))
+        return int(torch.multinomial(torch.softmax(logits, -1), 1, generator=gen))
     logits = logits / temperature
     if top_k > 0:
         kth = torch.topk(logits, min(top_k, logits.numel())).values[-1]
@@ -142,12 +162,48 @@ def sample(logits: torch.Tensor, temperature: float, top_k: int, gen: torch.Gene
     return int(torch.multinomial(torch.softmax(logits, -1), 1, generator=gen))
 
 
+@dataclass
+class SampleState:
+    """Per-row bookkeeping of device-side generation, updated by ``ops.sample_tokens(state=...)`` (see its docstring)."""
+
+    tokens: torch.Tensor  # int64 [B]: the next decode step's input; a finished row keeps its last token
+    history: torch.Tensor  # int64 [B, max_new]: the new tokens
+    n_out: torch.Tensor  # int32 [B]
+    active: torch.Tensor  # bool [B]
+    prompt_len: torch.Tensor  # int32 [B]
+    max_seq_len: int
+    eos_id: int | None
+
+    @classmethod
+    def allocate(cls, prompts: list[list[int]], max_new: int, max_seq_len: int, eos_id: int | None, device) -> "SampleState":
+        lens = [len(p) for p in prompts]
+        return cls(torch.tensor([p[-1] for p in prompts], dtype=torch.int64, device=device),
+                   torch.zeros((len(prompts), max_new), dtype=torch.int64, device=device),
+                   torch.zeros(len(prompts), dtype=torch.int32, device=device),
+                   torch.tensor([n < max_seq_len for n in lens], dtype=torch.bool, device=device),
+                   torch.tensor(lens, dtype=torch.int32, device=device), max_seq_len, eos_id)  # fmt: skip
+
+
+CHECK_EVERY = 16  # device-sampled generation reads the "any row still active" flag once per this many steps
+
+
 @torch.no_grad()
-def generate_batch(model: Transformer, prompts: list[list[int]], *, max_new: int, temperature: float = 0.0, top_k: int = 0, seed: int = 0,
-                   eos_id: int | None = None, graphs: bool | None = None) -> list[list[int]]:  # fmt: skip
+def generate_batch(model: Transformer, prompts: list[list[int]], *, max_new: int, temperature: float = 0.0, top_k: int = 0,
+                   top_p: float = 1.0, min_p: float = 0.0, seed: int = 0, eos_id: int | None = None, graphs: bool | None = None,
+                   sampler: str = "host") -> list[list[int]]:  # fmt: skip
     """Prompt + continuation of every prompt. A row stops at ``max_new`` new tokens, at ``model.args.max_seq_len`` tokens in all, or
-    after ``eos_id``. Rows are sampled in order from one CPU generator seeded with ``seed``. ``graphs``: replay the decode step from
-    a CUDA graph (default: on CUDA)."""
+    after ``eos_id`` (kept). ``graphs``: replay the decode step from a CUDA graph (default: on CUDA).
+
+    ``sampler`` picks the random stream as well as where sampling runs:
+
+    * ``"host"`` (default): each step's logits are copied to the host and the rows are sampled in order from one CPU generator
+      seeded with ``seed`` (:func:`sample`). It reproduces the seeded outputs of earlier versions.
+    * ``"device"``: ``ops.sample_tokens`` draws on the device from a Philox stream keyed by ``seed + b`` for row b at each token's
+      position, so a row's draws do not depend on the other rows. The first token comes from the prefill logits; on CUDA each later
+      step (decode step, sampler and bookkeeping) is one CUDA graph replay writing its own next input, and the host reads a
+      "still active" flag once every 16 steps and the tokens once at the end. Greedy tokens are the same under both samplers."""
+    if sampler not in ("host", "device"):
+        raise ValueError(f"sampler must be 'host' or 'device', got {sampler!r}")
     model.eval()
     dev = model.output.device
     ids = [list(p) for p in prompts]
@@ -155,9 +211,13 @@ def generate_batch(model: Transformer, prompts: list[list[int]], *, max_new: int
     active = [len(p) < limit for p in ids]
     if max_new <= 0 or not any(active):
         return ids
+    use_graphs = graphs if graphs is not None else dev.type == "cuda"
+    if sampler == "device":
+        return _generate_device(model, ids, max_new, dict(temperature=temperature, top_k=top_k, top_p=top_p, min_p=min_p), seed,
+                                eos_id, use_graphs)  # fmt: skip
     gen = torch.Generator(device="cpu").manual_seed(seed)
     logits, cache = prefill(model, ids, cache_capacity(limit, [len(p) for p in ids], max_new))
-    if graphs if graphs is not None else dev.type == "cuda":
+    if use_graphs:
         step = GraphDecoder(model, cache)
     else:
         step = lambda t: model.decode_step(t, cache)  # noqa: E731
@@ -166,7 +226,7 @@ def generate_batch(model: Transformer, prompts: list[list[int]], *, max_new: int
         for b, row in enumerate(ids):
             if not active[b]:
                 continue
-            nxt = sample(rows[b], temperature, top_k, gen)
+            nxt = sample(rows[b], temperature, top_k, gen, top_p, min_p)
             row.append(nxt)
             active[b] = len(row) < limit and not (eos_id is not None and nxt == eos_id)
         if i == max_new - 1 or not any(active):
@@ -174,3 +234,29 @@ def generate_batch(model: Transformer, prompts: list[list[int]], *, max_new: int
         # finished rows keep feeding their last token; their logits are never read (and past the capacity nothing is written)
         logits = step(torch.tensor([row[-1] for row in ids], dtype=torch.int64, device=dev))
     return ids
+
+
+def _generate_device(model: Transformer, ids: list[list[int]], max_new: int, knobs: dict, seed: int, eos_id: int | None,
+                     graphs: bool) -> list[list[int]]:  # fmt: skip
+    """``generate_batch(sampler="device")``: sampling, the next step's input and the stop rules all stay on the device."""
+    dev = model.output.device
+    limit = model.args.max_seq_len
+    logits, cache = prefill(model, ids, cache_capacity(limit, [len(p) for p in ids], max_new))
+    st = SampleState.allocate(ids, max_new, limit, eos_id, dev)
+    seeds = torch.tensor([seed + b for b in range(len(ids))], dtype=torch.int64, device=dev)
+
+    def draw(lg: torch.Tensor) -> None:  # the position of the token drawn is the row's cache length
+        ops.sample_tokens(lg, **knobs, seeds=seeds, positions=cache.len, out=st.tokens, state=st)
+
+    draw(logits)
+    if max_new > 1:
+        if graphs:
+            advance = GraphDecoder(model, cache, tokens=st.tokens, then=draw).replay
+        else:
+            advance = lambda: draw(model.decode_step(st.tokens, cache))  # noqa: E731
+        for i in range(max_new - 1):
+            if i % CHECK_EVERY == 0 and not bool(st.active.any()):
+                break
+            advance()
+    hist, n = st.history.cpu(), st.n_out.cpu()
+    return [p + hist[b, : int(n[b])].tolist() for b, p in enumerate(ids)]

@@ -916,3 +916,79 @@ def decode_attention(qkv: torch.Tensor, kv: torch.Tensor, length: torch.Tensor, 
         return out
     q = qkv.view(B, H + 2 * Hkv, D)[:, :H]
     return reference.decode_attention(q, kv, length, lo, window).reshape(B, H * D).to(qkv.dtype)
+
+
+# --------------------------------------------------------------------------- sampling
+
+
+def _sample_args(temperature: float, top_k: int, top_p: float, min_p: float) -> None:
+    if not (math.isfinite(temperature) and temperature >= 0):
+        raise ValueError(f"temperature must be finite and >= 0, got {temperature}")
+    if top_k < 0:
+        raise ValueError(f"top_k must be >= 0 (0 = off), got {top_k}")
+    if not 0 < top_p <= 1:
+        raise ValueError(f"top_p must be in (0, 1] (1 = off), got {top_p}")
+    if not 0 <= min_p <= 1:
+        raise ValueError(f"min_p must be in [0, 1] (0 = off), got {min_p}")
+
+
+def sample_tokens(logits: torch.Tensor, *, temperature: float = 0.0, top_k: int = 0, top_p: float = 1.0, min_p: float = 0.0,
+                  seeds: torch.Tensor, positions: torch.Tensor, out: torch.Tensor | None = None, state=None) -> torch.Tensor:  # fmt: skip
+    """One token per row of ``logits`` [B, V] → int64 [B] (``out`` if given).
+
+    The contract, shared by the native kernel (csrc/sample_sm90.cu: CUDA bf16 logits with unit column stride) and
+    :func:`reference.sample_tokens` (everything else; no host synchronisation, so a CUDA graph can capture it too):
+
+    * Greedy: ``temperature == 0`` returns the argmax, the lowest index among tied maxima (``torch.argmax``); the other knobs are
+      ignored.
+    * Otherwise ``p_i ∝ exp((l_i − l_max) / T)``, and the filters apply in Hugging Face order, temperature → top-k → top-p → min-p.
+      Each keeps an upper set of the logit order, tie groups (equal logits) whole, so the keep-set is ``{i : l_i >= t*}``:
+
+      - top-k (``k > 0``): every token whose logit is at least the k-th largest (ties may keep more than k; ``k >= V`` keeps all).
+      - top-p (``0 < p <= 1``, 1 = off): on the top-k set S, the largest threshold t with ``mass{i ∈ S : p_i >= t} >= p·mass(S)``;
+        keeps ``S ∩ {p_i >= t}``, so the tie group that crosses p stays whole.
+      - min-p (``0 <= m <= 1``, 0 = off): keeps ``p_i >= m·p_max``, i.e. ``l_i >= l_max + T·ln m``.
+    * Draw: the inverse CDF in vocabulary index order over the kept set. With ``target = u·mass(kept)`` the token is the first kept
+      index whose inclusive prefix mass exceeds ``target``, or, should rounding leave none, the last kept index.
+    * Random stream: Philox4x32-10 with key = the row's 64-bit seed (``seeds`` int64 [B]: lo, hi words) and counter =
+      ``(position, 0, 0, 0)`` (``positions`` int32 [B]: the index in its row of the token being drawn), so a draw depends on nothing
+      but (seed, row position); ``u = ((x0 >> 8) + 0.5)·2^-24``.
+
+    Both implementations compute ``p_i`` in fp64 (``exp((l_i − l_max)·(1/T))`` with T the fp32 value, ``p_max = 1``), round it to
+    a 2^-40 fixed-point integer and sum masses in integers, so every sum (the top-p mass, the prefix of the draw) is exact in any
+    order and the kernel is deterministic; ``p·mass(S)`` is compared in fp64 and the min-p bound is ``l_max + fp32(T·ln m)`` in fp32.
+    They can differ only where two fp64 ``exp`` results round to different fixed-point integers.
+
+    ``state``: bookkeeping of a generation loop (``inference.SampleState``). An inactive row (``state.active[b]`` false) writes
+    nothing, so ``out`` keeps its last token; an active row writes its token to ``out`` and ``state.history[b, state.n_out[b]]``,
+    increments ``n_out`` and goes inactive at ``history.shape[1]`` new tokens, at ``prompt_len + n_out == max_seq_len``, or after
+    ``eos_id`` (kept in the output)."""
+    if logits.dim() != 2:
+        raise ValueError(f"logits must be [B, V], got {tuple(logits.shape)}")
+    _sample_args(temperature, top_k, top_p, min_p)
+    B, V = logits.shape
+    if out is None:
+        out = torch.empty(B, dtype=torch.int64, device=logits.device)
+    if logits.is_cuda and logits.dtype == torch.bfloat16 and logits.stride(1) == 1:
+        assert seeds.dtype == out.dtype == torch.int64 and positions.dtype == torch.int32
+        assert seeds.is_contiguous() and positions.is_contiguous() and out.is_contiguous()
+        book = [None] * 4
+        max_new = max_seq = 0
+        eos = -1
+        if state is not None:
+            assert state.history.dtype == torch.int64 and state.n_out.dtype == torch.int32 and state.active.dtype == torch.bool
+            assert state.prompt_len.dtype == torch.int32 and state.history.is_contiguous()
+            book = [state.history.data_ptr(), state.n_out.data_ptr(), state.active.data_ptr(), state.prompt_len.data_ptr()]
+            max_new, max_seq = state.history.shape[1], state.max_seq_len
+            eos = -1 if state.eos_id is None else int(state.eos_id)
+        _launch("pb_sample_tokens", logits.data_ptr(), logits.stride(0) if B > 1 else V, B, V, float(temperature), int(top_k),
+                float(top_p), float(min_p), seeds.data_ptr(), positions.data_ptr(), out.data_ptr(), *book, max_new, max_seq, eos,
+                _stream())  # fmt: skip
+        return out
+    tok = reference.sample_tokens(logits, temperature, top_k, top_p, min_p, seeds, positions)
+    if state is None:
+        out.copy_(tok)
+    else:
+        reference.sample_bookkeeping(tok, out, state.history, state.n_out, state.active, state.prompt_len, state.max_seq_len,
+                                     state.eos_id)  # fmt: skip
+    return out

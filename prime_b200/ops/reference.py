@@ -135,6 +135,118 @@ def decode_attention(q: torch.Tensor, kv: torch.Tensor, length: torch.Tensor, lo
     return torch.einsum("bhk,bkhd->bhd", p, vf.masked_fill(~visible.view(B, cap, 1, 1), 0.0))
 
 
+# ----------------------------------------------------------------------------------------------------------- sampling
+# The contract is stated in ``ops.sample_tokens``. Nothing below reads a value back to the host, so on CUDA the fallback can be
+# captured in a CUDA graph like the native kernel.
+MASS_UNIT = 2.0**40  # fixed-point scale of a token's mass p_i in [0, 1]: every mass sum is an exact int64 sum
+_M32 = 0xFFFFFFFF
+
+
+def _mulhilo32(a: int, b: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor]:
+    """(hi, lo) 32-bit words of the 64-bit product of the constant a and the uint32 values in int64 tensor b, without overflow."""
+    p_lo = a * (b & 0xFFFF)  # < 2^48
+    p_hi = a * (b >> 16)  # < 2^48
+    t = p_lo + ((p_hi & 0xFFFF) << 16)
+    return (p_hi >> 16) + (t >> 32), t & _M32
+
+
+def philox4x32_10(key: torch.Tensor, counter: torch.Tensor) -> torch.Tensor:
+    """Philox4x32-10 (Salmon et al., SC'11) in int64 arithmetic: key int64 [..., 2], counter int64 [..., 4] (uint32 words) → the
+    four uint32 output words [..., 4]."""
+    k0, k1 = key[..., 0] & _M32, key[..., 1] & _M32
+    c0, c1, c2, c3 = (counter[..., i] & _M32 for i in range(4))
+    for r in range(10):
+        if r:
+            k0, k1 = (k0 + 0x9E3779B9) & _M32, (k1 + 0xBB67AE85) & _M32
+        hi0, lo0 = _mulhilo32(0xD2511F53, c0)
+        hi1, lo1 = _mulhilo32(0xCD9E8D57, c2)
+        c0, c1, c2, c3 = hi1 ^ c1 ^ k0, lo1, hi0 ^ c3 ^ k1, lo0
+    return torch.stack((c0, c1, c2, c3), dim=-1)
+
+
+def sample_uniform_bits(seeds: torch.Tensor, positions: torch.Tensor) -> torch.Tensor:
+    """r = x0 >> 8 (24 bits, int64 [B]) of Philox4x32-10 with key = the 64-bit seed and counter = (position, 0, 0, 0); the draw's
+    u = (r + 0.5)·2^-24."""
+    s = seeds.long()
+    key = torch.stack((s & _M32, (s >> 32) & _M32), dim=-1)
+    z = torch.zeros_like(s)
+    return philox4x32_10(key, torch.stack((positions.long() & _M32, z, z, z), dim=-1))[..., 0] >> 8
+
+
+def _f32(x: float) -> float:
+    return float(torch.tensor(x, dtype=torch.float32))
+
+
+def sample_masses(logits: torch.Tensor, temperature: float) -> torch.Tensor:
+    """Fixed-point masses int64 [B, V]: p_i = exp((l_i - l_max)·(1/T)) in fp64 (T the fp32 value), times 2^40, rounded."""
+    lf = logits.float()
+    x = (lf.double() - lf.amax(-1, keepdim=True).double()) * (1.0 / _f32(temperature))
+    return (torch.exp(x) * MASS_UNIT).round().long()
+
+
+def sample_keep(logits: torch.Tensor, temperature: float, top_k: int = 0, top_p: float = 1.0, min_p: float = 0.0,
+                mass: torch.Tensor | None = None) -> torch.Tensor:  # fmt: skip
+    """Keep-set bool [B, V] of temperature > 0 sampling: top-k, then top-p on the top-k set, then min-p, each an upper set of the
+    logit order with tie groups kept whole (the contract of ``ops.sample_tokens``). Sort-based; masses from :func:`sample_masses`."""
+    lf = logits.float()
+    B, V = lf.shape
+    if mass is None:
+        mass = sample_masses(lf, temperature)
+    lmax = lf.amax(-1, keepdim=True)
+    keep = torch.ones((B, V), dtype=torch.bool, device=lf.device)
+    if (top_k > 0 and top_k < V) or top_p < 1.0:
+        ls, idx = lf.sort(dim=-1, descending=True, stable=True)
+        t = torch.full_like(lmax, -math.inf)
+        if top_k > 0 and top_k < V:
+            t = ls[:, top_k - 1 : top_k]  # the k-th largest logit: its whole tie group stays
+        if top_p < 1.0:
+            in_s = ls >= t
+            cum = torch.where(in_s, mass.gather(1, idx), 0).cumsum(-1)
+            need = cum[:, -1:].double() * _f32(top_p)
+            j = (cum.double() < need).sum(-1, keepdim=True)  # first sorted position whose inclusive mass reaches need
+            t = torch.maximum(t, ls.gather(1, j.clamp(max=V - 1)))
+        keep = lf >= t
+    if min_p > 0.0:
+        off = _f32(_f32(temperature) * math.log(_f32(min_p)))
+        keep &= lf >= lmax + torch.tensor(off, dtype=torch.float32, device=lf.device)
+    return keep
+
+
+def sample_tokens(logits: torch.Tensor, temperature: float, top_k: int, top_p: float, min_p: float, seeds: torch.Tensor,
+                  positions: torch.Tensor) -> torch.Tensor:  # fmt: skip
+    """One token per row of logits [B, V] → int64 [B], by the contract of ``ops.sample_tokens``: fp32 logits, fp64 masses rounded to
+    fixed point, int64 mass sums."""
+    lf = logits.float()
+    if temperature == 0:
+        return lf.argmax(-1)
+    B, V = lf.shape
+    mass = sample_masses(lf, temperature)
+    keep = sample_keep(lf, temperature, top_k, top_p, min_p, mass)
+    cum = torch.where(keep, mass, 0).cumsum(-1)
+    M = cum[:, -1]
+    a = 2 * sample_uniform_bits(seeds.to(lf.device), positions.to(lf.device)) + 1  # u·M = (2r + 1)·M / 2^25, in int64
+    target = a * (M >> 25) + ((a * (M & (2**25 - 1))) >> 25)
+    tok = (cum <= target.view(B, 1)).sum(-1)
+    last = torch.where(keep, torch.arange(V, device=lf.device), -1).amax(-1)
+    return torch.where(tok < V, tok, last)
+
+
+def sample_bookkeeping(tokens: torch.Tensor, out: torch.Tensor, history: torch.Tensor, n_out: torch.Tensor, active: torch.Tensor,
+                       prompt_len: torch.Tensor, max_seq_len: int, eos_id: int | None) -> None:  # fmt: skip
+    """The bookkeeping of ``ops.sample_tokens(state=...)``, in place: an active row writes its token to ``out`` and to
+    ``history[b, n_out[b]]``, counts it, and stops at ``max_new`` tokens, at ``max_seq_len`` in all, or after ``eos_id``."""
+    max_new = history.shape[1]
+    act = active.bool()
+    out.copy_(torch.where(act, tokens, out))
+    col = n_out.long().clamp(max=max_new - 1).view(-1, 1)
+    history.scatter_(1, col, torch.where(act.view(-1, 1), tokens.view(-1, 1), history.gather(1, col)))
+    n_out.add_(act.to(n_out.dtype))
+    stop = (n_out >= max_new) | (prompt_len + n_out >= max_seq_len)
+    if eos_id is not None:
+        stop |= tokens == eos_id
+    active.copy_(act & ~stop)
+
+
 def cross_entropy(logits: torch.Tensor, targets: torch.Tensor, ignore_index: int = -100) -> torch.Tensor:
     return F.cross_entropy(logits.float().view(-1, logits.shape[-1]), targets.view(-1), ignore_index=ignore_index)
 

@@ -1,6 +1,6 @@
-"""KV-cache decoding on one GPU: the split-KV decode-attention kernel against SDPA, and end-to-end generation.
+"""KV-cache decoding on one GPU: the split-KV decode-attention kernel against SDPA, end-to-end generation, and device sampling.
 
-    python tools/decode_bench.py [--out results.json] [--skip-e2e]
+    python tools/decode_bench.py [--out results.json] [--skip-e2e] [--only-sampler]
 
 Kernel section: ``ops.decode_attention`` (pb_decode_attn, split policy of pb_decode_attn_splits) at 1B heads (H = Hkv = 16) and
 Llama-3-8B heads (H = 32, Hkv = 8), D = 128, B ∈ {1, 8, 32} × context ∈ {1 K, 8 K, 32 K}, plus one windowed case; every row sees
@@ -12,6 +12,13 @@ same process.
 End-to-end section: a random-init Llama-2 1B, prompt 512, 256 new tokens, greedy, B ∈ {1, 8}: tokens/s of cached generation with
 CUDA graphs, cached generation eager, and the recompute loop (``eval._generate_recompute``, one row at a time). Also the share of
 one eager decode step's kernel time spent in the M = B GEMMs (torch.profiler, a separate pass).
+
+Sampler sections: ``ops.sample_tokens`` (pb_sample_tokens) alone at V ∈ {32000, 128256}, B ∈ {1, 8, 64}, greedy and T = 0.8 /
+top_p = 0.9, timed like the kernel section (bytes = the logits read once); then 1B generation with ``sampler="device"`` next to
+``"host"`` at B ∈ {1, 8}, greedy and T = 0.8 / top_p = 0.9, the two alternating in one process, with the sampler's share of one
+device-loop step's kernel time (torch.profiler).
+
+    python tools/decode_bench.py --only-sampler
 """
 
 from __future__ import annotations
@@ -149,19 +156,102 @@ def gemm_share(model, prompts, capacity: int) -> float:
     return round(gemm / tot, 3) if tot else float("nan")
 
 
+SAMPLE_KNOBS = {"greedy": dict(temperature=0.0), "T0.8_p0.9": dict(temperature=0.8, top_p=0.9)}
+
+
+def sampler_kernel_section(flush) -> list[dict]:
+    rows = []
+    dev = torch.device("cuda", 0)
+    for V in (32000, 128256):
+        for B in (1, 8, 64):
+            logits = (torch.randn(B, V, device=dev) * 3).to(torch.bfloat16)
+            seeds = torch.arange(B, dtype=torch.int64, device=dev)
+            pos = torch.full((B,), 600, dtype=torch.int32, device=dev)
+            out = torch.empty(B, dtype=torch.int64, device=dev)
+            for name, knobs in SAMPLE_KNOBS.items():
+                ms = timed(lambda: ops.sample_tokens(logits, **knobs, seeds=seeds, positions=pos, out=out), flush)
+                nbytes = B * V * 2
+                r = {"sampler": name, "V": V, "B": B, "us": round(ms * 1e3, 1), "bytes": nbytes, "GB_s": round(nbytes / ms / 1e6, 1)}
+                print(json.dumps(r), flush=True)
+                rows.append(r)
+    return rows
+
+
+def sampler_e2e_section(prompt_len: int = 512, new: int = 256, rounds: int = 2) -> list[dict]:
+    model = build_model("1B", device="cuda", dtype=torch.bfloat16, seed=0).eval()
+    g = torch.Generator().manual_seed(0)
+    rows = []
+    for B in (1, 8):
+        prompts = [torch.randint(0, model.args.vocab_size, (prompt_len,), generator=g).tolist() for _ in range(B)]
+        for name, knobs in SAMPLE_KNOBS.items():
+            r = {"B": B, "sampling": name, "prompt": prompt_len, "new_tokens": new, "card": card()}
+            best = {}
+            for sampler in ("host", "device"):
+                ev.generate_batch(model, prompts, max_new=8, sampler=sampler, **knobs)  # warm-up
+            for _ in range(rounds):  # alternate, keep each arm's best
+                for sampler in ("host", "device"):
+                    torch.cuda.synchronize()
+                    t = time.perf_counter()
+                    out = ev.generate_batch(model, prompts, max_new=new, sampler=sampler, **knobs)
+                    torch.cuda.synchronize()
+                    tok_s = sum(len(o) - prompt_len for o in out) / (time.perf_counter() - t)
+                    best[sampler] = max(best.get(sampler, 0.0), tok_s)
+            r["host_tok_s"], r["device_tok_s"] = round(best["host"], 1), round(best["device"], 1)
+            r["device_over_host"] = round(best["device"] / best["host"], 3)
+            r["sampler_share_of_device_step"] = sampler_share(model, prompts, prompt_len + new, knobs)
+            print(json.dumps(r), flush=True)
+            rows.append(r)
+    return rows
+
+
+@torch.no_grad()
+def sampler_share(model, prompts, capacity: int, knobs: dict) -> float:
+    """Share of one device-loop step's CUDA kernel time (decode step + sample_tokens, eager) spent in the sampling kernel."""
+    from torch.profiler import ProfilerActivity, profile
+
+    logits, cache = inference.prefill(model, prompts, inference.cache_capacity(model.args.max_seq_len, [len(p) for p in prompts], capacity))
+    B = len(prompts)
+    tok = torch.zeros(B, dtype=torch.int64, device="cuda")
+    seeds = torch.arange(B, dtype=torch.int64, device="cuda")
+
+    def step():
+        ops.sample_tokens(model.decode_step(tok, cache), **knobs, seeds=seeds, positions=cache.len, out=tok)
+
+    for _ in range(3):
+        step()
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(5):
+            step()
+        torch.cuda.synchronize()
+    tot = samp = 0.0
+    for e in prof.key_averages():
+        t = e.device_time_total
+        tot += t
+        if "sample_tokens" in e.key:
+            samp += t
+    return round(samp / tot, 4) if tot else float("nan")
+
+
 def main() -> None:
     ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
     ap.add_argument("--out", default=None, help="also write the results as JSON here")
     ap.add_argument("--skip-e2e", action="store_true")
+    ap.add_argument("--only-sampler", action="store_true", help="run only the two sampler sections")
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("decode_bench needs a CUDA device")
     info = card()
     print(json.dumps({"card": info}), flush=True)
     flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")
-    res = {"card": info, "kernel": kernel_section(flush)}
+    res = {"card": info}
+    if not a.only_sampler:
+        res["kernel"] = kernel_section(flush)
+    res["sampler_kernel"] = sampler_kernel_section(flush)
     if not a.skip_e2e:
-        res["e2e"] = e2e_section()
+        if not a.only_sampler:
+            res["e2e"] = e2e_section()
+        res["sampler_e2e"] = sampler_e2e_section()
     if a.out:
         Path(a.out).parent.mkdir(parents=True, exist_ok=True)
         Path(a.out).write_text(json.dumps(res, indent=1))
