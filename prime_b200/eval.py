@@ -5,6 +5,7 @@
     python -m prime_b200.eval ppl --ckpt … --model 1B --data data/c4_val --document-mask   # attention within documents only
     python -m prime_b200.eval generate --ckpt … --model 1B --prompt-ids 1,306,626 --max-new 32
     python -m prime_b200.eval generate --ckpt … --model 1B --prompt-ids 1,306,626 --temperature 0.8 --top-p 0.9 --sampler device
+    python -m prime_b200.eval generate --ckpt … --model 1B --draft-ckpt … --draft-model 150M --spec-k 4 --prompt-ids 1,306,626
 
 The model is rebuilt on one device from the per-rank optimizer shards (``checkpoint.assemble_full_model``) or from a Hugging
 Face directory (``models.hf.load_hf_dir``); the forward runs through the same ops as training (native kernels on an H100, the
@@ -25,7 +26,7 @@ import torch.nn.functional as F
 
 from . import ops
 from .data import MemmapTokenDataset
-from .inference import generate_batch, sample
+from .inference import generate_batch, generate_speculative, sample
 from .models.llama import Transformer
 
 
@@ -84,15 +85,18 @@ def _generate_recompute(model: Transformer, prompt: list[int], *, max_new: int, 
     return ids
 
 
-def load_model(a, device: str) -> Transformer:
+def load_model(a, device: str, prefix: str = "") -> Transformer:
+    """The model named by ``--ckpt`` / ``--hf`` / ``--model`` / ``--type-model`` (``prefix="draft_"``: the ``--draft-*`` ones)."""
     dtype = torch.bfloat16 if device.startswith("cuda") else torch.float32
-    if a.hf:
+    hf = getattr(a, prefix + "hf")
+    if hf:
         from .models.hf import load_hf_dir
 
-        return load_hf_dir(a.hf, device=device, dtype=dtype)
+        return load_hf_dir(hf, device=device, dtype=dtype)
     from .checkpoint import assemble_full_model
 
-    return assemble_full_model(a.ckpt, a.model, a.type_model).to(device=device, dtype=dtype)
+    return assemble_full_model(getattr(a, prefix + "ckpt"), getattr(a, prefix + "model"), getattr(a, prefix + "type_model")).to(
+        device=device, dtype=dtype)  # fmt: skip
 
 
 def main(argv: list[str] | None = None) -> dict:
@@ -125,7 +129,16 @@ def main(argv: list[str] | None = None) -> dict:
     g.add_argument("--sampler", default="host", choices=["host", "device"],
                    help="host: CPU generator, as earlier versions; device: sample inside the captured decode step (Philox stream)")
     g.add_argument("--seed", type=int, default=0)
+    dsrc = g.add_mutually_exclusive_group()
+    dsrc.add_argument("--draft-ckpt", help="speculative decoding: the draft model's checkpoint step directory")
+    dsrc.add_argument("--draft-hf", help="speculative decoding: the draft model's Hugging Face directory")
+    g.add_argument("--draft-model", default="150M")
+    g.add_argument("--draft-type-model", default="llama2", choices=["llama2", "llama3"])
+    g.add_argument("--spec-k", type=int, default=4, help="draft tokens per speculative round")
     a = ap.parse_args(argv)
+    spec = a.cmd == "generate" and (a.draft_ckpt or a.draft_hf)
+    if spec and a.sampler == "host":
+        raise SystemExit("speculative decoding samples on the device: --sampler host cannot be combined with a draft model")
     model = load_model(a, a.device)
     if a.cmd == "ppl":
         if a.document_mask or a.eos_id is not None:
@@ -137,6 +150,12 @@ def main(argv: list[str] | None = None) -> dict:
             model.doc_eos_id = eos
         ds = MemmapTokenDataset(a.data, a.seq, vocab_size=model.args.vocab_size, shuffle=False)
         out = perplexity(model, ds, batches=min(a.batches, max(1, ds.windows // a.batch_size)), batch_size=a.batch_size, device=a.device)
+    elif spec:
+        r = generate_speculative(model, load_model(a, a.device, "draft_"), [[int(x) for x in a.prompt_ids.split(",")]], k=a.spec_k,
+                                 max_new=a.max_new, temperature=a.temperature, top_k=a.top_k, top_p=a.top_p, min_p=a.min_p,
+                                 seed=a.seed)  # fmt: skip
+        out = {"ids": r.ids[0], "spec": {"rounds": r.rounds, "drafted": r.drafted, "accepted": r.accepted,
+                                         "acceptance": r.accepted / max(r.drafted, 1)}}  # fmt: skip
     else:
         ids = generate(model, [int(x) for x in a.prompt_ids.split(",")], max_new=a.max_new, temperature=a.temperature, top_k=a.top_k,
                        top_p=a.top_p, min_p=a.min_p, seed=a.seed, sampler=a.sampler)  # fmt: skip

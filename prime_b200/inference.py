@@ -34,6 +34,7 @@ class LayerKV:
     cache: "KVCache"
     index: int
     decoding: bool
+    verifying: bool = False  # a speculative verify step: T tokens per row
 
     @property
     def kv(self) -> torch.Tensor:
@@ -53,13 +54,14 @@ class KVCache:
     cos: torch.Tensor  # fp32 [>= capacity, D/2] RoPE tables, held here so a captured graph's pointers stay valid
     sin: torch.Tensor
     window: int | None  # ModelArgs.sliding_window
+    lo_q: torch.Tensor | None = None  # int32 [B, T]: each query's document start in the last verify step
 
     @property
     def capacity(self) -> int:
         return self.kv.shape[2]
 
-    def layer(self, i: int, decoding: bool = False) -> LayerKV:
-        return LayerKV(self, i, decoding)
+    def layer(self, i: int, decoding: bool = False, verifying: bool = False) -> LayerKV:
+        return LayerKV(self, i, decoding, verifying)
 
     @classmethod
     def allocate(cls, model: Transformer, batch: int, capacity: int, device) -> "KVCache":
@@ -260,3 +262,108 @@ def _generate_device(model: Transformer, ids: list[list[int]], max_new: int, kno
             advance()
     hist, n = st.history.cpu(), st.n_out.cpu()
     return [p + hist[b, : int(n[b])].tolist() for b, p in enumerate(ids)]
+
+
+# ----------------------------------------------------------------------------------------------------------- speculative decoding
+MAX_SPEC_K = 15  # drafts per round, the accept kernel's limit
+
+
+@dataclass
+class SpecResult:
+    ids: list[list[int]]  # prompt + continuation of every prompt
+    rounds: int  # rounds of the row that ran the most
+    drafted: int  # draft tokens proposed, over all rows and rounds
+    accepted: int  # of those, accepted by the target
+
+
+@torch.no_grad()
+def generate_speculative(model: Transformer, draft: Transformer, prompts: list[list[int]], *, k: int = 4, max_new: int,
+                         temperature: float = 0.0, top_k: int = 0, top_p: float = 1.0, min_p: float = 0.0, seed: int = 0,
+                         eos_id: int | None = None, graphs: bool | None = None) -> SpecResult:  # fmt: skip
+    """Speculative decoding: ``draft`` proposes ``k`` tokens per round and ``model`` checks them in one verify step; the output has the
+    distribution of ``generate_batch(sampler="device")`` with the same knobs, and greedy output is the target's greedy output.
+
+    Both models are prefilled and the first token is drawn from the target's prefill logits with ``ops.sample_tokens``. Then, per
+    round and row, with cache length L and the pending token x at index L:
+
+    1. The draft runs k + 1 decode steps on x, d_1 .. d_k; after step i <= k it draws d_i (index L + i) with ``ops.sample_tokens``
+       (the same knobs, Philox counter (L + i, 0, 0, 0)). The last step only puts d_k into the draft's cache.
+    2. The target runs one verify step (:meth:`Transformer.verify_step`) on [x, d_1 .. d_k] at indices L .. L + k.
+    3. ``ops.spec_accept`` accepts a prefix d_1 .. d_n by the exact rejection rule (Leviathan et al. 2023, Chen et al. 2023), draws
+       y from the residual or, when all k are accepted, from p_{k+1}, and emits d_1 .. d_n, y through the stop rules of
+       ``generate_batch`` (``max_new``, ``model.args.max_seq_len``, ``eos_id`` kept). Both caches keep the accepted prefix and y is
+       pending. Document masking (``doc_eos_id``) and sliding windows keep their meaning inside the verify step.
+
+    On CUDA (``graphs`` default) one whole round is one CUDA graph replay over static buffers; the host reads the "any row active"
+    flag every 16 rounds and the history once at the end. Without graphs the same calls run eagerly; on the CPU through the
+    reference ops. Each model keeps its own window, head dimension and GQA ratio; the vocabulary, device and ``doc_eos_id`` must
+    match."""
+    if draft.args.vocab_size != model.args.vocab_size:
+        raise ValueError(f"draft vocabulary {draft.args.vocab_size} != target vocabulary {model.args.vocab_size}")
+    if draft.output.device != model.output.device:
+        raise ValueError(f"draft on {draft.output.device}, target on {model.output.device}")
+    if draft.doc_eos_id != model.doc_eos_id:
+        raise ValueError(f"draft doc_eos_id {draft.doc_eos_id} != target doc_eos_id {model.doc_eos_id}")
+    if not 1 <= k <= MAX_SPEC_K:
+        raise ValueError(f"k must be in [1, {MAX_SPEC_K}], got {k}")
+    ops.functional._sample_args(temperature, top_k, top_p, min_p)
+    model.eval()
+    draft.eval()
+    dev = model.output.device
+    ids = [list(p) for p in prompts]
+    limit = model.args.max_seq_len
+    if max_new <= 0 or not any(len(p) < limit for p in ids):
+        return SpecResult(ids, 0, 0, 0)
+    B = len(ids)
+    cap = _round_up(cache_capacity(limit, [len(p) for p in ids], max_new) + k + 1, PAD)
+    logits, cache = prefill(model, ids, cap)
+    _, dcache = prefill(draft, ids, cap)
+    st = SampleState.allocate(ids, max_new, limit, eos_id, dev)
+    knobs = dict(temperature=temperature, top_k=top_k, top_p=top_p, min_p=min_p)
+    seeds = torch.tensor([seed + b for b in range(B)], dtype=torch.int64, device=dev)
+    xs = torch.zeros((k + 1, B), dtype=torch.int64, device=dev)  # the round's inputs: xs[0] = the pending token, xs[i] = d_i
+    qbuf = torch.empty((k, B, model.args.vocab_size), dtype=logits.dtype, device=dev)
+    drafted = torch.zeros(B, dtype=torch.int64, device=dev)
+    accepted = torch.zeros(B, dtype=torch.int64, device=dev)
+    ops.sample_tokens(logits, **knobs, seeds=seeds, positions=cache.len, out=xs[0], state=st)
+
+    def round_() -> None:
+        for i in range(k + 1):
+            lg = draft.decode_step(xs[i], dcache)
+            if i < k:
+                qbuf[i].copy_(lg)
+                ops.sample_tokens(qbuf[i], **knobs, seeds=seeds, positions=dcache.len, out=xs[i + 1])
+        toks = xs.t().contiguous()
+        p = model.verify_step(toks, cache)
+        ops.spec_accept(p, qbuf, **knobs, seeds=seeds, tokens=toks, lo_q=cache.lo_q, target=cache, draft=dcache, state=st,
+                        pending=xs[0], drafted=drafted, accepted=accepted)  # fmt: skip
+
+    advance = round_
+    if graphs if graphs is not None else dev.type == "cuda":
+        advance = _capture(round_, [cache.len, cache.lo, cache.last_tok, dcache.len, dcache.lo, dcache.last_tok, xs, qbuf, drafted,
+                                    accepted, st.history, st.n_out, st.active])  # fmt: skip
+    for i in range(max_new - 1):  # every round emits at least one token per active row
+        if i % CHECK_EVERY == 0 and not bool(st.active.any()):
+            break
+        advance()
+    hist, n = st.history.cpu(), st.n_out.cpu()
+    d = drafted.cpu()
+    return SpecResult([p + hist[b, : int(n[b])].tolist() for b, p in enumerate(ids)], int(d.max()) // k, int(d.sum()),
+                      int(accepted.sum()))  # fmt: skip
+
+
+def _capture(fn, state: list[torch.Tensor]):
+    """``fn`` captured in a CUDA graph; returns its replay. A warm-up run outside the capture (library load, kernel attributes)
+    changes ``state``, so ``state`` is restored afterwards; the cache rows it wrote are written again by the first replay."""
+    saved = [t.clone() for t in state]
+    side = torch.cuda.Stream(device=state[0].device)
+    side.wait_stream(torch.cuda.current_stream())
+    with torch.cuda.stream(side):
+        fn()
+    torch.cuda.current_stream().wait_stream(side)
+    graph = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(graph):
+        fn()
+    for t, s in zip(state, saved):
+        t.copy_(s)
+    return graph.replay

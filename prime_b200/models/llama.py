@@ -112,9 +112,15 @@ class Attention(nn.Module):
         """``doc``: (doc_start, doc_end) of ``ops.document_bounds`` for document-masked and / or sliding-window attention, None =
         plain causal. ``kv``: this layer's handle of an ``inference.KVCache``, None outside generation. When prefilling, the rotated
         K|V columns of every position are also copied into the cache; when decoding, ``x`` is [B, 1, dim], the new token is appended
-        to the cache and attends over it."""
+        to the cache and attends over it; when verifying, ``x`` is [B, T, dim], the T tokens are appended and each attends over the
+        cache up to itself, within its document (``cache.lo_q``) and window."""
         B, S, _ = x.shape
         H, Hkv, D = self.n_heads, self.n_kv_heads, self.head_dim
+        if kv is not None and kv.verifying:
+            qkv = ops.linear(x, self.wqkv)  # M = B·T
+            ops.kv_append_tokens(qkv, kv.kv, kv.cache.len, cos, sin, H, Hkv)
+            out = ops.verify_attention(qkv, kv.kv, kv.cache.len, kv.cache.lo_q, kv.cache.window, H, Hkv)
+            return ops.linear(out, self.wo)
         if kv is not None and kv.decoding:
             qkv = ops.linear(x, self.wqkv).view(B, -1)  # M = B: the new token of every row
             ops.kv_append(qkv, kv.kv, kv.cache.len, cos, sin, H, Hkv)
@@ -271,6 +277,19 @@ class Transformer(nn.Module):
             h, delta = layer(h, delta, cache.cos, cache.sin, self.attn_impl, None, cache.layer(i, decoding=True))
         x, _ = ops.add_rmsnorm(delta, h, self.norm.weight, self.args.norm_eps)
         return ops.linear(x.view(B, -1), self.output)
+
+    def verify_step(self, tokens: torch.Tensor, cache) -> torch.Tensor:
+        """The verify step of speculative decoding over a filled ``inference.KVCache``: ``tokens`` int64 [B, T], the next T tokens of
+        every row → logits [B, T, V], those of query t predicting the token after tokens[:, t]. It computes what T decode steps would,
+        in one forward at M = B·T: the cache state afterwards is theirs, and each query's document start is left in ``cache.lo_q``."""
+        B, T = tokens.shape
+        cache.lo_q = ops.verify_advance(tokens, cache.len, cache.lo, cache.last_tok, self.doc_eos_id)
+        h = ops.embedding(tokens, self.tok_embeddings.weight)
+        delta = None
+        for i, layer in enumerate(self.layers):
+            h, delta = layer(h, delta, cache.cos, cache.sin, self.attn_impl, None, cache.layer(i, verifying=True))
+        x, _ = ops.add_rmsnorm(delta, h, self.norm.weight, self.args.norm_eps)
+        return ops.linear(x.view(B * T, -1), self.output).view(B, T, -1)  # the LM head at M = B·T
 
     def loss(self, tokens: torch.Tensor, targets: torch.Tensor, *, grad_scale: float = 1.0, loss_acc: torch.Tensor | None = None) -> torch.Tensor:
         """Mean next-token loss; gradient (not value) is scaled by ``grad_scale``; call ``.backward()`` on it. ``loss_acc``: fp32

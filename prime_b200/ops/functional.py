@@ -992,3 +992,113 @@ def sample_tokens(logits: torch.Tensor, *, temperature: float = 0.0, top_k: int 
         reference.sample_bookkeeping(tok, out, state.history, state.n_out, state.active, state.prompt_len, state.max_seq_len,
                                      state.eos_id)  # fmt: skip
     return out
+
+
+# --------------------------------------------------------------------------- speculative decoding
+
+
+def verify_advance(tokens: torch.Tensor, length: torch.Tensor, lo: torch.Tensor, last_tok: torch.Tensor, eos_id: int | None) -> torch.Tensor:
+    """:func:`decode_advance` for T tokens per row (``tokens`` int64 [B, T]), in place: the rule applied to the tokens in order, so
+    the state afterwards is that of T decode steps. Returns each query's document start ``lo_q`` int32 [B, T]: an EOS among the
+    tokens starts a new document for the queries after it."""
+    B, T = tokens.shape
+    lo_q = torch.empty((B, T), dtype=torch.int32, device=tokens.device)
+    if tokens.is_cuda:
+        assert tokens.dtype == last_tok.dtype == torch.int64 and length.dtype == lo.dtype == torch.int32
+        assert tokens.is_contiguous() and length.is_contiguous() and lo.is_contiguous() and last_tok.is_contiguous()
+        _launch("pb_verify_advance", tokens.data_ptr(), T, -1 if eos_id is None else int(eos_id), length.data_ptr(), lo.data_ptr(),
+                lo_q.data_ptr(), last_tok.data_ptr(), B, _stream())  # fmt: skip
+        return lo_q
+    for t in range(T):
+        if eos_id is not None:
+            lo.copy_(torch.where(last_tok == eos_id, length + t, lo))
+        lo_q[:, t] = lo
+        last_tok.copy_(tokens[:, t])
+    length.add_(T)
+    return lo_q
+
+
+def kv_append_tokens(qkv: torch.Tensor, kv: torch.Tensor, length: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor, n_heads: int,
+                     n_kv_heads: int) -> torch.Tensor:  # fmt: skip
+    """:func:`kv_append` for T tokens per row: ``qkv`` [B, T, (H+2Hkv)·D], token t of row b at position len[b] - T + t. Positions
+    outside the cache are left alone. Returns ``qkv``."""
+    B, T = qkv.shape[:2]
+    H, Hkv = n_heads, n_kv_heads
+    D = qkv.shape[-1] // (H + 2 * Hkv)
+    cap = kv.shape[1]
+    if _decode_native(qkv, kv, H, Hkv):
+        assert length.dtype == torch.int32 and cos.dtype == torch.float32 and cos.is_contiguous() and sin.is_contiguous()
+        assert cos.shape[0] >= cap and cos.shape[1] == D // 2
+        _launch("pb_kv_append_tokens", qkv.data_ptr(), kv.data_ptr(), length.data_ptr(), cos.data_ptr(), sin.data_ptr(), B, T, H, Hkv,
+                D, cap, _stream())  # fmt: skip
+        return qkv
+    for t in range(T):  # token t is the one a decode step would append with len = len - T + t + 1
+        kv_append(qkv[:, t], kv, length - (T - 1 - t), cos, sin, H, Hkv)
+    return qkv
+
+
+def verify_attention(qkv: torch.Tensor, kv: torch.Tensor, length: torch.Tensor, lo_q: torch.Tensor | None, window: int | None,
+                     n_heads: int, n_kv_heads: int, splits: int | None = None) -> torch.Tensor:  # fmt: skip
+    """Attention of T (rotated) queries per row, ``qkv`` [B, T, (H+2Hkv)·D], over the layer's cache → [B, T, H·D]. Query t of row b
+    sits at position pos = len[b] - T + t and sees keys max(lo_q[b, t], pos + 1 - window) <= k <= pos. On CUDA the split-KV verify
+    kernel with the split policy of :func:`decode_attn_splits` (at T = 1 bitwise equal to :func:`decode_attention`), else the fp32
+    :func:`reference.verify_attention`."""
+    B, T = qkv.shape[:2]
+    H, Hkv = n_heads, n_kv_heads
+    D = qkv.shape[-1] // (H + 2 * Hkv)
+    cap = kv.shape[1]
+    if _decode_native(qkv, kv, H, Hkv):
+        assert length.dtype == torch.int32 and (lo_q is None or (lo_q.dtype == torch.int32 and lo_q.is_contiguous()))
+        if splits is None:
+            splits = decode_attn_splits(B, Hkv, cap)
+        out = torch.empty((B, T, H * D), dtype=qkv.dtype, device=qkv.device)
+        part = torch.empty((B, T, H, splits, D + 2), dtype=torch.float32, device=qkv.device) if splits > 1 else None
+        _launch("pb_verify_attn", qkv.data_ptr(), kv.data_ptr(), length.data_ptr(), _ptr(lo_q), int(window or 0), out.data_ptr(),
+                _ptr(part), B, T, H, Hkv, D, cap, splits, 1.0 / math.sqrt(D), _stream(), n=1 if splits == 1 else 2)  # fmt: skip
+        return out
+    q = qkv.view(B, T, H + 2 * Hkv, D)[:, :, :H]
+    return reference.verify_attention(q, kv, length, lo_q, window).reshape(B, T, H * D).to(qkv.dtype)
+
+
+def spec_accept(target_logits: torch.Tensor, draft_logits: torch.Tensor, *, temperature: float = 0.0, top_k: int = 0, top_p: float = 1.0,
+                min_p: float = 0.0, seeds: torch.Tensor, tokens: torch.Tensor, lo_q: torch.Tensor, target, draft, state,
+                pending: torch.Tensor, drafted: torch.Tensor, accepted: torch.Tensor) -> None:  # fmt: skip
+    """The accept step of one speculative round per row, in place (``inference.generate_speculative`` states the round in full).
+
+    ``target_logits`` [B, k+1, V]: the verify step's logits p_1 .. p_{k+1}; ``draft_logits`` [k, B, V]: q_1 .. q_k; ``tokens`` int64
+    [B, k+1]: the pending token x at index L, then the drafts d_1 .. d_k; ``lo_q``: :func:`verify_advance`'s; ``target`` / ``draft``:
+    the two ``inference.KVCache`` (the target's len = L + k + 1); ``state``: an ``inference.SampleState``.
+
+    * P_i / Q_i: the keep-set, temperature and fixed-point masses of :func:`sample_tokens` applied to p_i / q_i, normalised to 2^-40
+      fixed point by one correctly rounded fp64 division per token, ``round(mass_j·2^40 / fp64(mass(kept)))``.
+    * For i = 1 .. k: r = the top 24 bits of Philox word x0 at counter (L + i, 1, 0, 0); d_i is accepted iff
+      ``(2r + 1)·Q_i[d_i] < 2^25·P_i[d_i]`` in exact integers. At the first rejection y is drawn from ``max(0, P_i − Q_i)`` (from P_i
+      should that be all zero) by the inverse CDF of :func:`sample_tokens` in index order, with counter (L + i, 2, 0, 0); after k
+      acceptances y is drawn from P_{k+1} with counter (L + k + 1, 2, 0, 0). Greedy (``temperature == 0``): d_i is accepted iff it
+      is the argmax of p_i (lowest index among ties), and y is the argmax of the first p_i that rejects, or of p_{k+1}.
+    * An active row emits d_1 .. d_n, y into the history through the stop rules of ``sample_tokens(state=...)``, adds k to
+      ``drafted`` and n to ``accepted``, sets both caches to len = L + n + 1, lo = lo_q[b, n], last_tok = tokens[b, n], and writes y
+      to ``pending``. An inactive row writes nothing.
+
+    CUDA bf16 logits run the native kernel (csrc/sample_sm90.cu); everything else :func:`reference.spec_accept`, which reads values
+    back to the host and so cannot be captured."""
+    _sample_args(temperature, top_k, top_p, min_p)
+    B, T, V = target_logits.shape
+    k = T - 1
+    if not 1 <= k <= 15:
+        raise ValueError(f"k must be in [1, 15], got {k}")
+    if tuple(draft_logits.shape) != (k, B, V) or tuple(tokens.shape) != (B, T):
+        raise ValueError(f"draft logits {tuple(draft_logits.shape)} / tokens {tuple(tokens.shape)} do not match target [B={B}, k+1={T}, V]")
+    eos = -1 if state.eos_id is None else int(state.eos_id)
+    if target_logits.is_cuda and target_logits.dtype == draft_logits.dtype == torch.bfloat16:
+        tl, dl = target_logits.reshape(B * T, V), draft_logits.reshape(k * B, V)
+        assert tl.stride(1) == 1 and dl.stride(1) == 1 and state.active.dtype == torch.bool
+        _launch("pb_spec_accept", tl.data_ptr(), tl.stride(0), dl.data_ptr(), dl.stride(0), B, k, V, float(temperature), int(top_k),
+                float(top_p), float(min_p), seeds.data_ptr(), tokens.data_ptr(), lo_q.data_ptr(), target.len.data_ptr(),
+                target.lo.data_ptr(), target.last_tok.data_ptr(), draft.len.data_ptr(), draft.lo.data_ptr(), draft.last_tok.data_ptr(),
+                pending.data_ptr(), state.history.data_ptr(), state.n_out.data_ptr(), state.active.data_ptr(),
+                state.prompt_len.data_ptr(), state.history.shape[1], state.max_seq_len, eos, drafted.data_ptr(), accepted.data_ptr(),
+                _stream())  # fmt: skip
+        return
+    reference.spec_accept(target_logits, draft_logits, temperature, top_k, top_p, min_p, seeds, tokens, lo_q, target, draft, state,
+                          pending, drafted, accepted)  # fmt: skip

@@ -135,6 +135,18 @@ def decode_attention(q: torch.Tensor, kv: torch.Tensor, length: torch.Tensor, lo
     return torch.einsum("bhk,bkhd->bhd", p, vf.masked_fill(~visible.view(B, cap, 1, 1), 0.0))
 
 
+def verify_attention(q: torch.Tensor, kv: torch.Tensor, length: torch.Tensor, lo_q: torch.Tensor | None = None,
+                     window: int | None = None) -> torch.Tensor:  # fmt: skip
+    """T queries per row over a KV cache, in fp32: q [B, T, H, D] (rotated) → [B, T, H, D]. Query t of row b sits at position
+    pos = len[b] - T + t and sees keys max(lo_q[b, t], pos + 1 - window) <= k <= pos: :func:`decode_attention` of each query."""
+    B, T, H, D = q.shape
+    out = []
+    for t in range(T):
+        lo = None if lo_q is None else lo_q[:, t]
+        out.append(decode_attention(q[:, t], kv, length - (T - 1 - t), lo, window))
+    return torch.stack(out, dim=1)
+
+
 # ----------------------------------------------------------------------------------------------------------- sampling
 # The contract is stated in ``ops.sample_tokens``. Nothing below reads a value back to the host, so on CUDA the fallback can be
 # captured in a CUDA graph like the native kernel.
@@ -245,6 +257,88 @@ def sample_bookkeeping(tokens: torch.Tensor, out: torch.Tensor, history: torch.T
     if eos_id is not None:
         stop |= tokens == eos_id
     active.copy_(act & ~stop)
+
+
+def spec_masses(logits: torch.Tensor, temperature: float, top_k: int = 0, top_p: float = 1.0, min_p: float = 0.0) -> torch.Tensor:
+    """The filtered distributions of ``ops.spec_accept``, int64 [N, V]: the kept fixed-point masses of ``ops.sample_tokens`` divided
+    by their total, round(mass_j·2^40 / fp64(total)), in fp64 (every mass < 2^41 is exact in fp64, and so is its product with 2^40).
+    Greedy (temperature 0): 2^40 at the argmax."""
+    lf = logits.float()
+    if temperature == 0:
+        return F.one_hot(lf.argmax(-1), lf.shape[-1]).long() << 40
+    mass = sample_masses(lf, temperature)
+    kept = torch.where(sample_keep(lf, temperature, top_k, top_p, min_p, mass), mass, 0)
+    total = kept.sum(-1, keepdim=True)
+    return (kept.double() * MASS_UNIT / total.double()).round().long()
+
+
+def _philox_r(seed: int, pos: int, word1: int) -> int:
+    """The top 24 bits of Philox4x32-10 word x0 with key = seed and counter = (pos, word1, 0, 0)."""
+    key = torch.tensor([seed & _M32, (seed >> 32) & _M32], dtype=torch.int64)
+    return int(philox4x32_10(key, torch.tensor([pos & _M32, word1, 0, 0], dtype=torch.int64))[0]) >> 8
+
+
+def spec_accept_row(P: torch.Tensor, Q: torch.Tensor, drafts: list[int], seed: int, L: int, greedy: bool) -> tuple[int, int]:
+    """The accept rule of ``ops.spec_accept`` for one row: P [k+1, V] and Q [k, V] from :func:`spec_masses`, the k drafts, the seed
+    and the cache length L before the round → (n accepted, y). Exact: the comparisons and the draw are in Python integers."""
+    k = len(drafts)
+    for i in range(1, k + 2):
+        p = P[i - 1]
+        if i <= k:
+            d = drafts[i - 1]
+            if greedy:
+                if int(p.argmax()) == d:
+                    continue
+                return i - 1, int(p.argmax())
+            r = _philox_r(seed, L + i, 1)
+            if (2 * r + 1) * int(Q[i - 1, d]) < (1 << 25) * int(p[d]):
+                continue
+            w = (p - Q[i - 1]).clamp(min=0)
+            if int(w.sum()) == 0:
+                w = p
+        elif greedy:
+            return k, int(p.argmax())
+        else:
+            w = p
+        total = int(w.sum())
+        target = ((2 * _philox_r(seed, L + i, 2) + 1) * total) >> 25
+        y = int((w.cumsum(0) <= target).sum())
+        return i - 1, y
+    raise AssertionError("unreachable")
+
+
+def spec_accept(target_logits: torch.Tensor, draft_logits: torch.Tensor, temperature: float, top_k: int, top_p: float, min_p: float,
+                seeds: torch.Tensor, tokens: torch.Tensor, lo_q: torch.Tensor, target, draft, state, pending: torch.Tensor,
+                drafted: torch.Tensor, accepted: torch.Tensor) -> None:  # fmt: skip
+    """``ops.spec_accept`` row by row on the host (the bit-exact oracle of the kernel); writes its outputs in place."""
+    B, T, V = target_logits.shape
+    k = T - 1
+    max_new = state.history.shape[1]
+    knobs = (temperature, top_k, top_p, min_p)
+    act = state.active.cpu()
+    for b in range(B):
+        if not bool(act[b]):
+            continue
+        L = int(target.len[b]) - T
+        P = spec_masses(target_logits[b], *knobs)
+        Q = spec_masses(draft_logits[:, b], *knobs)
+        toks = [int(x) for x in tokens[b].tolist()]
+        n, y = spec_accept_row(P, Q, toks[1:], int(seeds[b]), L, temperature == 0)
+        no = int(state.n_out[b])
+        for tok in toks[1 : n + 1] + [y]:
+            state.history[b, no] = tok
+            no += 1
+            if no >= max_new or int(state.prompt_len[b]) + no >= state.max_seq_len or tok == state.eos_id:
+                state.active[b] = False
+                break
+        state.n_out[b] = no
+        drafted[b] += k
+        accepted[b] += n
+        for c in (target, draft):
+            c.len[b] = L + n + 1
+            c.lo[b] = lo_q[b, n]
+            c.last_tok[b] = toks[n]
+        pending[b] = y
 
 
 def cross_entropy(logits: torch.Tensor, targets: torch.Tensor, ignore_index: int = -100) -> torch.Tensor:

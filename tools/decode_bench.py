@@ -19,6 +19,15 @@ top_p = 0.9, timed like the kernel section (bytes = the logits read once); then 
 device-loop step's kernel time (torch.profiler).
 
     python tools/decode_bench.py --only-sampler
+
+Speculative section (``--speculative``, alone): a random-init Llama-2 1B target with a random-init 150M draft, prompt 512,
+B ∈ {1, 8}, k ∈ {2, 4, 8}. CUDA events around graph replays, median of 20: one target decode step, one verify step at T = k + 1,
+one draft decode step, and the accept kernel alone. The break-even acceptance rate α is where the expected tokens per round,
+(1 − α^{k+1}) / (1 − α), equals the round's time over one decode step's. Then greedy generation of 256 new tokens: tokens/s and
+acceptance of ``generate_speculative`` with the target as its own draft (the overhead ceiling) and with the independent draft (the
+floor, random weights agree rarely), next to ``generate_batch(sampler="device")``.
+
+    python tools/decode_bench.py --speculative
 """
 
 from __future__ import annotations
@@ -233,11 +242,98 @@ def sampler_share(model, prompts, capacity: int, knobs: dict) -> float:
     return round(samp / tot, 4) if tot else float("nan")
 
 
+def _replay_ms(replay, state: list[torch.Tensor], reps: int = 20) -> float:
+    """Median ms of one graph replay (CUDA events), the state restored after every replay so every call sees the same lengths."""
+    saved = [t.clone() for t in state]
+    ts = []
+    for _ in range(reps + 1):
+        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        a.record()
+        replay()
+        b.record()
+        b.synchronize()
+        ts.append(a.elapsed_time(b))
+        for t, v in zip(state, saved):
+            t.copy_(v)
+    return statistics.median(ts[1:])
+
+
+def _break_even(ratio: float, k: int) -> float | None:
+    """α with (1 − α^{k+1}) / (1 − α) = ratio (bisection); None if even α = 1 (k + 1 tokens per round) does not pay."""
+    if ratio > k + 1:
+        return None
+    lo, hi = 0.0, 1.0
+    for _ in range(60):
+        mid = (lo + hi) / 2
+        if sum(mid**j for j in range(k + 1)) < ratio:
+            lo = mid
+        else:
+            hi = mid
+    return round(hi, 3)
+
+
+def speculative_section(prompt_len: int = 512, new: int = 256) -> list[dict]:
+    dev = torch.device("cuda")
+    target = build_model("1B", device=dev, seed=0)
+    draft = build_model("150M", device=dev, seed=1)
+    V = target.args.vocab_size
+    rows = []
+    for B in (1, 8):
+        g = torch.Generator().manual_seed(B)
+        prompts = torch.randint(1, V, (B, prompt_len), generator=g).tolist()
+        cap = prompt_len + 1024
+        _, tc = inference.prefill(target, prompts, cap)
+        _, dc = inference.prefill(draft, prompts, cap)
+        t_state, d_state = [tc.len, tc.lo, tc.last_tok], [dc.len, dc.lo, dc.last_tok]
+        tok = torch.ones(B, dtype=torch.int64, device=dev)
+        decode_ms = _replay_ms(inference.GraphDecoder(target, tc, tokens=tok).replay, t_state)
+        draft_ms = _replay_ms(inference.GraphDecoder(draft, dc, tokens=tok).replay, d_state)
+        for k in (2, 4, 8):
+            T = k + 1
+            toks = torch.ones(B, T, dtype=torch.int64, device=dev)
+            verify_ms = _replay_ms(inference._capture(lambda: target.verify_step(toks, tc), t_state), t_state)
+            tl = (torch.randn(B, T, V, device=dev) * 2).to(torch.bfloat16)
+            dl = (torch.randn(k, B, V, device=dev) * 2).to(torch.bfloat16)
+            st = inference.SampleState.allocate(prompts, new, 4096, None, dev)
+            z = [torch.zeros(B, dtype=torch.int64, device=dev) for _ in range(3)]
+            lo_q = torch.zeros(B, T, dtype=torch.int32, device=dev)
+            tc.len.add_(T)
+            acc_state = t_state + d_state + [st.history, st.n_out, st.active, *z]
+            accept_ms = _replay_ms(lambda: ops.spec_accept(tl, dl, temperature=0.8, top_p=0.9, seeds=z[0], tokens=toks, lo_q=lo_q,
+                                                           target=tc, draft=dc, state=st, pending=z[0], drafted=z[1],
+                                                           accepted=z[2]), acc_state)  # fmt: skip
+            tc.len.sub_(T)
+            round_ms = T * draft_ms + verify_ms + accept_ms
+            r = {"B": B, "k": k, "decode_ms": round(decode_ms, 3), "verify_ms": round(verify_ms, 3),
+                 "verify_over_decode": round(verify_ms / decode_ms, 2), "draft_step_ms": round(draft_ms, 3),
+                 "accept_ms": round(accept_ms, 3), "round_ms": round(round_ms, 3),
+                 "break_even_acceptance": _break_even(round_ms / decode_ms, k)}  # fmt: skip
+            for name, dr in (("self", target), ("independent", draft)):
+                inference.generate_speculative(target, dr, prompts, k=k, max_new=8)  # warm-up
+                torch.cuda.synchronize()
+                t0 = time.perf_counter()
+                res = inference.generate_speculative(target, dr, prompts, k=k, max_new=new)
+                torch.cuda.synchronize()
+                dt = time.perf_counter() - t0
+                r[f"{name}_tok_s"] = round(sum(len(x) - prompt_len for x in res.ids) / dt, 1)
+                r[f"{name}_acceptance"] = round(res.accepted / max(res.drafted, 1), 3)
+            inference.generate_batch(target, prompts, max_new=8, sampler="device")
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            out = inference.generate_batch(target, prompts, max_new=new, sampler="device")
+            torch.cuda.synchronize()
+            r["baseline_tok_s"] = round(sum(len(x) - prompt_len for x in out) / (time.perf_counter() - t0), 1)
+            print(json.dumps(r), flush=True)
+            rows.append(r)
+    return rows
+
+
 def main() -> None:
     ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
     ap.add_argument("--out", default=None, help="also write the results as JSON here")
     ap.add_argument("--skip-e2e", action="store_true")
     ap.add_argument("--only-sampler", action="store_true", help="run only the two sampler sections")
+    ap.add_argument("--speculative", action="store_true", help="run only the speculative-decoding section")
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("decode_bench needs a CUDA device")
@@ -245,6 +341,12 @@ def main() -> None:
     print(json.dumps({"card": info}), flush=True)
     flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")
     res = {"card": info}
+    if a.speculative:
+        res["speculative"] = speculative_section()
+        if a.out:
+            Path(a.out).parent.mkdir(parents=True, exist_ok=True)
+            Path(a.out).write_text(json.dumps(res, indent=1))
+        return
     if not a.only_sampler:
         res["kernel"] = kernel_section(flush)
     res["sampler_kernel"] = sampler_kernel_section(flush)
