@@ -10,9 +10,18 @@
 //
 // A verify step (speculative decoding) runs T tokens per row at once: query t of row b sits at position len[b] - T + t and sees key
 // k iff max(lo[b, t], pos + 1 - window) <= k <= pos, with lo [B, T] the document start of each query.
+//
+// An e4m3 cache (the *_fp8 launchers) has the same layout in bytes, kv uint8 [B, capacity, 2·Hkv·D], plus kv_scale uint8
+// [B, capacity, 2·Hkv·D/32]: byte j of a row is the UE8M0 exponent e of its columns 32j .. 32j+31 (scale 2^(e-127)). The values are
+// the MX quantisation (mx_common.cuh) of exactly what the bf16 cache would hold: K after its one bf16 rounding, V as is. Every
+// dequantised value is exact in fp32, so attention over the e4m3 cache is attention over a known bf16 cache.
 #include <math.h>
 
+#include <algorithm>
+#include <type_traits>
+
 #include "common.cuh"
+#include "mx_common.cuh"
 
 namespace {
 
@@ -48,6 +57,21 @@ __global__ void verify_advance_kernel(const int64_t* __restrict__ tokens, int T,
 }
 
 // ------------------------------------------------------------------------------------------------------------------ KV append
+// Columns 8·vh .. 8·vh+7 of a Q or K head rotated at position pos: interleaved pairs, fp32, one bf16 rounding.
+__device__ __forceinline__ bf16x8 rope8(const bf16x8& x, const float4* __restrict__ cosb, const float4* __restrict__ sinb, int pos, int vec,
+                                       int vh) {
+  float v[8], o[8];
+  pb::unpack8(x, v);
+  const float4 c = cosb[(int64_t)pos * vec + vh], s = sinb[(int64_t)pos * vec + vh];
+  const float cc[4] = {c.x, c.y, c.z, c.w}, sn[4] = {s.x, s.y, s.z, s.w};
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    o[2 * j] = v[2 * j] * cc[j] - v[2 * j + 1] * sn[j];
+    o[2 * j + 1] = v[2 * j] * sn[j] + v[2 * j + 1] * cc[j];
+  }
+  return pb::pack8(o);
+}
+
 // One token's fused row at position pos: Q heads are rotated in place, K heads are rotated into the cache row dst, V heads are
 // copied; the rotation is rope_inplace_kernel's (interleaved pairs, fp32, one bf16 rounding).
 __device__ __forceinline__ void append_row(bf16x8* __restrict__ row, bf16x8* __restrict__ dst, const float4* __restrict__ cosb,
@@ -56,18 +80,7 @@ __device__ __forceinline__ void append_row(bf16x8* __restrict__ row, bf16x8* __r
   for (int i = threadIdx.x; i < n; i += blockDim.x) {
     const int head = i / vec, vh = i - head * vec;
     bf16x8 x = row[i];
-    if (head < H + Hkv) {
-      float v[8], o[8];
-      pb::unpack8(x, v);
-      const float4 c = cosb[(int64_t)pos * vec + vh], s = sinb[(int64_t)pos * vec + vh];
-      const float cc[4] = {c.x, c.y, c.z, c.w}, sn[4] = {s.x, s.y, s.z, s.w};
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        o[2 * j] = v[2 * j] * cc[j] - v[2 * j + 1] * sn[j];
-        o[2 * j + 1] = v[2 * j] * sn[j] + v[2 * j + 1] * cc[j];
-      }
-      x = pb::pack8(o);
-    }
+    if (head < H + Hkv) x = rope8(x, cosb, sinb, pos, vec, vh);
     if (head < H)
       row[i] = x;
     else
@@ -97,6 +110,74 @@ __global__ void __launch_bounds__(128) kv_append_tokens_kernel(bf16x8* __restric
   append_row(qkv + ((int64_t)b * T + t) * n, kv + ((int64_t)b * capacity + pos) * (2 * Hkv * vec), cosb, sinb, pos, H, Hkv, vec);
 }
 
+// ------------------------------------------------------------------------------------------------------------- e4m3 cache writes
+// A thread holds 8 columns, so the 4 lanes of an aligned quad hold one 32-column block (D % 32 == 0: a block never straddles two
+// heads). The quad's amax takes two shuffles; the lane holding the block's first columns writes its exponent.
+__device__ __forceinline__ float quad_amax(const float (&f)[8]) {
+  float a = 0.f;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) a = fmaxf(a, fabsf(f[j]));
+  a = fmaxf(a, __shfl_xor_sync(0xffffffffu, a, 1));
+  return fmaxf(a, __shfl_xor_sync(0xffffffffu, a, 2));
+}
+
+// Columns 8c .. 8c+7 of a cache row (f, already at their bf16 values) into e4m3 bytes dst[c] and, for c % 4 == 0, exponent sdst[c/4].
+__device__ __forceinline__ void store_e4m3x8(const float (&f)[8], float amax, uint2* __restrict__ dst, uint8_t* __restrict__ sdst, int c) {
+  float inv;
+  const uint32_t e = pb::ue8m0_for(amax, inv);
+  dst[c] = make_uint2(pb::pack_e4m3x4(f[0] * inv, f[1] * inv, f[2] * inv, f[3] * inv),
+                      pb::pack_e4m3x4(f[4] * inv, f[5] * inv, f[6] * inv, f[7] * inv));
+  if ((c & 3) == 0) sdst[c >> 2] = (uint8_t)e;
+}
+
+// kv_append_tokens_kernel into an e4m3 cache: one CTA per (token, row), token t of row b at position len[b] - T + t. Q heads are
+// rotated in place as there; K heads are rotated and rounded to bf16, then quantised with V into the cache row.
+__global__ void __launch_bounds__(128) kv_append_fp8_kernel(bf16x8* __restrict__ qkv, uint2* __restrict__ kv, uint8_t* __restrict__ kv_scale,
+                                                            const int* __restrict__ len, const float4* __restrict__ cosb,
+                                                            const float4* __restrict__ sinb, int T, int H, int Hkv, int vec, int capacity) {
+  const int t = blockIdx.x, b = blockIdx.y;
+  const int pos = len[b] - T + t;
+  if (pos < 0 || pos >= capacity) return;
+  const int n = (H + 2 * Hkv) * vec;
+  bf16x8* row = qkv + ((int64_t)b * T + t) * n;
+  const int64_t r = (int64_t)b * capacity + pos;
+  uint2* dst = kv + r * (2 * Hkv * vec);
+  uint8_t* sdst = kv_scale + r * (2 * Hkv * vec / 4);
+  for (int i0 = 0; i0 < n; i0 += blockDim.x) {  // a bound uniform over the warp: the quad shuffles need every lane
+    const int i = i0 + threadIdx.x;
+    const int head = i / vec;
+    bf16x8 x{};
+    float f[8] = {};
+    if (i < n) {
+      x = row[i];
+      if (head < H + Hkv) x = rope8(x, cosb, sinb, pos, vec, i - head * vec);
+      pb::unpack8(x, f);
+    }
+    const float amax = quad_amax(f);  // n % 4 == 0: a quad is wholly inside or wholly past the row, and inside one head
+    if (i >= n) continue;
+    if (head < H)
+      row[i] = x;
+    else
+      store_e4m3x8(f, amax, dst, sdst, i - H * vec);
+  }
+}
+
+// Prefill: bf16 rows src + (b·S + s)·ld, cols wide, into e4m3 cache rows s = 0 .. S-1 of row b. One thread per 8 columns.
+__global__ void __launch_bounds__(256) kv_quantize_kernel(const __nv_bfloat16* __restrict__ src, int64_t ld, uint2* __restrict__ kv,
+                                                          uint8_t* __restrict__ kv_scale, int S, int vec, int capacity, int64_t total) {
+  for (int64_t i0 = (int64_t)blockIdx.x * blockDim.x; i0 < total; i0 += (int64_t)gridDim.x * blockDim.x) {  // uniform bound
+    const int64_t i = i0 + threadIdx.x;
+    const int64_t r = i / vec;  // b·S + s
+    const int c = (int)(i - r * vec);
+    float f[8] = {};
+    if (i < total) pb::unpack8(pb::ldg_stream(reinterpret_cast<const bf16x8*>(src + r * ld + c * 8)), f);
+    const float amax = quad_amax(f);
+    if (i >= total) continue;
+    const int64_t b = r / S, row = b * capacity + (r - b * S);
+    store_e4m3x8(f, amax, kv + row * vec, kv_scale + row * (vec / 4), c);
+  }
+}
+
 // ------------------------------------------------------------------------------------------------------------- split-KV attention
 struct DecodeParams {
   const __nv_bfloat16* qkv;  // [B, (H + 2Hkv)·D], Q rotated ([B, T, ·] when verifying)
@@ -108,7 +189,27 @@ struct DecodeParams {
   int H, Hkv, G, chunks, capacity, window, splits, keys_per_split;
   float scale_log2;
   int T;  // verify: tokens per row
+  const uint8_t* kv_scale;  // e4m3 cache: [B, capacity, 2·Hkv·D/32] UE8M0 exponents (kv then holds the e4m3 bytes)
 };
+
+// 8 e4m3 values (one 8-byte load) → fp32, exactly: cvt.rn.f16x2.e4m3x2 per pair, the low byte the lower column
+__device__ __forceinline__ void unpack8_e4m3(const uint2& x, float (&f)[8]) {
+  const uint32_t w[2] = {x.x, x.y};
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    uint32_t h2;
+    asm("cvt.rn.f16x2.e4m3x2 %0, %1;" : "=r"(h2) : "h"((unsigned short)(w[i >> 1] >> (16 * (i & 1)))));
+    const float2 t = __half22float2(*reinterpret_cast<const __half2*>(&h2));
+    f[2 * i] = t.x;
+    f[2 * i + 1] = t.y;
+  }
+}
+__device__ __forceinline__ uint2 ldg_stream8(const uint8_t* p) {
+  uint2 r;
+  asm volatile("ld.global.nc.L1::no_allocate.v2.u32 {%0,%1}, [%2];" : "=r"(r.x), "=r"(r.y) : "l"(p));
+  return r;
+}
+__device__ __forceinline__ float ue8m0_scale(uint8_t e) { return __uint_as_float((uint32_t)e << 23); }  // 2^(e-127), e in [1, 254]
 
 constexpr int kDecThreads = 128;
 constexpr int kDecWarps = kDecThreads / 32;
@@ -119,11 +220,16 @@ constexpr int kDecWarps = kDecThreads / 32;
 // and the CTA's key loop covers the union of those ranges. A lane group of D/8 lanes holds one key, each lane 8 of its dimensions; a
 // warp covers 32·8/D keys per load and every lane keeps kUnroll keys' K and V loads in flight. Scores are reduced over the lane group
 // by shuffles; each lane group runs its own online softmax, and the groups are merged (shuffles, then shared memory) at the end.
-template <int D, int GC, bool kMulti>
+//
+// kFp8: the cache holds e4m3 bytes with a UE8M0 exponent per 32 columns. A lane loads its 8 K and 8 V bytes (8-byte streaming
+// loads) and its blocks' two exponents, converts exactly, and applies the power-of-two scales as products that round nothing: K's
+// to its partial dot product before the lane-group reduction, V's to p before the V FMA. Every sum is then the bf16 kernel's sum
+// over the dequantised cache.
+template <int D, int GC, bool kMulti, bool kFp8 = false>
 __device__ __forceinline__ void attn_body(const DecodeParams& p) {
   constexpr int LPK = D / 8;   // lanes per key
   constexpr int KPW = 32 / LPK;  // keys per warp and load
-  constexpr int kUnroll = GC >= 8 ? 2 : 4;
+  constexpr int kUnroll = GC >= 8 ? 2 : 4;  // the fp8 kernels too: 8 keys per lane halved occupancy (DESIGN.md §1.5)
   constexpr int KPI = kDecWarps * KPW * kUnroll;  // keys per CTA iteration
   __shared__ float s_m[kDecWarps][GC], s_l[kDecWarps][GC];
   __shared__ float s_acc[kDecWarps][GC][D];
@@ -194,28 +300,44 @@ __device__ __forceinline__ void attn_body(const DecodeParams& p) {
     }
     const __nv_bfloat16* kbase = p.kv + (int64_t)b * p.capacity * ldkv + hk * D + sub * 8;
     const __nv_bfloat16* vbase = kbase + p.Hkv * D;
+    // e4m3 cache: one byte per column, one exponent per 32 columns (the lane's 8 columns lie in one block)
+    const uint8_t* kbase8 = reinterpret_cast<const uint8_t*>(p.kv) + (int64_t)b * p.capacity * ldkv + hk * D + sub * 8;
+    const uint8_t* sbase = p.kv_scale + (int64_t)b * p.capacity * (ldkv / 32) + (hk * D + sub * 8) / 32;
     // the loop bound is uniform over the warp (the shuffles below need every lane); keys past k1 are loaded by no lane and score -inf
     for (int wb = k0 + warp * KPW * kUnroll; wb < k1; wb += KPI) {
       const int base = wb + grp;
-      bf16x8 kr[kUnroll] = {}, vr[kUnroll] = {};
+      using Raw = std::conditional_t<kFp8, uint2, bf16x8>;
+      Raw kr[kUnroll] = {}, vr[kUnroll] = {};
+      uint8_t ke[kFp8 ? kUnroll : 1] = {}, ve[kFp8 ? kUnroll : 1] = {};
 #pragma unroll
       for (int u = 0; u < kUnroll; ++u) {
         const int key = base + u * KPW;
         if (key < k1) {
-          kr[u] = pb::ldg_stream(reinterpret_cast<const bf16x8*>(kbase + (int64_t)key * ldkv));
-          vr[u] = pb::ldg_stream(reinterpret_cast<const bf16x8*>(vbase + (int64_t)key * ldkv));
+          if constexpr (kFp8) {
+            kr[u] = ldg_stream8(kbase8 + (int64_t)key * ldkv);
+            vr[u] = ldg_stream8(kbase8 + (int64_t)key * ldkv + p.Hkv * D);
+            ke[u] = __ldg(sbase + (int64_t)key * (ldkv / 32));
+            ve[u] = __ldg(sbase + (int64_t)key * (ldkv / 32) + p.Hkv * D / 32);
+          } else {
+            kr[u] = pb::ldg_stream(reinterpret_cast<const bf16x8*>(kbase + (int64_t)key * ldkv));
+            vr[u] = pb::ldg_stream(reinterpret_cast<const bf16x8*>(vbase + (int64_t)key * ldkv));
+          }
         }
       }
       float s[kUnroll][GC];
 #pragma unroll
       for (int u = 0; u < kUnroll; ++u) {
         float kf[8];
-        pb::unpack8(kr[u], kf);
+        if constexpr (kFp8)
+          unpack8_e4m3(kr[u], kf);
+        else
+          pb::unpack8(kr[u], kf);
 #pragma unroll
         for (int g = 0; g < GC; ++g) {
           float d = 0.f;
 #pragma unroll
           for (int j = 0; j < 8; ++j) d = fmaf(q[g][j], kf[j], d);
+          if constexpr (kFp8) d *= ue8m0_scale(ke[u]);
 #pragma unroll
           for (int o = LPK / 2; o > 0; o >>= 1) d += __shfl_xor_sync(0xffffffffu, d, o);
           if constexpr (kMulti) {
@@ -245,12 +367,16 @@ __device__ __forceinline__ void attn_body(const DecodeParams& p) {
       for (int u = 0; u < kUnroll; ++u) {
         if (base + u * KPW >= k1) continue;
         float vf[8];
-        pb::unpack8(vr[u], vf);
+        if constexpr (kFp8)
+          unpack8_e4m3(vr[u], vf);
+        else
+          pb::unpack8(vr[u], vf);
 #pragma unroll
         for (int g = 0; g < GC; ++g) {
           l[g] += s[u][g];
+          const float pv = kFp8 ? s[u][g] * ue8m0_scale(ve[u]) : s[u][g];
 #pragma unroll
-          for (int j = 0; j < 8; ++j) acc[g][j] = fmaf(s[u][g], vf[j], acc[g][j]);
+          for (int j = 0; j < 8; ++j) acc[g][j] = fmaf(pv, vf[j], acc[g][j]);
         }
       }
     }
@@ -353,33 +479,37 @@ __global__ void __launch_bounds__(128) decode_combine_kernel(const float* __rest
   }
 }
 
-template <int D>
-int launch_decode(const DecodeParams& p0, int B, cudaStream_t stream) {
-  DecodeParams p = p0;
-  const int gc = p.G > 4 ? 8 : p.G > 2 ? 4 : p.G;  // smallest power of two >= G, at most 8 (G > 8: several chunks of 8)
-  p.chunks = (p.G + gc - 1) / gc;
-  const dim3 grid(p.splits, p.Hkv * p.chunks, B);
-  if (gc == 8) decode_attn_kernel<D, 8><<<grid, kDecThreads, 0, stream>>>(p);
-  else if (gc == 4) decode_attn_kernel<D, 4><<<grid, kDecThreads, 0, stream>>>(p);
-  else if (gc == 2) decode_attn_kernel<D, 2><<<grid, kDecThreads, 0, stream>>>(p);
-  else decode_attn_kernel<D, 1><<<grid, kDecThreads, 0, stream>>>(p);
-  if (p.splits > 1) decode_combine_kernel<<<B * p.H, 128, 0, stream>>>(p.part, p.out, p.H, D, p.splits);
-  PB_CHECK_LAUNCH();
-  return 0;
+template <int D, int GC>
+__global__ void __launch_bounds__(kDecThreads) decode_attn_fp8_kernel(const DecodeParams p) {
+  attn_body<D, GC, false, true>(p);
 }
 
-// The verify step: T·G query vectors per KV group, in chunks of the smallest power of two >= T·G, at most 8.
-template <int D>
-int launch_verify(const DecodeParams& p0, int B, cudaStream_t stream) {
+template <int D, int GC>
+__global__ void __launch_bounds__(kDecThreads) verify_attn_fp8_kernel(const DecodeParams p) {
+  attn_body<D, GC, true, true>(p);
+}
+
+template <int D, int GC, bool kMulti, bool kFp8>
+void attn_kernel(dim3 grid, const DecodeParams& p, cudaStream_t stream) {
+  if constexpr (kMulti && kFp8) verify_attn_fp8_kernel<D, GC><<<grid, kDecThreads, 0, stream>>>(p);
+  else if constexpr (kMulti) verify_attn_kernel<D, GC><<<grid, kDecThreads, 0, stream>>>(p);
+  else if constexpr (kFp8) decode_attn_fp8_kernel<D, GC><<<grid, kDecThreads, 0, stream>>>(p);
+  else decode_attn_kernel<D, GC><<<grid, kDecThreads, 0, stream>>>(p);
+}
+
+// Decoding, the G query heads of a KV group; verifying (kMulti), its T·G query vectors: in chunks of the smallest power of two
+// >= that count, at most 8 (more: several chunks of 8). Then the combine over the B·T·H output rows when the keys are split.
+template <int D, bool kMulti, bool kFp8>
+int launch_attn(const DecodeParams& p0, int B, cudaStream_t stream) {
   DecodeParams p = p0;
-  const int nq = p.T * p.G;
+  const int nq = kMulti ? p.T * p.G : p.G;
   const int gc = nq > 4 ? 8 : nq > 2 ? 4 : nq;
   p.chunks = (nq + gc - 1) / gc;
   const dim3 grid(p.splits, p.Hkv * p.chunks, B);
-  if (gc == 8) verify_attn_kernel<D, 8><<<grid, kDecThreads, 0, stream>>>(p);
-  else if (gc == 4) verify_attn_kernel<D, 4><<<grid, kDecThreads, 0, stream>>>(p);
-  else if (gc == 2) verify_attn_kernel<D, 2><<<grid, kDecThreads, 0, stream>>>(p);
-  else verify_attn_kernel<D, 1><<<grid, kDecThreads, 0, stream>>>(p);
+  if (gc == 8) attn_kernel<D, 8, kMulti, kFp8>(grid, p, stream);
+  else if (gc == 4) attn_kernel<D, 4, kMulti, kFp8>(grid, p, stream);
+  else if (gc == 2) attn_kernel<D, 2, kMulti, kFp8>(grid, p, stream);
+  else attn_kernel<D, 1, kMulti, kFp8>(grid, p, stream);
   if (p.splits > 1) decode_combine_kernel<<<B * p.T * p.H, 128, 0, stream>>>(p.part, p.out, p.H, D, p.splits);
   PB_CHECK_LAUNCH();
   return 0;
@@ -434,7 +564,7 @@ PB_EXPORT int pb_decode_attn(const void* qkv, const void* kv, const int* len, co
   const int tiles = (capacity + kSplitKeys - 1) / kSplitKeys;
   DecodeParams p{(const __nv_bfloat16*)qkv, (const __nv_bfloat16*)kv, len, lo, (__nv_bfloat16*)out, part, H, Hkv, H / Hkv, 1,
                  capacity, window, splits, (tiles + splits - 1) / splits * kSplitKeys, scale * 1.4426950408889634f, 1};
-  return D == 128 ? launch_decode<128>(p, B, stream) : launch_decode<64>(p, B, stream);
+  return D == 128 ? launch_attn<128, false, false>(p, B, stream) : launch_attn<64, false, false>(p, B, stream);
 }
 
 // The split policy of pb_decode_attn: a function of the cache geometry only, never of the lengths, so a decode step captured in a
@@ -490,5 +620,76 @@ PB_EXPORT int pb_verify_attn(const void* qkv, const void* kv, const int* len, co
   const int tiles = (capacity + kSplitKeys - 1) / kSplitKeys;
   DecodeParams p{(const __nv_bfloat16*)qkv, (const __nv_bfloat16*)kv, len, lo, (__nv_bfloat16*)out, part, H, Hkv, H / Hkv, 1,
                  capacity, window, splits, (tiles + splits - 1) / splits * kSplitKeys, scale * 1.4426950408889634f, T};
-  return D == 128 ? launch_verify<128>(p, B, stream) : launch_verify<64>(p, B, stream);
+  return D == 128 ? launch_attn<128, true, false>(p, B, stream) : launch_attn<64, true, false>(p, B, stream);
+}
+
+// ------------------------------------------------------------------------------------------------------------ e4m3 cache (fp8)
+// The layout is the bf16 cache's in bytes, kv uint8 [B, capacity, 2·Hkv·D], plus kv_scale uint8 [B, capacity, 2·Hkv·D/32] (see the
+// top of this file). Same return codes as above; a null kv_scale is -1, and kv_scale must be 4-byte and kv 8-byte aligned (-6).
+
+// pb_kv_append_tokens into an e4m3 cache (T = 1: the decode step's append): Q heads rotated in place, then the rotated K (rounded
+// to bf16) and V of each token quantised into its cache row.
+PB_EXPORT int pb_kv_append_fp8(void* qkv, void* kv, void* kv_scale, const int* len, const float* cos, const float* sin, int B, int T, int H,
+                               int Hkv, int D, int capacity, cudaStream_t stream) {
+  if (qkv == nullptr || kv == nullptr || kv_scale == nullptr || len == nullptr || cos == nullptr || sin == nullptr) return -1;
+  if (D != 64 && D != 128) return -2;
+  if (B < 1 || T < 1 || H < 1 || Hkv < 1 || capacity < 1 || H % Hkv != 0) return -3;
+  if (!aligned(qkv, 16) || !aligned(kv, 8) || !aligned(kv_scale, 4) || !aligned(cos, 16) || !aligned(sin, 16) || !aligned(len, 4)) return -6;
+  kv_append_fp8_kernel<<<dim3(T, B), 128, 0, stream>>>((bf16x8*)qkv, (uint2*)kv, (uint8_t*)kv_scale, len, (const float4*)cos,
+                                                       (const float4*)sin, T, H, Hkv, D / 8, capacity);
+  PB_CHECK_LAUNCH();
+  return 0;
+}
+
+// Prefill: quantise S bf16 rows per sequence, row (b, s) at src + (b·S + s)·src_row_stride elements and cols wide (the K|V columns
+// of the fused QKV activation: src = qkv + H·D, stride (H + 2Hkv)·D), into rows 0 .. S-1 of the e4m3 cache. -3 for S > capacity
+// or cols not a multiple of 32 or wider than the stride; src and its stride must keep 16-byte rows (-6).
+PB_EXPORT int pb_kv_quantize(const void* src, int64_t src_row_stride, void* kv, void* kv_scale, int B, int S, int cols, int capacity,
+                             cudaStream_t stream) {
+  if (src == nullptr || kv == nullptr || kv_scale == nullptr) return -1;
+  if (B < 1 || S < 1 || capacity < S || cols < 32 || cols % 32 != 0 || src_row_stride < cols) return -3;
+  if (!aligned(src, 16) || src_row_stride % 8 != 0 || !aligned(kv, 8) || !aligned(kv_scale, 4)) return -6;
+  const int64_t total = (int64_t)B * S * (cols / 8);
+  const int grid = (int)std::min<int64_t>((total + 255) / 256, 132 * 16);
+  kv_quantize_kernel<<<grid, 256, 0, stream>>>((const __nv_bfloat16*)src, src_row_stride, (uint2*)kv, (uint8_t*)kv_scale, S, cols / 8,
+                                               capacity, total);
+  PB_CHECK_LAUNCH();
+  return 0;
+}
+
+// pb_decode_attn over an e4m3 cache. At the same split count its result is the bf16 kernel's math on the dequantised cache.
+PB_EXPORT int pb_decode_attn_fp8(const void* qkv, const void* kv, const void* kv_scale, const int* len, const int* lo, int window, void* out,
+                                 float* part, int B, int H, int Hkv, int D, int capacity, int splits, float scale, cudaStream_t stream) {
+  if (qkv == nullptr || kv == nullptr || kv_scale == nullptr || len == nullptr || out == nullptr || (splits > 1 && part == nullptr)) return -1;
+  if (D != 64 && D != 128) return -2;
+  if (B < 1 || H < 1 || Hkv < 1 || capacity < 1 || H % Hkv != 0) return -3;
+  if (window < 0) return -4;
+  if (splits < 1) return -5;
+  if (!aligned(qkv, 16) || !aligned(kv, 8) || !aligned(kv_scale, 4) || !aligned(out, 16) || !aligned(len, 4) || !aligned(lo, 4) ||
+      !aligned(part, 4))
+    return -6;
+  const int tiles = (capacity + kSplitKeys - 1) / kSplitKeys;
+  DecodeParams p{(const __nv_bfloat16*)qkv, (const __nv_bfloat16*)kv, len, lo, (__nv_bfloat16*)out, part, H, Hkv, H / Hkv, 1,
+                 capacity, window, splits, (tiles + splits - 1) / splits * kSplitKeys, scale * 1.4426950408889634f, 1,
+                 (const uint8_t*)kv_scale};
+  return D == 128 ? launch_attn<128, false, true>(p, B, stream) : launch_attn<64, false, true>(p, B, stream);
+}
+
+// pb_verify_attn over an e4m3 cache; with T = 1 it computes exactly what pb_decode_attn_fp8 computes, bit for bit.
+PB_EXPORT int pb_verify_attn_fp8(const void* qkv, const void* kv, const void* kv_scale, const int* len, const int* lo, int window, void* out,
+                                 float* part, int B, int T, int H, int Hkv, int D, int capacity, int splits, float scale,
+                                 cudaStream_t stream) {
+  if (qkv == nullptr || kv == nullptr || kv_scale == nullptr || len == nullptr || out == nullptr || (splits > 1 && part == nullptr)) return -1;
+  if (D != 64 && D != 128) return -2;
+  if (B < 1 || T < 1 || H < 1 || Hkv < 1 || capacity < 1 || H % Hkv != 0) return -3;
+  if (window < 0) return -4;
+  if (splits < 1) return -5;
+  if (!aligned(qkv, 16) || !aligned(kv, 8) || !aligned(kv_scale, 4) || !aligned(out, 16) || !aligned(len, 4) || !aligned(lo, 4) ||
+      !aligned(part, 4))
+    return -6;
+  const int tiles = (capacity + kSplitKeys - 1) / kSplitKeys;
+  DecodeParams p{(const __nv_bfloat16*)qkv, (const __nv_bfloat16*)kv, len, lo, (__nv_bfloat16*)out, part, H, Hkv, H / Hkv, 1,
+                 capacity, window, splits, (tiles + splits - 1) / splits * kSplitKeys, scale * 1.4426950408889634f, T,
+                 (const uint8_t*)kv_scale};
+  return D == 128 ? launch_attn<128, true, true>(p, B, stream) : launch_attn<64, true, true>(p, B, stream);
 }

@@ -11,11 +11,10 @@
 // 128 rows x 4 K-blocks and stores the byte of (row r, block kb) at  (r % 32) * 16 + ((r % 128) / 32) * 4 + kb.
 //
 // Tile 128 x 64 x 128 (K bytes), 4 warps of 32 x 64, operands staged in padded shared memory with cp.async (double-buffered).
-#include <cuda_fp8.h>
-
 #include <algorithm>
 
 #include "common.cuh"
+#include "mx_common.cuh"
 #include "tc_common.cuh"
 
 namespace {
@@ -137,20 +136,8 @@ __global__ void __launch_bounds__(kThreads) gemm_mxfp8_kernel(const uint8_t* __r
 }
 
 // ---------------------------------------------------------------------------------------------------------------- quantisers
-// smallest power of two s with amax / s <= 448 (e4m3 max), as a biased UE8M0 exponent; and 1/s
-__device__ __forceinline__ uint32_t ue8m0_for(float amax, float& inv_scale) {
-  const uint32_t bits = __float_as_uint(amax * (1.0f / 448.0f));
-  uint32_t e = (bits >> 23) & 0xFF;
-  if (bits & 0x7FFFFF) e += 1;
-  e = min(max(e, 1u), 254u);
-  inv_scale = __uint_as_float((254u - e) << 23);
-  return e;
-}
-__device__ __forceinline__ uint32_t pack_e4m3x4(float a, float b, float c, float d) {
-  const uint32_t lo = __nv_cvt_float2_to_fp8x2(make_float2(a, b), __NV_SATFINITE, __NV_E4M3);
-  const uint32_t hi = __nv_cvt_float2_to_fp8x2(make_float2(c, d), __NV_SATFINITE, __NV_E4M3);
-  return lo | (hi << 16);
-}
+using pb::pack_e4m3x4;  // the MX rule (mx_common.cuh), shared with the e4m3 KV cache
+using pb::ue8m0_for;
 
 // x bf16 [R, C] (row stride ld) → q e4m3 [R, C] (dense) + scales for blocks of 32 along C. One thread per 32-element block.
 __global__ void __launch_bounds__(256) quantize_mxfp8_kernel(const __nv_bfloat16* __restrict__ x, int64_t ld, uint8_t* __restrict__ q,

@@ -6,6 +6,7 @@
     python -m prime_b200.eval generate --ckpt … --model 1B --prompt-ids 1,306,626 --max-new 32
     python -m prime_b200.eval generate --ckpt … --model 1B --prompt-ids 1,306,626 --temperature 0.8 --top-p 0.9 --sampler device
     python -m prime_b200.eval generate --ckpt … --model 1B --draft-ckpt … --draft-model 150M --spec-k 4 --prompt-ids 1,306,626
+    python -m prime_b200.eval generate --ckpt … --model 1B --prompt-ids 1,306,626 --kv-dtype fp8   # e4m3 KV cache: half the bytes
 
 The model is rebuilt on one device from the per-rank optimizer shards (``checkpoint.assemble_full_model``) or from a Hugging
 Face directory (``models.hf.load_hf_dir``); the forward runs through the same ops as training (native kernels on an H100, the
@@ -47,11 +48,12 @@ def perplexity(model: Transformer, dataset, *, batches: int, batch_size: int, de
 
 
 def generate(model: Transformer, prompt: list[int], *, max_new: int, temperature: float = 0.0, top_k: int = 0, top_p: float = 1.0,
-             min_p: float = 0.0, seed: int = 0, eos_id: int | None = None, sampler: str = "host") -> list[int]:  # fmt: skip
+             min_p: float = 0.0, seed: int = 0, eos_id: int | None = None, sampler: str = "host", kv_dtype: str = "bf16") -> list[int]:  # fmt: skip
     """Greedy (temperature 0) or temperature / top-k / top-p / min-p sampling; returns prompt + continuation. ``sampler``: "host"
-    (the random stream of earlier versions) or "device" (``ops.sample_tokens``'s Philox stream), see ``generate_batch``."""
+    (the random stream of earlier versions) or "device" (``ops.sample_tokens``'s Philox stream), see ``generate_batch``; ``kv_dtype``:
+    "bf16" or "fp8" (an e4m3 KV cache)."""
     return generate_batch(model, [prompt], max_new=max_new, temperature=temperature, top_k=top_k, top_p=top_p, min_p=min_p, seed=seed,
-                          eos_id=eos_id, sampler=sampler)[0]  # fmt: skip
+                          eos_id=eos_id, sampler=sampler, kv_dtype=kv_dtype)[0]  # fmt: skip
 
 
 @torch.no_grad()
@@ -135,6 +137,8 @@ def main(argv: list[str] | None = None) -> dict:
     g.add_argument("--draft-model", default="150M")
     g.add_argument("--draft-type-model", default="llama2", choices=["llama2", "llama3"])
     g.add_argument("--spec-k", type=int, default=4, help="draft tokens per speculative round")
+    g.add_argument("--kv-dtype", default="bf16", choices=["bf16", "fp8"],
+                   help="KV-cache storage: bf16, or fp8 = e4m3 with a power-of-two scale per 32 values (about half the bytes)")
     a = ap.parse_args(argv)
     spec = a.cmd == "generate" and (a.draft_ckpt or a.draft_hf)
     if spec and a.sampler == "host":
@@ -153,12 +157,12 @@ def main(argv: list[str] | None = None) -> dict:
     elif spec:
         r = generate_speculative(model, load_model(a, a.device, "draft_"), [[int(x) for x in a.prompt_ids.split(",")]], k=a.spec_k,
                                  max_new=a.max_new, temperature=a.temperature, top_k=a.top_k, top_p=a.top_p, min_p=a.min_p,
-                                 seed=a.seed)  # fmt: skip
+                                 seed=a.seed, kv_dtype=a.kv_dtype)  # fmt: skip
         out = {"ids": r.ids[0], "spec": {"rounds": r.rounds, "drafted": r.drafted, "accepted": r.accepted,
                                          "acceptance": r.accepted / max(r.drafted, 1)}}  # fmt: skip
     else:
         ids = generate(model, [int(x) for x in a.prompt_ids.split(",")], max_new=a.max_new, temperature=a.temperature, top_k=a.top_k,
-                       top_p=a.top_p, min_p=a.min_p, seed=a.seed, sampler=a.sampler)  # fmt: skip
+                       top_p=a.top_p, min_p=a.min_p, seed=a.seed, sampler=a.sampler, kv_dtype=a.kv_dtype)  # fmt: skip
         out = {"ids": ids}
     print(json.dumps(out))
     return out

@@ -3,7 +3,9 @@ CUDA graph.
 
 The cache keeps, per layer, exactly the K|V columns of the fused QKV activation with K already rotated, so prefill fills it with one
 strided copy per layer and a decode step appends one row per sequence (``ops.kv_append``) and runs split-KV attention over it
-(``ops.decode_attention``). The per-row state (``len``, ``lo``: the first key the current query may see, ``last_tok``) lives on the
+(``ops.decode_attention``). With ``kv_dtype="fp8"`` the cache holds those values as e4m3 with one power-of-two scale per 32 columns
+(the format of ``ops.kv_append``): 1 + 1/32 bytes per value instead of 2, so twice the context fits and the attention kernel, bound by
+the bytes it reads, reads about half as many. The per-row state (``len``, ``lo``: the first key the current query may see, ``last_tok``) lives on the
 device, so a decode step depends on no host value that changes between tokens.
 
 Sampling runs on the host (one CPU generator, the stream of earlier versions) or, with ``sampler="device"``, inside the step:
@@ -40,14 +42,33 @@ class LayerKV:
     def kv(self) -> torch.Tensor:
         return self.cache.kv[self.index]
 
+    @property
+    def kv_scale(self) -> torch.Tensor | None:
+        return None if self.cache.kv_scale is None else self.cache.kv_scale[self.index]
+
     def store(self, qkv: torch.Tensor, k_col: int) -> None:
-        """Prefill: copy the rotated K|V columns (from ``k_col`` on) of every position of qkv [B, S, ·] into the cache."""
-        self.kv[:, : qkv.shape[1]].copy_(qkv[..., k_col:])
+        """Prefill: copy the rotated K|V columns (from ``k_col`` on) of every position of qkv [B, S, ·] into the cache, quantised
+        (``ops.kv_quantize``) when the cache is e4m3."""
+        if self.cache.kv_scale is not None:
+            ops.kv_quantize(qkv[..., k_col:], self.kv, self.kv_scale)
+        else:
+            self.kv[:, : qkv.shape[1]].copy_(qkv[..., k_col:])
+
+
+KV_DTYPES = ("bf16", "fp8")
+
+
+def check_kv_dtype(model: Transformer, kv_dtype: str) -> None:
+    """``kv_dtype`` is "bf16" (the model's dtype) or "fp8" (e4m3 with a scale per 32 columns, which needs head_dim % 32 == 0)."""
+    if kv_dtype not in KV_DTYPES:
+        raise ValueError(f"kv_dtype must be one of {KV_DTYPES}, got {kv_dtype!r}")
+    if kv_dtype == "fp8" and model.args.head_dim % 32:
+        raise ValueError(f"an fp8 KV cache needs head_dim % 32 == 0 (one scale per 32 columns of a head), got {model.args.head_dim}")
 
 
 @dataclass
 class KVCache:
-    kv: torch.Tensor  # [L, B, capacity, 2·Hkv·D]
+    kv: torch.Tensor  # [L, B, capacity, 2·Hkv·D]: the model's dtype, or uint8 e4m3 bytes with kv_scale
     len: torch.Tensor  # int32 [B]: valid cache rows
     lo: torch.Tensor  # int32 [B]: first key of the current query's document
     last_tok: torch.Tensor  # int64 [B]
@@ -55,6 +76,7 @@ class KVCache:
     sin: torch.Tensor
     window: int | None  # ModelArgs.sliding_window
     lo_q: torch.Tensor | None = None  # int32 [B, T]: each query's document start in the last verify step
+    kv_scale: torch.Tensor | None = None  # uint8 [L, B, capacity, 2·Hkv·D/32]: UE8M0 exponents of an e4m3 cache (ops.kv_append)
 
     @property
     def capacity(self) -> int:
@@ -64,13 +86,17 @@ class KVCache:
         return LayerKV(self, i, decoding, verifying)
 
     @classmethod
-    def allocate(cls, model: Transformer, batch: int, capacity: int, device) -> "KVCache":
+    def allocate(cls, model: Transformer, batch: int, capacity: int, device, kv_dtype: str = "bf16") -> "KVCache":
+        """``kv_dtype``: "bf16" keeps the model's dtype; "fp8" stores e4m3 bytes and one exponent byte per 32 values."""
+        check_kv_dtype(model, kv_dtype)
         a = model.args
-        dtype = model.output.dtype
+        dtype = model.output.dtype if kv_dtype == "bf16" else torch.uint8
         cos, sin = model.rope_tables(capacity, device)
-        kv = torch.empty((a.n_layers, batch, capacity, 2 * a.kv_heads * a.head_dim), dtype=dtype, device=device)
+        cols = 2 * a.kv_heads * a.head_dim
+        kv = torch.empty((a.n_layers, batch, capacity, cols), dtype=dtype, device=device)
+        scale = None if kv_dtype == "bf16" else torch.empty((a.n_layers, batch, capacity, cols // 32), dtype=torch.uint8, device=device)
         z32 = torch.zeros(batch, dtype=torch.int32, device=device)
-        return cls(kv, z32, z32.clone(), torch.zeros(batch, dtype=torch.int64, device=device), cos, sin, a.sliding_window)
+        return cls(kv, z32, z32.clone(), torch.zeros(batch, dtype=torch.int64, device=device), cos, sin, a.sliding_window, kv_scale=scale)
 
 
 def cache_capacity(max_seq_len: int, prompt_lens: list[int], max_new: int) -> int:
@@ -80,9 +106,10 @@ def cache_capacity(max_seq_len: int, prompt_lens: list[int], max_new: int) -> in
 
 
 @torch.no_grad()
-def prefill(model: Transformer, prompts: list[list[int]], capacity: int) -> tuple[torch.Tensor, KVCache]:
+def prefill(model: Transformer, prompts: list[list[int]], capacity: int, kv_dtype: str = "bf16") -> tuple[torch.Tensor, KVCache]:
     """Run the prompts (right-padded to one length, a multiple of 128 on CUDA) through ``forward_hidden`` while filling a new cache of
-    ``capacity`` rows. Returns the logits [B, V] at each row's last prompt position and the cache, positioned after the prompts."""
+    ``capacity`` rows (``kv_dtype``: see :meth:`KVCache.allocate`). Returns the logits [B, V] at each row's last prompt position and
+    the cache, positioned after the prompts."""
     dev = model.output.device
     lens = [len(p) for p in prompts]
     if min(lens) < 1:
@@ -94,7 +121,7 @@ def prefill(model: Transformer, prompts: list[list[int]], capacity: int) -> tupl
     tokens = torch.zeros((B, S), dtype=torch.int64)
     for b, p in enumerate(prompts):
         tokens[b, : len(p)] = torch.tensor(p, dtype=torch.int64)
-    cache = KVCache.allocate(model, B, capacity, dev)
+    cache = KVCache.allocate(model, B, capacity, dev, kv_dtype)
     # causal attention makes the right padding invisible to the prompt, and the cache rows it fills are overwritten before any
     # query reads them
     x = model.forward_hidden(tokens.to(dev), cache)
@@ -192,9 +219,10 @@ CHECK_EVERY = 16  # device-sampled generation reads the "any row still active" f
 @torch.no_grad()
 def generate_batch(model: Transformer, prompts: list[list[int]], *, max_new: int, temperature: float = 0.0, top_k: int = 0,
                    top_p: float = 1.0, min_p: float = 0.0, seed: int = 0, eos_id: int | None = None, graphs: bool | None = None,
-                   sampler: str = "host") -> list[list[int]]:  # fmt: skip
+                   sampler: str = "host", kv_dtype: str = "bf16") -> list[list[int]]:  # fmt: skip
     """Prompt + continuation of every prompt. A row stops at ``max_new`` new tokens, at ``model.args.max_seq_len`` tokens in all, or
-    after ``eos_id`` (kept). ``graphs``: replay the decode step from a CUDA graph (default: on CUDA).
+    after ``eos_id`` (kept). ``graphs``: replay the decode step from a CUDA graph (default: on CUDA). ``kv_dtype``: "bf16" (default)
+    or "fp8", the e4m3 cache of :meth:`KVCache.allocate`, with half the bytes per value.
 
     ``sampler`` picks the random stream as well as where sampling runs:
 
@@ -206,6 +234,7 @@ def generate_batch(model: Transformer, prompts: list[list[int]], *, max_new: int
       "still active" flag once every 16 steps and the tokens once at the end. Greedy tokens are the same under both samplers."""
     if sampler not in ("host", "device"):
         raise ValueError(f"sampler must be 'host' or 'device', got {sampler!r}")
+    check_kv_dtype(model, kv_dtype)
     model.eval()
     dev = model.output.device
     ids = [list(p) for p in prompts]
@@ -216,9 +245,9 @@ def generate_batch(model: Transformer, prompts: list[list[int]], *, max_new: int
     use_graphs = graphs if graphs is not None else dev.type == "cuda"
     if sampler == "device":
         return _generate_device(model, ids, max_new, dict(temperature=temperature, top_k=top_k, top_p=top_p, min_p=min_p), seed,
-                                eos_id, use_graphs)  # fmt: skip
+                                eos_id, use_graphs, kv_dtype)  # fmt: skip
     gen = torch.Generator(device="cpu").manual_seed(seed)
-    logits, cache = prefill(model, ids, cache_capacity(limit, [len(p) for p in ids], max_new))
+    logits, cache = prefill(model, ids, cache_capacity(limit, [len(p) for p in ids], max_new), kv_dtype)
     if use_graphs:
         step = GraphDecoder(model, cache)
     else:
@@ -239,11 +268,11 @@ def generate_batch(model: Transformer, prompts: list[list[int]], *, max_new: int
 
 
 def _generate_device(model: Transformer, ids: list[list[int]], max_new: int, knobs: dict, seed: int, eos_id: int | None,
-                     graphs: bool) -> list[list[int]]:  # fmt: skip
+                     graphs: bool, kv_dtype: str = "bf16") -> list[list[int]]:  # fmt: skip
     """``generate_batch(sampler="device")``: sampling, the next step's input and the stop rules all stay on the device."""
     dev = model.output.device
     limit = model.args.max_seq_len
-    logits, cache = prefill(model, ids, cache_capacity(limit, [len(p) for p in ids], max_new))
+    logits, cache = prefill(model, ids, cache_capacity(limit, [len(p) for p in ids], max_new), kv_dtype)
     st = SampleState.allocate(ids, max_new, limit, eos_id, dev)
     seeds = torch.tensor([seed + b for b in range(len(ids))], dtype=torch.int64, device=dev)
 
@@ -279,7 +308,7 @@ class SpecResult:
 @torch.no_grad()
 def generate_speculative(model: Transformer, draft: Transformer, prompts: list[list[int]], *, k: int = 4, max_new: int,
                          temperature: float = 0.0, top_k: int = 0, top_p: float = 1.0, min_p: float = 0.0, seed: int = 0,
-                         eos_id: int | None = None, graphs: bool | None = None) -> SpecResult:  # fmt: skip
+                         eos_id: int | None = None, graphs: bool | None = None, kv_dtype: str = "bf16") -> SpecResult:  # fmt: skip
     """Speculative decoding: ``draft`` proposes ``k`` tokens per round and ``model`` checks them in one verify step; the output has the
     distribution of ``generate_batch(sampler="device")`` with the same knobs, and greedy output is the target's greedy output.
 
@@ -297,7 +326,7 @@ def generate_speculative(model: Transformer, draft: Transformer, prompts: list[l
     On CUDA (``graphs`` default) one whole round is one CUDA graph replay over static buffers; the host reads the "any row active"
     flag every 16 rounds and the history once at the end. Without graphs the same calls run eagerly; on the CPU through the
     reference ops. Each model keeps its own window, head dimension and GQA ratio; the vocabulary, device and ``doc_eos_id`` must
-    match."""
+    match. ``kv_dtype`` ("bf16" or "fp8", see :meth:`KVCache.allocate`) applies to the target's and the draft's cache."""
     if draft.args.vocab_size != model.args.vocab_size:
         raise ValueError(f"draft vocabulary {draft.args.vocab_size} != target vocabulary {model.args.vocab_size}")
     if draft.output.device != model.output.device:
@@ -306,6 +335,8 @@ def generate_speculative(model: Transformer, draft: Transformer, prompts: list[l
         raise ValueError(f"draft doc_eos_id {draft.doc_eos_id} != target doc_eos_id {model.doc_eos_id}")
     if not 1 <= k <= MAX_SPEC_K:
         raise ValueError(f"k must be in [1, {MAX_SPEC_K}], got {k}")
+    check_kv_dtype(model, kv_dtype)
+    check_kv_dtype(draft, kv_dtype)
     ops.functional._sample_args(temperature, top_k, top_p, min_p)
     model.eval()
     draft.eval()
@@ -316,8 +347,8 @@ def generate_speculative(model: Transformer, draft: Transformer, prompts: list[l
         return SpecResult(ids, 0, 0, 0)
     B = len(ids)
     cap = _round_up(cache_capacity(limit, [len(p) for p in ids], max_new) + k + 1, PAD)
-    logits, cache = prefill(model, ids, cap)
-    _, dcache = prefill(draft, ids, cap)
+    logits, cache = prefill(model, ids, cap, kv_dtype)
+    _, dcache = prefill(draft, ids, cap, kv_dtype)
     st = SampleState.allocate(ids, max_new, limit, eos_id, dev)
     knobs = dict(temperature=temperature, top_k=top_k, top_p=top_p, min_p=min_p)
     seeds = torch.tensor([seed + b for b in range(B)], dtype=torch.int64, device=dev)

@@ -118,13 +118,13 @@ class Attention(nn.Module):
         H, Hkv, D = self.n_heads, self.n_kv_heads, self.head_dim
         if kv is not None and kv.verifying:
             qkv = ops.linear(x, self.wqkv)  # M = B·T
-            ops.kv_append_tokens(qkv, kv.kv, kv.cache.len, cos, sin, H, Hkv)
-            out = ops.verify_attention(qkv, kv.kv, kv.cache.len, kv.cache.lo_q, kv.cache.window, H, Hkv)
+            ops.kv_append_tokens(qkv, kv.kv, kv.cache.len, cos, sin, H, Hkv, kv_scale=kv.kv_scale)
+            out = ops.verify_attention(qkv, kv.kv, kv.cache.len, kv.cache.lo_q, kv.cache.window, H, Hkv, kv_scale=kv.kv_scale)
             return ops.linear(out, self.wo)
         if kv is not None and kv.decoding:
             qkv = ops.linear(x, self.wqkv).view(B, -1)  # M = B: the new token of every row
-            ops.kv_append(qkv, kv.kv, kv.cache.len, cos, sin, H, Hkv)
-            out = ops.decode_attention(qkv, kv.kv, kv.cache.len, kv.cache.lo, kv.cache.window, H, Hkv)
+            ops.kv_append(qkv, kv.kv, kv.cache.len, cos, sin, H, Hkv, kv_scale=kv.kv_scale)
+            out = ops.decode_attention(qkv, kv.kv, kv.cache.len, kv.cache.lo, kv.cache.window, H, Hkv, kv_scale=kv.kv_scale)
             return ops.linear(out.view(B, 1, H * D), self.wo)
         if self.fp8:
             qkv = ops.linear_mxfp8(x, self.wqkv)

@@ -168,6 +168,11 @@ def _sigs() -> dict:
         "pb_verify_advance": [vp, i32, i64, vp, vp, vp, vp, i32, vp],
         "pb_kv_append_tokens": [vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp],
         "pb_verify_attn": [vp, vp, vp, vp, i32, vp, vp, i32, i32, i32, i32, i32, i32, i32, f32, vp],
+        # the e4m3 KV cache (csrc/decode_sm90.cu)
+        "pb_kv_append_fp8": [vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp],
+        "pb_kv_quantize": [vp, i64, vp, vp, i32, i32, i32, i32, vp],
+        "pb_decode_attn_fp8": [vp, vp, vp, vp, vp, i32, vp, vp, i32, i32, i32, i32, i32, i32, f32, vp],
+        "pb_verify_attn_fp8": [vp, vp, vp, vp, vp, i32, vp, vp, i32, i32, i32, i32, i32, i32, i32, f32, vp],
         # token sampling (csrc/sample_sm90.cu)
         "pb_sample_tokens": [vp, i64, i32, i32, f32, i32, f32, f32, vp, vp, vp, vp, vp, vp, vp, i32, i32, i64, vp],
         "pb_spec_accept": [vp, i64, vp, i64, i32, i32, i32, f32, i32, f32, f32, *[vp] * 14, i32, i32, i64, vp, vp, vp],

@@ -836,11 +836,29 @@ def rope_attention_qkv(qkv: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor, 
 # --------------------------------------------------------------------------- KV-cache decoding
 
 
-def _decode_native(qkv: torch.Tensor, kv: torch.Tensor, n_heads: int, n_kv_heads: int) -> bool:
-    """Shapes and layouts the decode kernels (csrc/decode_sm90.cu) take: bf16, contiguous, D in {64, 128}, H % Hkv == 0."""
+def _decode_native(qkv: torch.Tensor, kv: torch.Tensor, n_heads: int, n_kv_heads: int, kv_scale: torch.Tensor | None = None) -> bool:
+    """Shapes and layouts the decode kernels (csrc/decode_sm90.cu) take: bf16, contiguous, D in {64, 128}, H % Hkv == 0; the cache
+    bf16, or e4m3 (uint8) with its uint8 exponents (see :func:`kv_append`)."""
+    if (kv.dtype == torch.uint8) != (kv_scale is not None):
+        raise ValueError(f"an e4m3 cache is uint8 with a kv_scale tensor, a bf16 cache has none; got {kv.dtype} with kv_scale "
+                         f"{'given' if kv_scale is not None else 'None'}")  # fmt: skip
     D = qkv.shape[-1] // (n_heads + 2 * n_kv_heads)
-    return (qkv.is_cuda and qkv.dtype == torch.bfloat16 and kv.dtype == torch.bfloat16 and qkv.is_contiguous() and kv.is_contiguous()
-            and D in (64, 128) and n_heads % n_kv_heads == 0)  # fmt: skip
+    cache = kv.dtype == torch.bfloat16 if kv_scale is None else kv_scale.dtype == torch.uint8 and kv_scale.is_contiguous()
+    return (qkv.is_cuda and qkv.dtype == torch.bfloat16 and cache and qkv.is_contiguous() and kv.is_contiguous() and D in (64, 128)
+            and n_heads % n_kv_heads == 0)  # fmt: skip
+
+
+def _put_rows(kv: torch.Tensor, kv_scale: torch.Tensor | None, idx: torch.Tensor, ok: torch.Tensor, new: torch.Tensor) -> None:
+    """Cache rows ``new`` [B, cols] into the flat rows ``idx`` of the cache where ``ok``, with no host synchronisation (no nonzero /
+    item: on CUDA the fallbacks are captured in the decode step's graph as well). An e4m3 cache receives ``quantize_kv(new)``."""
+    for dst, val in [(kv, new)] if kv_scale is None else zip((kv, kv_scale), reference.quantize_kv(new)):
+        flat = dst.view(-1, dst.shape[-1])
+        flat.index_copy_(0, idx, torch.where(ok.view(-1, 1), val, flat.index_select(0, idx)))
+
+
+def _cache_values(kv: torch.Tensor, kv_scale: torch.Tensor | None) -> torch.Tensor:
+    """The cache as the fallback attention reads it: the bf16 cache, or the e4m3 cache dequantised (exact, fp32)."""
+    return kv if kv_scale is None else reference.dequantize_kv(kv, kv_scale)
 
 
 def decode_attn_splits(batch: int, n_kv_heads: int, capacity: int) -> int:
@@ -867,17 +885,29 @@ def decode_advance(tokens: torch.Tensor, length: torch.Tensor, lo: torch.Tensor,
 
 
 def kv_append(qkv: torch.Tensor, kv: torch.Tensor, length: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor, n_heads: int,
-              n_kv_heads: int) -> torch.Tensor:  # fmt: skip
+              n_kv_heads: int, kv_scale: torch.Tensor | None = None) -> torch.Tensor:  # fmt: skip
     """The new token of every row, un-rotated fused QKV [B, (H+2Hkv)·D], at position len[b] - 1: rotates its Q heads in place and
     writes its rotated K heads and its V heads into row len[b] - 1 of the layer's cache ``kv`` [B, capacity, 2·Hkv·D]. Rows whose
-    position is outside the cache are left alone. Returns ``qkv``."""
+    position is outside the cache are left alone. Returns ``qkv``.
+
+    The e4m3 cache (``kv`` uint8 with ``kv_scale``; CUDA: ``pb_kv_append_fp8``) has the same layout in bytes, and ``kv_scale`` uint8
+    [B, capacity, 2·Hkv·D/32] holds one biased UE8M0 exponent e per 32 columns of a row (columns 32j .. 32j+31 → byte j; D % 32 ==
+    0, so a block never straddles two heads): the value is e4m3 · 2^(e-127). The rule is MXFP8's (``reference.quantize_mxfp8``,
+    csrc/mx_common.cuh): the smallest power of two s with amax / s <= 448, e clamped to [1, 254], then x / s rounded to nearest even
+    with saturation. Its input is the value the bf16 cache would hold, the rotated K after its one bf16 rounding and V as is, so the
+    e4m3 cache is ``reference.quantize_kv`` of the bf16 cache byte for byte, and every dequantised value is exact in fp32 and bf16.
+    Queries stay bf16; rows past ``len`` are never read."""
     B = qkv.shape[0]
     H, Hkv = n_heads, n_kv_heads
     D = qkv.shape[-1] // (H + 2 * Hkv)
     cap = kv.shape[1]
-    if _decode_native(qkv, kv, H, Hkv):
+    if _decode_native(qkv, kv, H, Hkv, kv_scale):
         assert length.dtype == torch.int32 and cos.dtype == torch.float32 and cos.is_contiguous() and sin.is_contiguous()
         assert cos.shape[0] >= cap and cos.shape[1] == D // 2
+        if kv_scale is not None:
+            _launch("pb_kv_append_fp8", qkv.data_ptr(), kv.data_ptr(), kv_scale.data_ptr(), length.data_ptr(), cos.data_ptr(),
+                    sin.data_ptr(), B, 1, H, Hkv, D, cap, _stream())  # fmt: skip
+            return qkv
         _launch("pb_kv_append", qkv.data_ptr(), kv.data_ptr(), length.data_ptr(), cos.data_ptr(), sin.data_ptr(), B, H, Hkv, D, cap,
                 _stream())  # fmt: skip
         return qkv
@@ -886,36 +916,53 @@ def kv_append(qkv: torch.Tensor, kv: torch.Tensor, length: torch.Tensor, cos: to
     p = pos.clamp(0, cap - 1)
     x = qkv.view(B, H + 2 * Hkv, D)
     rot = reference.rope_at(x[:, : H + Hkv], cos[p], sin[p])
-    # no host synchronisation (no nonzero / item): on CUDA this fallback is captured in the decode step's graph as well
-    flat = kv.view(B * cap, -1)
     idx = torch.arange(B, device=kv.device) * cap + p
     new = torch.cat((rot[:, H:], x[:, H + Hkv :]), dim=1).reshape(B, -1)
-    flat.index_copy_(0, idx, torch.where(ok.view(B, 1), new, flat.index_select(0, idx)))
+    _put_rows(kv, kv_scale, idx, ok, new)
     x[:, :H] = torch.where(ok.view(B, 1, 1), rot[:, :H], x[:, :H])
     return qkv
 
 
+def kv_quantize(src: torch.Tensor, kv: torch.Tensor, kv_scale: torch.Tensor) -> None:
+    """Prefill of an e4m3 cache: the rows ``src`` [B, S, cols] (the rotated K|V columns of the fused QKV activation, a strided view
+    with unit column stride) quantised into rows 0 .. S-1 of ``kv`` uint8 [B, capacity, cols] and ``kv_scale`` uint8 [B, capacity,
+    cols / 32] by the rule of :func:`kv_append`. On CUDA the native ``pb_kv_quantize`` reads the strided bf16 rows once, with no
+    temporaries."""
+    B, S, cols = src.shape
+    if src.is_cuda:
+        assert src.dtype == torch.bfloat16 and kv.dtype == kv_scale.dtype == torch.uint8 and kv.is_contiguous() and kv_scale.is_contiguous()
+        assert src.stride(2) == 1 and src.stride(0) == S * src.stride(1) and kv.shape[-1] == cols and kv_scale.shape[-1] == cols // 32
+        _launch("pb_kv_quantize", src.data_ptr(), src.stride(1), kv.data_ptr(), kv_scale.data_ptr(), B, S, cols, kv.shape[1], _stream())
+        return
+    q, e = reference.quantize_kv(src)
+    kv[:, :S].copy_(q)
+    kv_scale[:, :S].copy_(e)
+
+
 def decode_attention(qkv: torch.Tensor, kv: torch.Tensor, length: torch.Tensor, lo: torch.Tensor | None, window: int | None,
-                     n_heads: int, n_kv_heads: int, splits: int | None = None) -> torch.Tensor:  # fmt: skip
+                     n_heads: int, n_kv_heads: int, splits: int | None = None, kv_scale: torch.Tensor | None = None) -> torch.Tensor:  # fmt: skip
     """Attention of the one (rotated) query per row in ``qkv`` [B, (H+2Hkv)·D] over the layer's cache ``kv`` [B, capacity, 2·Hkv·D]
     → [B, H·D]. Row b sees keys max(lo[b], len[b] - window) <= k < len[b] (``lo`` None = 0, ``window`` None = none). On CUDA the
     split-KV kernel (one launch, or two with the combine when ``splits`` > 1; None = :func:`decode_attn_splits`), else the fp32
-    :func:`reference.decode_attention`."""
+    :func:`reference.decode_attention`. ``kv_scale``: the cache is e4m3 (:func:`kv_append`); the kernel computes the bf16 kernel's
+    sums over the dequantised cache, and the fallback dequantises it."""
     B = qkv.shape[0]
     H, Hkv = n_heads, n_kv_heads
     D = qkv.shape[-1] // (H + 2 * Hkv)
     cap = kv.shape[1]
-    if _decode_native(qkv, kv, H, Hkv):
+    if _decode_native(qkv, kv, H, Hkv, kv_scale):
         assert length.dtype == torch.int32 and (lo is None or lo.dtype == torch.int32)
         if splits is None:
             splits = decode_attn_splits(B, Hkv, cap)
         out = torch.empty((B, H * D), dtype=qkv.dtype, device=qkv.device)
         part = torch.empty((B, H, splits, D + 2), dtype=torch.float32, device=qkv.device) if splits > 1 else None
-        _launch("pb_decode_attn", qkv.data_ptr(), kv.data_ptr(), length.data_ptr(), _ptr(lo), int(window or 0), out.data_ptr(), _ptr(part),
-                B, H, Hkv, D, cap, splits, 1.0 / math.sqrt(D), _stream(), n=1 if splits == 1 else 2)  # fmt: skip
+        fp8 = () if kv_scale is None else (kv_scale.data_ptr(),)
+        _launch("pb_decode_attn" if kv_scale is None else "pb_decode_attn_fp8", qkv.data_ptr(), kv.data_ptr(), *fp8, length.data_ptr(),
+                _ptr(lo), int(window or 0), out.data_ptr(), _ptr(part), B, H, Hkv, D, cap, splits, 1.0 / math.sqrt(D), _stream(),
+                n=1 if splits == 1 else 2)  # fmt: skip
         return out
     q = qkv.view(B, H + 2 * Hkv, D)[:, :H]
-    return reference.decode_attention(q, kv, length, lo, window).reshape(B, H * D).to(qkv.dtype)
+    return reference.decode_attention(q, _cache_values(kv, kv_scale), length, lo, window).reshape(B, H * D).to(qkv.dtype)
 
 
 # --------------------------------------------------------------------------- sampling
@@ -1019,45 +1066,51 @@ def verify_advance(tokens: torch.Tensor, length: torch.Tensor, lo: torch.Tensor,
 
 
 def kv_append_tokens(qkv: torch.Tensor, kv: torch.Tensor, length: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor, n_heads: int,
-                     n_kv_heads: int) -> torch.Tensor:  # fmt: skip
+                     n_kv_heads: int, kv_scale: torch.Tensor | None = None) -> torch.Tensor:  # fmt: skip
     """:func:`kv_append` for T tokens per row: ``qkv`` [B, T, (H+2Hkv)·D], token t of row b at position len[b] - T + t. Positions
-    outside the cache are left alone. Returns ``qkv``."""
+    outside the cache are left alone. Returns ``qkv``. ``kv_scale``: the cache is e4m3."""
     B, T = qkv.shape[:2]
     H, Hkv = n_heads, n_kv_heads
     D = qkv.shape[-1] // (H + 2 * Hkv)
     cap = kv.shape[1]
-    if _decode_native(qkv, kv, H, Hkv):
+    if _decode_native(qkv, kv, H, Hkv, kv_scale):
         assert length.dtype == torch.int32 and cos.dtype == torch.float32 and cos.is_contiguous() and sin.is_contiguous()
         assert cos.shape[0] >= cap and cos.shape[1] == D // 2
+        if kv_scale is not None:
+            _launch("pb_kv_append_fp8", qkv.data_ptr(), kv.data_ptr(), kv_scale.data_ptr(), length.data_ptr(), cos.data_ptr(),
+                    sin.data_ptr(), B, T, H, Hkv, D, cap, _stream())  # fmt: skip
+            return qkv
         _launch("pb_kv_append_tokens", qkv.data_ptr(), kv.data_ptr(), length.data_ptr(), cos.data_ptr(), sin.data_ptr(), B, T, H, Hkv,
                 D, cap, _stream())  # fmt: skip
         return qkv
     for t in range(T):  # token t is the one a decode step would append with len = len - T + t + 1
-        kv_append(qkv[:, t], kv, length - (T - 1 - t), cos, sin, H, Hkv)
+        kv_append(qkv[:, t], kv, length - (T - 1 - t), cos, sin, H, Hkv, kv_scale)
     return qkv
 
 
 def verify_attention(qkv: torch.Tensor, kv: torch.Tensor, length: torch.Tensor, lo_q: torch.Tensor | None, window: int | None,
-                     n_heads: int, n_kv_heads: int, splits: int | None = None) -> torch.Tensor:  # fmt: skip
+                     n_heads: int, n_kv_heads: int, splits: int | None = None, kv_scale: torch.Tensor | None = None) -> torch.Tensor:  # fmt: skip
     """Attention of T (rotated) queries per row, ``qkv`` [B, T, (H+2Hkv)·D], over the layer's cache → [B, T, H·D]. Query t of row b
     sits at position pos = len[b] - T + t and sees keys max(lo_q[b, t], pos + 1 - window) <= k <= pos. On CUDA the split-KV verify
     kernel with the split policy of :func:`decode_attn_splits` (at T = 1 bitwise equal to :func:`decode_attention`), else the fp32
-    :func:`reference.verify_attention`."""
+    :func:`reference.verify_attention`. ``kv_scale``: the cache is e4m3, as in :func:`decode_attention`."""
     B, T = qkv.shape[:2]
     H, Hkv = n_heads, n_kv_heads
     D = qkv.shape[-1] // (H + 2 * Hkv)
     cap = kv.shape[1]
-    if _decode_native(qkv, kv, H, Hkv):
+    if _decode_native(qkv, kv, H, Hkv, kv_scale):
         assert length.dtype == torch.int32 and (lo_q is None or (lo_q.dtype == torch.int32 and lo_q.is_contiguous()))
         if splits is None:
             splits = decode_attn_splits(B, Hkv, cap)
         out = torch.empty((B, T, H * D), dtype=qkv.dtype, device=qkv.device)
         part = torch.empty((B, T, H, splits, D + 2), dtype=torch.float32, device=qkv.device) if splits > 1 else None
-        _launch("pb_verify_attn", qkv.data_ptr(), kv.data_ptr(), length.data_ptr(), _ptr(lo_q), int(window or 0), out.data_ptr(),
-                _ptr(part), B, T, H, Hkv, D, cap, splits, 1.0 / math.sqrt(D), _stream(), n=1 if splits == 1 else 2)  # fmt: skip
+        fp8 = () if kv_scale is None else (kv_scale.data_ptr(),)
+        _launch("pb_verify_attn" if kv_scale is None else "pb_verify_attn_fp8", qkv.data_ptr(), kv.data_ptr(), *fp8, length.data_ptr(),
+                _ptr(lo_q), int(window or 0), out.data_ptr(), _ptr(part), B, T, H, Hkv, D, cap, splits, 1.0 / math.sqrt(D), _stream(),
+                n=1 if splits == 1 else 2)  # fmt: skip
         return out
     q = qkv.view(B, T, H + 2 * Hkv, D)[:, :, :H]
-    return reference.verify_attention(q, kv, length, lo_q, window).reshape(B, T, H * D).to(qkv.dtype)
+    return reference.verify_attention(q, _cache_values(kv, kv_scale), length, lo_q, window).reshape(B, T, H * D).to(qkv.dtype)
 
 
 def spec_accept(target_logits: torch.Tensor, draft_logits: torch.Tensor, *, temperature: float = 0.0, top_k: int = 0, top_p: float = 1.0,

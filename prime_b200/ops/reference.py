@@ -427,19 +427,26 @@ def _mxfp8_sf_index(rows: int, k: int, device=None) -> torch.Tensor:
     return ((kb >> 2) * atoms + (r >> 7)) * 512 + (r & 31) * 16 + ((r & 127) >> 5) * 4 + (kb & 3)
 
 
-def quantize_mxfp8(x: torch.Tensor, transpose: bool = False) -> tuple[torch.Tensor, torch.Tensor]:
-    """OCP MX e4m3: per 32 contiguous contraction elements a power-of-two scale 2^e, the smallest with amax / 2^e <= 448."""
-    xf = (x.t() if transpose else x).float().contiguous()
-    rows, k = xf.shape
-    assert k % 128 == 0
-    blocks = xf.view(rows, k // 32, 32)
+def _mx_e4m3(blocks: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor]:
+    """The MX e4m3 rule on fp32 blocks [..., 32]: the exponent e (int32 [...]) of the smallest power of two 2^(e-127) with
+    amax / 2^(e-127) <= 448, e clamped to [1, 254], and the e4m3 bytes (uint8 [..., 32]) of x / 2^(e-127), rounded to nearest even
+    with saturation (csrc/mx_common.cuh)."""
     amax = blocks.abs().amax(dim=-1)
     v = (amax * (1.0 / 448.0)).to(torch.float32)
     bits = v.view(torch.int32)
     e = (bits >> 23) & 0xFF
     e = torch.where((bits & 0x7FFFFF) != 0, e + 1, e).clamp(1, 254)
     inv = ((254 - e) << 23).to(torch.int32).view(torch.float32)
-    q = (blocks * inv.unsqueeze(-1)).clamp(-448.0, 448.0).to(torch.float8_e4m3fn).view(torch.uint8).view(rows, k)
+    return (blocks * inv.unsqueeze(-1)).clamp(-448.0, 448.0).to(torch.float8_e4m3fn).view(torch.uint8), e
+
+
+def quantize_mxfp8(x: torch.Tensor, transpose: bool = False) -> tuple[torch.Tensor, torch.Tensor]:
+    """OCP MX e4m3: per 32 contiguous contraction elements a power-of-two scale 2^e, the smallest with amax / 2^e <= 448."""
+    xf = (x.t() if transpose else x).float().contiguous()
+    rows, k = xf.shape
+    assert k % 128 == 0
+    q, e = _mx_e4m3(xf.view(rows, k // 32, 32))
+    q = q.view(rows, k)
     sf = torch.full(((k // 128) * ((rows + 127) // 128 + 1) * 512,), 127, dtype=torch.uint8, device=x.device)
     sf[_mxfp8_sf_index(rows, k, x.device).reshape(-1)] = e.to(torch.uint8).reshape(-1)
     return q, sf
@@ -450,3 +457,20 @@ def dequantize_mxfp8(q: torch.Tensor, sf: torch.Tensor) -> torch.Tensor:
     e = sf[_mxfp8_sf_index(rows, k, q.device).reshape(-1)].view(rows, k // 32).to(torch.int32)
     scale = (e << 23).view(torch.float32)
     return (q.view(torch.float8_e4m3fn).float().view(rows, k // 32, 32) * scale.unsqueeze(-1)).view(rows, k)
+
+
+# ----------------------------------------------------------------------------------------------------------- e4m3 KV cache
+def quantize_kv(x: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor]:
+    """Cache rows x [..., C] (C % 32 == 0; the values the bf16 cache would hold) → (e4m3 bytes uint8 [..., C], UE8M0 exponents
+    uint8 [..., C / 32]): the MX rule of :func:`quantize_mxfp8` per 32 consecutive columns, the exponents stored dense."""
+    C = x.shape[-1]
+    assert C % 32 == 0, C
+    q, e = _mx_e4m3(x.float().reshape(*x.shape[:-1], C // 32, 32))
+    return q.reshape(x.shape), e.to(torch.uint8)
+
+
+def dequantize_kv(q: torch.Tensor, e: torch.Tensor) -> torch.Tensor:
+    """fp32 [..., C] of :func:`quantize_kv`'s output: every value e4m3 · 2^(e - 127), exact."""
+    C = q.shape[-1]
+    scale = (e.to(torch.int32) << 23).view(torch.float32)
+    return (q.view(torch.float8_e4m3fn).float().reshape(*q.shape[:-1], C // 32, 32) * scale.unsqueeze(-1)).reshape(q.shape)

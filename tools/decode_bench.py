@@ -28,6 +28,15 @@ acceptance of ``generate_speculative`` with the target as its own draft (the ove
 floor, random weights agree rarely), next to ``generate_batch(sampler="device")``.
 
     python tools/decode_bench.py --speculative
+
+fp8 KV-cache section (``--kv-fp8``, alone): decode attention over the bf16 cache and over the e4m3 cache (``kv_dtype="fp8"``) at the
+shapes of the kernel section, timed the same way, with GB/s counted from the bytes each must read (bf16: 2 bytes per value; fp8: 1
+byte per value plus one scale byte per 32). Then a random-init Llama-2 1B at B = 8 with a 16 K-token prompt, device sampler, CUDA
+graphs: decode tokens/s with either cache (the time of 129 new tokens minus that of 1, so the prefill cancels). Last, a random-init
+Llama-2 7B at B = 4 and 32 K context (``max_seq_len`` = 32768): the cache bytes of both dtypes from the shapes, and decode tokens/s
+with the fp8 cache only, since the bf16 one does not fit next to the weights.
+
+    python tools/decode_bench.py --kv-fp8
 """
 
 from __future__ import annotations
@@ -328,12 +337,88 @@ def speculative_section(prompt_len: int = 512, new: int = 256) -> list[dict]:
     return rows
 
 
+def _kv_fp8_kernel_rows(flush) -> list[dict]:
+    rows = []
+    D = 128
+    dev = torch.device("cuda", 0)
+    cases = [(H, Hkv, B, ctx, None) for (H, Hkv) in ((16, 16), (32, 8)) for B in (1, 8, 32) for ctx in (1024, 8192, 32768)]
+    cases.append((32, 8, 8, 32768, 4096))
+    for H, Hkv, B, ctx, window in cases:
+        cols = 2 * Hkv * D
+        kv = torch.randn(B, ctx, cols, device=dev, dtype=torch.bfloat16)
+        kv8 = torch.empty(B, ctx, cols, dtype=torch.uint8, device=dev)
+        sc = torch.empty(B, ctx, cols // 32, dtype=torch.uint8, device=dev)
+        ops.kv_quantize(kv, kv8, sc)
+        qkv = torch.randn(B, (H + 2 * Hkv) * D, device=dev, dtype=torch.bfloat16)
+        length = torch.full((B,), ctx, dtype=torch.int32, device=dev)
+        vis = min(ctx, window or ctx)
+        r = {"heads": f"{H}/{Hkv}", "B": B, "context": ctx, "window": window, "splits": ops.decode_attn_splits(B, Hkv, ctx)}
+        for name, args, per_value in (("bf16", (kv, None), 2.0), ("fp8", (kv8, sc), 1.0 + 1.0 / 32)):
+            ms = timed(lambda: ops.decode_attention(qkv, args[0], length, None, window, H, Hkv, kv_scale=args[1]), flush)
+            nbytes = B * vis * cols * per_value + 2 * B * H * D * 2
+            r[f"{name}_ms"] = round(ms, 4)
+            r[f"{name}_GB_s"] = round(nbytes / ms / 1e6, 1)
+        r["fp8_speedup"] = round(r["bf16_ms"] / r["fp8_ms"], 2)
+        print(json.dumps(r), flush=True)
+        rows.append(r)
+        del kv, kv8, sc, qkv
+        torch.cuda.empty_cache()
+    return rows
+
+
+def _decode_tok_s(model, prompts, new: int, kv_dtype: str) -> float:
+    """Decode tokens/s of generate_batch(sampler="device", graphs on): (new − 1)·B tokens over the time of ``new`` new tokens
+    minus that of 1 (the prefill and the first token cancel)."""
+
+    def run(n):
+        torch.cuda.synchronize()
+        t = time.perf_counter()
+        inference.generate_batch(model, prompts, max_new=n, sampler="device", kv_dtype=kv_dtype)
+        torch.cuda.synchronize()
+        return time.perf_counter() - t
+
+    run(8)  # warm-up
+    return (new - 1) * len(prompts) / (run(new) - run(1))
+
+
+def kv_fp8_section(flush) -> dict:
+    out = {"kernel": _kv_fp8_kernel_rows(flush)}
+    g = torch.Generator().manual_seed(0)
+    model = build_model("1B", device="cuda", dtype=torch.bfloat16, seed=0, max_seq_len=16384 + 256).eval()
+    prompts = torch.randint(1, model.args.vocab_size, (8, 16384), generator=g).tolist()
+    r = {"model": "llama2 1B", "B": 8, "prompt": 16384, "new_tokens": 128}
+    for kv_dtype in ("bf16", "fp8"):
+        r[f"{kv_dtype}_tok_s"] = round(_decode_tok_s(model, prompts, 129, kv_dtype), 1)
+    r["fp8_over_bf16"] = round(r["fp8_tok_s"] / r["bf16_tok_s"], 3)
+    print(json.dumps(r), flush=True)
+    out["e2e_1b"] = r
+    del model
+    torch.cuda.empty_cache()
+    model = build_model("7B", device="cuda", dtype=torch.bfloat16, seed=0, max_seq_len=32768).eval()
+    a = model.args
+    B, ctx, new = 4, 32768, 64
+    per_row = a.n_layers * ctx * 2 * a.kv_heads * a.head_dim
+    r = {"model": "llama2 7B", "B": B, "context": ctx, "weights_GB": round(sum(p.numel() for p in model.parameters()) * 2 / 1e9, 2),
+         "cache_GiB_bf16": round(B * per_row * 2 / 2**30, 2), "cache_GiB_fp8": round(B * per_row * (1 + 1 / 32) / 2**30, 2),
+         "new_tokens": new}  # fmt: skip
+    prompts = torch.randint(1, a.vocab_size, (B, ctx - new), generator=g).tolist()
+    try:
+        r["fp8_tok_s"] = round(_decode_tok_s(model, prompts, new, "fp8"), 1)
+        r["peak_allocated_GB"] = round(torch.cuda.max_memory_allocated() / 1e9, 2)
+    except torch.cuda.OutOfMemoryError as e:
+        r["fp8_tok_s"] = f"out of memory: {str(e).splitlines()[0]}"
+    print(json.dumps(r), flush=True)
+    out["7b_32k"] = r
+    return out
+
+
 def main() -> None:
     ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
     ap.add_argument("--out", default=None, help="also write the results as JSON here")
     ap.add_argument("--skip-e2e", action="store_true")
     ap.add_argument("--only-sampler", action="store_true", help="run only the two sampler sections")
     ap.add_argument("--speculative", action="store_true", help="run only the speculative-decoding section")
+    ap.add_argument("--kv-fp8", action="store_true", help="run only the fp8 KV-cache section")
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("decode_bench needs a CUDA device")
@@ -341,8 +426,11 @@ def main() -> None:
     print(json.dumps({"card": info}), flush=True)
     flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")
     res = {"card": info}
-    if a.speculative:
-        res["speculative"] = speculative_section()
+    if a.speculative or a.kv_fp8:
+        if a.speculative:
+            res["speculative"] = speculative_section()
+        if a.kv_fp8:
+            res["kv_fp8"] = kv_fp8_section(flush)
         if a.out:
             Path(a.out).parent.mkdir(parents=True, exist_ok=True)
             Path(a.out).write_text(json.dumps(res, indent=1))

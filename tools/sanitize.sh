@@ -21,6 +21,9 @@ run memcheck  "gpu and not 16384 and not 128256 and not 14336" memcheck_edges te
 run synccheck "mxfp8 or swiglu_epilogue" synccheck_mxfp8
 # decode kernels: KV append, step bookkeeping and split-KV attention at the small shapes (the 32 K-key fp64 sweep is left to the plain run)
 run memcheck  "gpu and (kv_append or decode_advance or graph_replay or generate_on_cuda)" memcheck_decode tests/test_kv_cache.py
+# the e4m3 cache: append and prefill quantisers, verify attention at cap 2048, graphs and speculative rounds (the 32 K-key sweep, the
+# 8 K bound check and the 1B models are left to the plain run)
+run memcheck  "gpu and not decode_attn_fp8_matches and not analytic_bound and not 1b_shape" memcheck_kv_fp8 tests/test_kv_fp8_gpu.py
 # flash attention against fp64: every instantiation, tile-edge documents and windows, probes (S >= 4096 is left to the plain run)
 run memcheck  "gpu and not S4096 and not S8192 and not 32768" memcheck_attention_fp64 tests/test_attention_fp64_gpu.py
 run racecheck "gpu and not S4096 and not S8192 and not 32768 and not doc_bounds" racecheck_attention_fp64 tests/test_attention_fp64_gpu.py
