@@ -7,6 +7,7 @@
     python -m prime_b200.eval generate --ckpt … --model 1B --prompt-ids 1,306,626 --temperature 0.8 --top-p 0.9 --sampler device
     python -m prime_b200.eval generate --ckpt … --model 1B --draft-ckpt … --draft-model 150M --spec-k 4 --prompt-ids 1,306,626
     python -m prime_b200.eval generate --ckpt … --model 1B --prompt-ids 1,306,626 --kv-dtype fp8   # e4m3 KV cache: half the bytes
+    python -m prime_b200.eval generate --ckpt … --model 1B --prompt-ids 1,306,626 --weight-dtype fp8   # e4m3 projection weights
 
 The model is rebuilt on one device from the per-rank optimizer shards (``checkpoint.assemble_full_model``) or from a Hugging
 Face directory (``models.hf.load_hf_dir``); the forward runs through the same ops as training (native kernels on an H100, the
@@ -14,6 +15,11 @@ reference ops on the CPU).  Generation runs on a KV cache (``inference.py``): on
 on CUDA, then one decode step per token (the split-KV decode-attention kernel, the step replayed from a CUDA graph on the GPU), so
 T new tokens cost one prompt forward and T single-token steps instead of T full forwards. ``generate_batch`` samples ragged
 prompt lists together. Sliding windows and document masking (``Transformer.doc_eos_id``) behave as in the full forward.
+
+``--weight-dtype fp8`` (both commands; with a draft model it converts the draft as well) runs ``inference.quantize_weights`` after
+loading: the four projections of every block and the LM head are held as e4m3 with a power-of-two scale per 32 values (about 1.03
+bytes per weight instead of 2). Decode and verify steps read those bytes in place (``ops.linear`` on an ``ops.MXWeight``); prefill and
+perplexity run the bf16 kernels on the exactly dequantised weights. The embedding and the norms stay as loaded.
 """
 
 from __future__ import annotations
@@ -27,7 +33,7 @@ import torch.nn.functional as F
 
 from . import ops
 from .data import MemmapTokenDataset
-from .inference import generate_batch, generate_speculative, sample
+from .inference import generate_batch, generate_speculative, quantize_weights, sample
 from .models.llama import Transformer
 
 
@@ -112,6 +118,8 @@ def main(argv: list[str] | None = None) -> dict:
         p.add_argument("--model", default="1B")
         p.add_argument("--type-model", default="llama2", choices=["llama2", "llama3"])
         p.add_argument("--device", default="cuda" if torch.cuda.is_available() else "cpu")
+        p.add_argument("--weight-dtype", default="bf16", choices=["bf16", "fp8"],
+                       help="projection weights: as loaded, or fp8 = e4m3 with a power-of-two scale per 32 values (inference only)")
     p = sub.choices["ppl"]
     p.add_argument("--data", required=True, help="token files / directory / glob (see tools/tokenize_corpus.py)")
     p.add_argument("--seq", type=int, default=1024)
@@ -144,6 +152,8 @@ def main(argv: list[str] | None = None) -> dict:
     if spec and a.sampler == "host":
         raise SystemExit("speculative decoding samples on the device: --sampler host cannot be combined with a draft model")
     model = load_model(a, a.device)
+    if a.weight_dtype == "fp8":
+        quantize_weights(model)
     if a.cmd == "ppl":
         if a.document_mask or a.eos_id is not None:
             from .data import eos_id_from_meta
@@ -155,7 +165,10 @@ def main(argv: list[str] | None = None) -> dict:
         ds = MemmapTokenDataset(a.data, a.seq, vocab_size=model.args.vocab_size, shuffle=False)
         out = perplexity(model, ds, batches=min(a.batches, max(1, ds.windows // a.batch_size)), batch_size=a.batch_size, device=a.device)
     elif spec:
-        r = generate_speculative(model, load_model(a, a.device, "draft_"), [[int(x) for x in a.prompt_ids.split(",")]], k=a.spec_k,
+        draft = load_model(a, a.device, "draft_")
+        if a.weight_dtype == "fp8":
+            quantize_weights(draft)
+        r = generate_speculative(model, draft, [[int(x) for x in a.prompt_ids.split(",")]], k=a.spec_k,
                                  max_new=a.max_new, temperature=a.temperature, top_k=a.top_k, top_p=a.top_p, min_p=a.min_p,
                                  seed=a.seed, kv_dtype=a.kv_dtype)  # fmt: skip
         out = {"ids": r.ids[0], "spec": {"rounds": r.rounds, "drafted": r.drafted, "accepted": r.accepted,

@@ -8,6 +8,9 @@ strided copy per layer and a decode step appends one row per sequence (``ops.kv_
 the bytes it reads, reads about half as many. The per-row state (``len``, ``lo``: the first key the current query may see, ``last_tok``) lives on the
 device, so a decode step depends on no host value that changes between tokens.
 
+``quantize_weights`` converts a model's projections to e4m3 (``ops.MXWeight``) for inference: every entry point here then runs
+unchanged, the decode and verify steps reading about 1.03 bytes per weight instead of 2.
+
 Sampling runs on the host (one CPU generator, the stream of earlier versions) or, with ``sampler="device"``, inside the step:
 ``ops.sample_tokens`` draws each row's next token from a Philox stream keyed by (seed, position), writes it into the step's static
 input buffer and applies the stop rules on the device, so the captured graph runs step after step without the host.
@@ -291,6 +294,45 @@ def _generate_device(model: Transformer, ids: list[list[int]], max_new: int, kno
             advance()
     hist, n = st.history.cpu(), st.n_out.cpu()
     return [p + hist[b, : int(n[b])].tolist() for b, p in enumerate(ids)]
+
+
+# ------------------------------------------------------------------------------------------------------------- e4m3 weights
+def _projections(model: Transformer) -> list[tuple[torch.nn.Module, str]]:
+    """(module, attribute) of every weight ``quantize_weights`` converts: each block's wqkv, wo, w13 and w2, then the LM head."""
+    out = []
+    for blk in model.layers:
+        out += [(blk.attention, "wqkv"), (blk.attention, "wo"), (blk.feed_forward, "w13"), (blk.feed_forward, "w2")]
+    return out + [(model, "output")]
+
+
+@torch.no_grad()
+def quantize_weights(model: Transformer) -> Transformer:
+    """Convert, in place, ``wqkv``, ``wo``, ``w13`` and ``w2`` of every block and the LM head ``output`` to e4m3 ``ops.MXWeight``s
+    (``ops.quantize_weight``: one power-of-two scale per 32 values along the contraction dimension) for inference. Each parameter is
+    freed as soon as it is converted, so the peak stays near the model's own size. The embedding and the norms are left alone.
+
+    Afterwards ``prefill``, ``generate_batch``, ``generate_speculative`` and ``eval.perplexity`` run as before: decode and verify steps
+    read the e4m3 bytes in place (``ops.gemm_e4m3w``), prefill and full forwards run the bf16 kernels on the exactly dequantised
+    weights, and on the CPU everything runs the reference on W̃. The model can no longer be trained. Returns ``model``.
+
+    Raises ``ValueError`` for a contraction dimension that is not a multiple of 128, a model with MXFP8 training GEMMs on
+    (``set_fp8(True)``), ZeRO-3-sharded parameters, or a model that is already quantised."""
+    slots = _projections(model)
+    if any(isinstance(getattr(m, n), ops.MXWeight) for m, n in slots):
+        raise ValueError("the model's weights are already e4m3")
+    if any(blk.attention.fp8 or blk.feed_forward.fp8 for blk in model.layers):
+        raise ValueError("a model with MXFP8 training GEMMs (set_fp8(True)) cannot be converted; call set_fp8(False) first")
+    if any(getattr(getattr(m, n), "z3", None) is not None for m, n in slots):
+        raise ValueError("ZeRO-3-sharded weights cannot be converted to e4m3; assemble the full model first")
+    for m, n in slots:
+        w = getattr(m, n)
+        if w.shape[1] % 128:
+            raise ValueError(f"e4m3 weights need a contraction dimension % 128 == 0; {type(m).__name__}.{n} is {tuple(w.shape)}")
+    for m, n in slots:
+        mx = ops.quantize_weight(getattr(m, n))
+        delattr(m, n)  # the parameter (and, once the caller holds no reference to it, its memory) goes here
+        setattr(m, n, mx)
+    return model
 
 
 # ----------------------------------------------------------------------------------------------------------- speculative decoding

@@ -154,6 +154,11 @@ def _sigs() -> dict:
         "pb_gemm_reduce_scatter": [vp, vp, vp, i32, i32, i32, i32, i32, i32, i32, i32, i32, vp],
         "pb_quantize_mxfp8": [vp, i64, vp, vp, i32, i32, i32, vp],
         "pb_gemm_mxfp8": [vp, vp, vp, vp, vp, i32, i32, i32, i32, vp],
+        # e4m3 inference weights (csrc/gemm_e4m3w_sm90.cu)
+        "pb_gemm_e4m3w": [vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, vp],
+        "pb_gemm_e4m3w_splits": [i32, i32, i32, i32],
+        "pb_gemm_e4m3w_m_max": [],
+        "pb_dequantize_mxfp8": [vp, vp, vp, i32, i32, i64, vp],
         "pb_gemm_set_split_k": [i32],
         "pb_gemm_set_tile": [i32],
         "pb_gemm_tile_policy": [i32, i32, i32, i32, i32, i32, i32],

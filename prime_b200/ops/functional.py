@@ -9,6 +9,7 @@ native library on the *current* torch stream (so they compose with streams and C
 from __future__ import annotations
 
 import math
+from dataclasses import dataclass
 
 import torch
 
@@ -198,7 +199,21 @@ def _gemm_epi(a: torch.Tensor, w: torch.Tensor, out: torch.Tensor, *, b_mn_major
 
 
 def _matmul(a: torch.Tensor, weight: torch.Tensor, out: torch.Tensor, **epi) -> torch.Tensor:
-    """:func:`_gemm_epi` on ``weight``, gathered from the peers' shards inside the GEMM when it is ZeRO-3 sharded (``weight.z3``)."""
+    """:func:`_gemm_epi` on ``weight``, gathered from the peers' shards inside the GEMM when it is ZeRO-3 sharded (``weight.z3``).
+    An e4m3 :class:`MXWeight` (forward only): at M <= :func:`gemm_e4m3w_m_max` the skinny kernel reads its bytes in place, with
+    SwiGLU as the separate kernel (no RoPE epilogue: decode and verify rotate in the cache append); above it the weight is
+    dequantised into a transient bf16 buffer and the bf16 GEMM runs with its epilogues, as it would on the bf16 model holding W̃."""
+    if isinstance(weight, MXWeight):
+        assert not epi.get("b_mn_major") and epi.get("swiglu_bwd_gu") is None, "e4m3 weights have no backward"
+        M = a.shape[0]
+        if M > gemm_e4m3w_m_max():
+            return _gemm_epi(a, dequantize_weight(weight), out, rope=epi.get("rope"), swiglu_h=epi.get("swiglu_h"))
+        assert epi.get("rope") is None, "the skinny e4m3 GEMM has no RoPE epilogue"
+        gemm_e4m3w(a, weight, out=out)
+        h = epi.get("swiglu_h")
+        if h is not None:
+            _launch("pb_swiglu_fwd", out.data_ptr(), h.data_ptr(), M, weight.shape[0] // 2, _stream())
+        return out
     z = getattr(weight, "z3", None)
     if z is not None:
         return gemm_wgather(a, z, out=out, **epi)
@@ -286,9 +301,131 @@ class _LinearFn(torch.autograd.Function):
 
 
 def linear(x: torch.Tensor, weight: torch.Tensor) -> torch.Tensor:
+    """y = x Wᵀ; ``weight`` may be an e4m3 :class:`MXWeight` (inference only)."""
+    if isinstance(weight, MXWeight):
+        return _mx_linear(x, weight)
     if x.is_cuda:
         return _LinearFn.apply(x, weight)
     return reference.linear(x, weight)
+
+
+# --------------------------------------------------------------------------- e4m3 inference weights
+
+
+@dataclass(frozen=True, eq=False)
+class MXWeight:
+    """An inference weight W [N, K] held as e4m3: exactly what :func:`quantize_mxfp8` returns for it, the bytes ``q`` uint8 [N, K] and
+    one UE8M0 exponent per 32 values along K in ``sf`` (the 512-byte atom layout of ``reference._mxfp8_sf_index``), about 1.03 bytes
+    per weight. It stands for W̃ = ``reference.dequantize_mxfp8(q, sf)``, exact in fp32, and exact in bf16 for every block whose scale
+    is above the bf16 subnormal edge. ``dtype`` is the dtype of the weight it was made from, the one its products are computed in.
+
+    ``linear``, ``linear_qkv_rope``, ``linear_swiglu`` and ``mlp_swiglu`` take it in place of a weight tensor, forward only: a call that
+    would need its gradient raises. On CUDA (``_matmul``) M <= :func:`gemm_e4m3w_m_max` runs :func:`gemm_e4m3w`; larger M runs the bf16
+    GEMM on :func:`dequantize_weight`. On the CPU every op runs the reference on W̃ in the input's dtype."""
+
+    q: torch.Tensor
+    sf: torch.Tensor
+    dtype: torch.dtype
+
+    @property
+    def shape(self) -> torch.Size:
+        return self.q.shape
+
+    @property
+    def device(self) -> torch.device:
+        return self.q.device
+
+
+def quantize_weight(w: torch.Tensor) -> MXWeight:
+    """W [N, K] (K % 128 == 0) → :class:`MXWeight`: :func:`quantize_mxfp8` of a bf16 CUDA weight, ``reference.quantize_mxfp8`` of a CPU
+    weight of any float dtype, taken as stored."""
+    if w.dim() != 2 or w.shape[1] % 128:
+        raise ValueError(f"an e4m3 weight needs a 2-D [N, K] tensor with K % 128 == 0, got {tuple(w.shape)}")
+    w = w.detach()
+    if w.is_cuda:
+        if w.dtype != torch.bfloat16:
+            raise ValueError(f"a CUDA weight is quantised from bf16, got {w.dtype}")
+        q, sf = quantize_mxfp8(w.contiguous())
+    else:
+        q, sf = reference.quantize_mxfp8(w)
+    return MXWeight(q, sf, w.dtype)
+
+
+def dequantize_weight(w: MXWeight, out: torch.Tensor | None = None) -> torch.Tensor:
+    """W̃ of an :class:`MXWeight` in its ``dtype`` (``out``: [N, K] with unit column stride). On CUDA ``pb_dequantize_mxfp8``, bitwise
+    equal to ``reference.dequantize_mxfp8(q, sf).to(torch.bfloat16)``."""
+    N, K = w.shape
+    if not w.q.is_cuda:
+        full = reference.dequantize_mxfp8(w.q, w.sf).to(w.dtype)
+        return full if out is None else out.copy_(full)
+    if out is None:
+        out = torch.empty((N, K), dtype=torch.bfloat16, device=w.device)
+    assert out.shape == (N, K) and out.dtype == torch.bfloat16 and out.stride(1) == 1
+    _launch("pb_dequantize_mxfp8", w.q.data_ptr(), w.sf.data_ptr(), out.data_ptr(), N, K, out.stride(0), _stream())
+    return out
+
+
+_E4M3W_M_MAX: list[int] = []
+_SM_COUNT: dict = {}
+
+
+def gemm_e4m3w_m_max() -> int:
+    """The largest M :func:`gemm_e4m3w` takes (the native library's constant)."""
+    if not _E4M3W_M_MAX:
+        _E4M3W_M_MAX.append(int(_lib.load().pb_gemm_e4m3w_m_max()))
+    return _E4M3W_M_MAX[0]
+
+
+def gemm_e4m3w_splits(M: int, N: int, K: int, num_sms: int = 132) -> int:
+    """The split-K count :func:`gemm_e4m3w` uses for C[M, N] with contraction K on ``num_sms`` SMs: a function of the shape only, so a
+    captured step stays valid. Host-side only: needs the library, not a GPU."""
+    n = int(_lib.load().pb_gemm_e4m3w_splits(M, N, K, num_sms))
+    _lib.check(min(n, 0), "pb_gemm_e4m3w_splits")
+    return n
+
+
+def _num_sms(device: torch.device) -> int:
+    n = _SM_COUNT.get(device)
+    if n is None:
+        n = _SM_COUNT[device] = torch.cuda.get_device_properties(device).multi_processor_count
+    return n
+
+
+def gemm_e4m3w(x: torch.Tensor, w: MXWeight, *, out: torch.Tensor | None = None, splits: int | None = None) -> torch.Tensor:
+    """C[M, N] bf16 = x[M, K] · W̃ᵀ for 1 <= M <= :func:`gemm_e4m3w_m_max` on the native skinny kernel: each weight byte is read once,
+    dequantised exactly in registers, and multiplied on bf16 MMAs with fp32 accumulation. ``out``: [M, N] with unit column stride (a
+    strided view is fine; nothing outside its columns is written). ``splits``: the split-K count (None = :func:`gemm_e4m3w_splits`);
+    the fp32 partials go to a workspace allocated here and are summed in a fixed order, so two calls are bitwise equal."""
+    assert x.is_cuda and x.dtype == torch.bfloat16 and x.dim() == 2 and x.is_contiguous()
+    M, K = x.shape
+    N = w.shape[0]
+    assert w.shape[1] == K, f"contraction mismatch {K} vs {w.shape[1]}"
+    if out is None:
+        out = torch.empty((M, N), dtype=torch.bfloat16, device=x.device)
+    assert out.shape == (M, N) and out.dtype == torch.bfloat16 and out.stride(1) == 1
+    if splits is None:
+        splits = gemm_e4m3w_splits(M, N, K, _num_sms(x.device)) if 1 <= M <= gemm_e4m3w_m_max() else 1
+    ws = torch.empty((splits, M, N), dtype=torch.float32, device=x.device) if splits > 1 else None
+    _launch("pb_gemm_e4m3w", x.data_ptr(), w.q.data_ptr(), w.sf.data_ptr(), out.data_ptr(), _ptr(ws), M, N, K, out.stride(0) if M > 1 else N,
+            splits, _stream(), n=1 if splits == 1 else 2)  # fmt: skip
+    return out
+
+
+def _mx_no_grad(x: torch.Tensor) -> None:
+    if torch.is_grad_enabled() and x.requires_grad:
+        raise RuntimeError("e4m3 weights (ops.MXWeight) are for inference only and have no gradient: run the forward under "
+                           "torch.no_grad() or on inputs that do not require grad")  # fmt: skip
+
+
+def _mx_linear(x: torch.Tensor, w: MXWeight, rope: tuple | None = None) -> torch.Tensor:
+    """:func:`linear` (``rope``: :func:`linear_qkv_rope`) on an e4m3 weight; no autograd node, so nothing saves the weight."""
+    _mx_no_grad(x)
+    if not x.is_cuda:
+        return reference.linear(x, dequantize_weight(w).to(x.dtype))
+    x2 = _rows(x)
+    y = torch.empty((*x.shape[:-1], w.shape[0]), dtype=x.dtype, device=x.device)
+    _matmul(x2, w, y.view(-1, w.shape[0]), rope=rope)
+    return y
 
 
 # --------------------------------------------------------------------------- block-scaled fp8 (MXFP8)
@@ -398,7 +535,10 @@ def linear_qkv_rope(x: torch.Tensor, weight: torch.Tensor, cos: torch.Tensor, si
     """Fused QKV projection ⊕ RoPE: [B,S,dim] → [B,S,(H+2Hkv)·D] with the Q and K heads already rotated (GEMM epilogue).
     Must be consumed by ``rope_attention_qkv(..., pre_rotated=True)``, whose backward undoes the rotation in its own epilogues."""
     head_dim = weight.shape[0] // (n_heads + 2 * n_kv_heads)
-    return _LinearFn.apply(x, weight, (cos, sin, x.shape[1], (n_heads + n_kv_heads) * head_dim, head_dim))
+    rope = (cos, sin, x.shape[1], (n_heads + n_kv_heads) * head_dim, head_dim)
+    if isinstance(weight, MXWeight):
+        return _mx_linear(x, weight, rope)
+    return _LinearFn.apply(x, weight, rope)
 
 
 # --------------------------------------------------------------------------- embedding
@@ -684,7 +824,10 @@ class _MLPSwiGLUFn(torch.autograd.Function):
 
 def mlp_swiglu(x: torch.Tensor, w13: torch.Tensor, w2: torch.Tensor) -> torch.Tensor:
     """SwiGLU MLP ``linear(swiglu(linear(x, w13)), w2)``; on CUDA one autograd node with the SwiGLU forward AND backward fused into
-    GEMM epilogues (M > 128, hidden % 64 == 0), otherwise the composition of the separate ops."""
+    GEMM epilogues (M > 128, hidden % 64 == 0), otherwise the composition of the separate ops. With e4m3 weights (:class:`MXWeight`,
+    forward only) the composition, whose gate/up GEMM carries the SwiGLU epilogue wherever the bf16 path's does."""
+    if isinstance(w13, MXWeight) or isinstance(w2, MXWeight):
+        return linear(linear_swiglu(x, w13), w2)
     if (not _NO_EPILOGUE_FUSION and x.is_cuda and x.dtype == torch.bfloat16 and (w13.shape[0] // 2) % 64 == 0
             and x.numel() // x.shape[-1] > 128 and w2.stride(1) == 1 and w13.stride(1) == 1):  # fmt: skip
         return _MLPSwiGLUFn.apply(x, w13, w2)
@@ -693,6 +836,13 @@ def mlp_swiglu(x: torch.Tensor, w13: torch.Tensor, w2: torch.Tensor) -> torch.Te
 
 def linear_swiglu(x: torch.Tensor, w13: torch.Tensor) -> torch.Tensor:
     """``swiglu(linear(x, w13))``; fused into one GEMM on CUDA when the shape allows it (M > 128, FF % 64 == 0)."""
+    if isinstance(w13, MXWeight) and x.is_cuda and not _NO_EPILOGUE_FUSION:
+        _mx_no_grad(x)
+        x2 = _rows(x)
+        M, FF = x2.shape[0], w13.shape[0] // 2
+        h = torch.empty((*x.shape[:-1], FF), dtype=x.dtype, device=x.device)
+        _matmul(x2, w13, torch.empty((M, 2 * FF), dtype=x.dtype, device=x.device), swiglu_h=h.view(M, FF))
+        return h
     if not _NO_EPILOGUE_FUSION and x.is_cuda and x.dtype == torch.bfloat16 and (w13.shape[0] // 2) % 64 == 0 and x.numel() // x.shape[-1] > 128:
         return _LinearSwiGLUFn.apply(x, w13)
     return swiglu(linear(x, w13))

@@ -37,6 +37,15 @@ Llama-2 7B at B = 4 and 32 K context (``max_seq_len`` = 32768): the cache bytes 
 with the fp8 cache only, since the bf16 one does not fit next to the weights.
 
     python tools/decode_bench.py --kv-fp8
+
+fp8-weight section (``--weights-fp8``, alone). Kernel table: every projection shape (QKV, O, W13, W2, head) of Llama-2 1B, Llama-2
+7B and Llama-3 8B at M ∈ {1, 8, 16, 32, 64, M_MAX + 1}: ``ops.linear`` on the e4m3 weight (``pb_gemm_e4m3w`` up to M_MAX; above it
+the dequantise-then-bf16 path) next to ``ops.linear`` on the bf16 W̃, timed like the kernel section, with GB/s of the bytes each
+must read (weights at 1 + 1/32 or 2 bytes per value, plus x and C), their share of 3.35 TB/s and the split count. Steps: graph-replay
+times of a decode step and of a verify step at k = 4 (T = 5), bf16 against fp8 weights, random-init Llama-2 1B and 7B at B ∈ {1, 8},
+prompt 512. End to end: decode tokens/s (``_decode_tok_s``, 129 new tokens) and peak allocated memory for the same models.
+
+    python tools/decode_bench.py --weights-fp8
 """
 
 from __future__ import annotations
@@ -412,6 +421,89 @@ def kv_fp8_section(flush) -> dict:
     return out
 
 
+def _weight_shapes() -> list[tuple[str, str, int, int]]:
+    """(model, projection, N, K) of every projection of Llama-2 1B, Llama-2 7B and Llama-3 8B."""
+    from prime_b200.models.llama import get_model_args
+
+    out = []
+    for label, name, kind in (("llama2 1B", "1B", "llama2"), ("llama2 7B", "7B", "llama2"), ("llama3 8B", "7B", "llama3")):
+        a = get_model_args(name, kind)
+        qkv = (a.n_heads + 2 * a.kv_heads) * a.head_dim
+        out += [(label, "qkv", qkv, a.dim), (label, "o", a.dim, a.n_heads * a.head_dim), (label, "w13", 2 * a.ffn_hidden, a.dim),
+                (label, "w2", a.dim, a.ffn_hidden), (label, "head", a.vocab_size, a.dim)]  # fmt: skip
+    return out
+
+
+@torch.no_grad()
+def _weights_fp8_kernel_rows(flush) -> list[dict]:
+    rows = []
+    dev = torch.device("cuda", 0)
+    m_max = ops.gemm_e4m3w_m_max()
+    sms = torch.cuda.get_device_properties(dev).multi_processor_count
+    for label, proj, N, K in _weight_shapes():
+        mx = ops.quantize_weight((torch.randn(N, K, device=dev) * 0.02).to(torch.bfloat16))
+        wt = ops.dequantize_weight(mx)
+        for M in (1, 8, 16, 32, 64, m_max + 1):
+            x = torch.randn(M, K, device=dev, dtype=torch.bfloat16)
+            io = M * K * 2 + M * N * 2
+            r = {"model": label, "proj": proj, "M": M, "N": N, "K": K,
+                 "path": "gemm_e4m3w" if M <= m_max else "dequantize + bf16 GEMM",
+                 "splits": ops.gemm_e4m3w_splits(M, N, K, sms) if M <= m_max else None}  # fmt: skip
+            for name, w, per_value in (("fp8", mx, 1.0 + 1.0 / 32), ("bf16", wt, 2.0)):
+                ms = timed(lambda: ops.linear(x, w), flush)
+                nbytes = N * K * per_value + io
+                r[f"{name}_ms"] = round(ms, 4)
+                r[f"{name}_GB_s"] = round(nbytes / ms / 1e6, 1)
+                r[f"{name}_share"] = round(nbytes / ms / 1e-3 / HBM_BPS, 3)
+            r["fp8_speedup"] = round(r["bf16_ms"] / r["fp8_ms"], 2)
+            print(json.dumps(r), flush=True)
+            rows.append(r)
+        del mx, wt
+        torch.cuda.empty_cache()
+    return rows
+
+
+@torch.no_grad()
+def weights_fp8_section(flush) -> dict:
+    out = {"kernel": _weights_fp8_kernel_rows(flush), "steps": [], "e2e": []}
+    dev = torch.device("cuda")
+    for name in ("1B", "7B"):
+        model = build_model(name, device=dev, dtype=torch.bfloat16, seed=0).eval()
+        V = model.args.vocab_size
+        res = {}
+        for wdt in ("bf16", "fp8"):
+            if wdt == "fp8":
+                inference.quantize_weights(model)
+                torch.cuda.empty_cache()
+            for B in (1, 8):
+                prompts = torch.randint(1, V, (B, 512), generator=torch.Generator().manual_seed(B)).tolist()
+                _, c = inference.prefill(model, prompts, 2048)
+                state = [c.len, c.lo, c.last_tok]
+                tok = torch.ones(B, dtype=torch.int64, device=dev)
+                toks = torch.ones(B, 5, dtype=torch.int64, device=dev)
+                decode_ms = _replay_ms(inference.GraphDecoder(model, c, tokens=tok).replay, state)
+                verify_ms = _replay_ms(inference._capture(lambda: model.verify_step(toks, c), state), state)
+                del c
+                torch.cuda.reset_peak_memory_stats()
+                tok_s = _decode_tok_s(model, prompts, 129, "bf16")
+                res[(wdt, B)] = (decode_ms, verify_ms, tok_s, torch.cuda.max_memory_allocated() / 1e9)
+        for B in (1, 8):
+            b, f = res[("bf16", B)], res[("fp8", B)]
+            r = {"model": f"llama2 {name}", "B": B, "decode_ms_bf16": round(b[0], 3), "decode_ms_fp8": round(f[0], 3),
+                 "decode_speedup": round(b[0] / f[0], 2), "verify_k4_ms_bf16": round(b[1], 3), "verify_k4_ms_fp8": round(f[1], 3),
+                 "verify_speedup": round(b[1] / f[1], 2)}  # fmt: skip
+            e = {"model": f"llama2 {name}", "B": B, "prompt": 512, "new_tokens": 128, "tok_s_bf16": round(b[2], 1),
+                 "tok_s_fp8": round(f[2], 1), "fp8_over_bf16": round(f[2] / b[2], 3), "peak_allocated_GB_bf16": round(b[3], 2),
+                 "peak_allocated_GB_fp8": round(f[3], 2)}  # fmt: skip
+            print(json.dumps(r), flush=True)
+            print(json.dumps(e), flush=True)
+            out["steps"].append(r)
+            out["e2e"].append(e)
+        del model
+        torch.cuda.empty_cache()
+    return out
+
+
 def main() -> None:
     ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
     ap.add_argument("--out", default=None, help="also write the results as JSON here")
@@ -419,6 +511,7 @@ def main() -> None:
     ap.add_argument("--only-sampler", action="store_true", help="run only the two sampler sections")
     ap.add_argument("--speculative", action="store_true", help="run only the speculative-decoding section")
     ap.add_argument("--kv-fp8", action="store_true", help="run only the fp8 KV-cache section")
+    ap.add_argument("--weights-fp8", action="store_true", help="run only the fp8-weight section")
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("decode_bench needs a CUDA device")
@@ -426,7 +519,9 @@ def main() -> None:
     print(json.dumps({"card": info}), flush=True)
     flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")
     res = {"card": info}
-    if a.speculative or a.kv_fp8:
+    if a.speculative or a.kv_fp8 or a.weights_fp8:
+        if a.weights_fp8:
+            res["weights_fp8"] = weights_fp8_section(flush)
         if a.speculative:
             res["speculative"] = speculative_section()
         if a.kv_fp8:

@@ -24,6 +24,9 @@ run memcheck  "gpu and (kv_append or decode_advance or graph_replay or generate_
 # the e4m3 cache: append and prefill quantisers, verify attention at cap 2048, graphs and speculative rounds (the 32 K-key sweep, the
 # 8 K bound check and the 1B models are left to the plain run)
 run memcheck  "gpu and not decode_attn_fp8_matches and not analytic_bound and not 1b_shape" memcheck_kv_fp8 tests/test_kv_fp8_gpu.py
+# e4m3 weights: dequantisation, the skinny GEMM at every M, strided outputs, graphs and speculation (the projection-shape sweep, the
+# split-count sweep and the 1B models are left to the plain run)
+run memcheck  "gpu and not projection_shapes and not split_count and not 1b" memcheck_weights_fp8 tests/test_weights_fp8_gpu.py
 # flash attention against fp64: every instantiation, tile-edge documents and windows, probes (S >= 4096 is left to the plain run)
 run memcheck  "gpu and not S4096 and not S8192 and not 32768" memcheck_attention_fp64 tests/test_attention_fp64_gpu.py
 run racecheck "gpu and not S4096 and not S8192 and not 32768 and not doc_bounds" racecheck_attention_fp64 tests/test_attention_fp64_gpu.py
