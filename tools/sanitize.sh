@@ -37,10 +37,12 @@ run racecheck "gpu and not 5632" racecheck_gemm_wide tests/test_gemm_wide_gpu.py
 run memcheck  "gpu" memcheck_gemm_epilogue tests/test_gemm_epilogue_gpu.py
 run racecheck "gpu" racecheck_gemm_epilogue tests/test_gemm_epilogue_gpu.py
 run synccheck "gpu" synccheck_gemm_epilogue tests/test_gemm_epilogue_gpu.py
-# the collective GEMMs (all-gather, reduce-scatter, weight-gather) on a one-rank group against the local GEMM, bit for bit
-run memcheck  "gpu" memcheck_gemm_collective tests/test_gemm_collective_epilogue_gpu.py
-run racecheck "gpu" racecheck_gemm_collective tests/test_gemm_collective_epilogue_gpu.py
-run synccheck "gpu" synccheck_gemm_collective tests/test_gemm_collective_epilogue_gpu.py
+# the collective GEMMs (all-gather, reduce-scatter, weight-gather) with local buffers as the peers, against the local GEMM bit for
+# bit: groups of 1 and 2 at the small shapes (a gated tile traps after 4 s, which the tool's slowdown would put at risk; P >= 3, the
+# 7B MLP and the raster all-gather schedule are left to the plain run)
+run memcheck  "gpu and (P1 or P2) and not llama7b and not raster" memcheck_gemm_collective tests/test_gemm_collective_epilogue_gpu.py
+run racecheck "gpu and (P1 or P2) and not llama7b and not raster" racecheck_gemm_collective tests/test_gemm_collective_epilogue_gpu.py
+run synccheck "gpu and (P1 or P2) and not llama7b and not raster" synccheck_gemm_collective tests/test_gemm_collective_epilogue_gpu.py
 # optimizer, outer-step and peer-gather kernels with local buffers as peers, at the small shapes (block_sum / s_max shared memory;
 # pseudograd_quant's __syncthreads inside the grid-stride loop needs the 4229-block case)
 run memcheck  "gpu and not pass1 and not 4225 and not 1081352 and not 1600048 and not engine" memcheck_optimizer tests/test_optimizer_kernels_gpu.py
